@@ -3,10 +3,11 @@
 
 Workload at every N: SSD300 VGG-16 fp16 inference, per-GPU batch 64 of 300x300
 synthetic VOC-shaped images (BASELINE.json configs[1]) -- backbone + heads
-(tcgen05 convs) + anchors + decode + per-class NMS; weak scaling (images shard
+(wgmma convs) + anchors + decode + per-class NMS; weak scaling (images shard
 batch-parallel, one NCCL all-gather of the detection records per step).
 
   python bench.py --gpus N --steps K --warmup W          # this framework
+  python bench.py ... --dump-outputs DIR                 # + the last timed step's detection records as .npy
   python bench.py --impl reference --gpus N ...          # the reference's CPU path
                                                          # (oracle port: TF1.13 cannot run here)
 One JSON line on stdout (rank 0).
@@ -49,7 +50,7 @@ def bench_config(world):
     """`config` of the JSON line -- the same dict in both arms (ours and --impl reference)."""
     return {"workload": WORKLOAD, "global_batch": BATCH * world, "per_gpu_batch": BATCH,
             "parallelism": "dp%d (image shards, 1 all-gather of detections)" % world,
-            "l2": "per-step activation working set ~2 GB >> 126 MB L2 (no reuse between steps)",
+            "l2": "per-step activation working set ~2 GB >> 50 MB L2 (no reuse between steps)",
             "cuda_graph": True, "conv_gflop_per_img": CONV_GFLOP_PER_IMG,
             "pipeline": ("decode + NMS (+ all-gather) of step i run on a second stream under the first convolutions of step i+1; "
                          "candidate rows / lists / records double-buffered" if os.environ.get("ODT_PIPELINE", "1") != "0"
@@ -65,11 +66,12 @@ def measured_peaks():
     if os.path.exists(f):
         d = json.load(open(f))
         return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 / fp16 -- denominators, not reached rates
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -314,8 +316,8 @@ def conv_roofline(net, tc_ms, ms_step, peaks, peak_src, kname):
     return {"bound": "tensor", "kernel": kname, "achieved": achieved, "peak": sus, "unit": "TFLOP/s",
             "frac": achieved / sus, "frac_sustained": achieved / sus, "frac_burst": achieved / burst,
             "peak_burst": burst,
-            "peak_source": peak_src + " cuBLAS bf16: `peak`/`frac` use the sustained figure (the kernels are timed inside "
-                                      "back-to-back whole steps), frac_burst the best-of-10 burst figure",
+            "peak_source": peak_src + ": `peak`/`frac` use the sustained figure (the kernels are timed inside "
+                                      "back-to-back whole steps), frac_burst the burst figure",
             "launches_per_step": len(tc_ops), "tc_ms_per_step": tc_ms,
             "algorithmic_gflop_per_step": tc_flops / 1e9, "share_of_step": tc_ms / ms_step,
             "timing": "CUDA events around every launch of these kernels inside eager whole forwards straight after the timed "
@@ -331,6 +333,8 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-retinanet", action="store_true", help="skip the second workload (RetinaNet-800 B=16)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the detection records of the last timed step of each workload to DIR/<name>.npy")
     args = ap.parse_args()
     assert args.warmup >= 0 and args.steps >= 1
 
@@ -385,11 +389,12 @@ def main():
         if pipelined:
             net.capture_pipelined()
         counter = [0]
+        last = [net.tail]  # the Tail that holds the latest step's records
 
         def step():
             if pipelined:
-                net.run_pipelined(counter[0] & 1,
-                                  (lambda t: od.gather_records(t.rec, out=gathered)) if world > 1 else None)
+                last[0] = net.run_pipelined(counter[0] & 1,
+                                            (lambda t: od.gather_records(t.rec, out=gathered)) if world > 1 else None)
                 counter[0] += 1
                 return
             net.run()
@@ -417,7 +422,24 @@ def main():
             net.join_pipelined()  # the closing event waits for the last tails as well
         e1.record()
         barrier()
-        return max_over_ranks(e0.elapsed_time(e1))
+        ms = max_over_ranks(e0.elapsed_time(e1))
+        if args.dump_outputs and rank == 0:
+            dump_step_outputs[net] = gathered.clone() if gathered is not None else last[0].rec.clone()
+        return ms
+
+    dump_step_outputs = {}
+
+    def write_dump(name, net):
+        """Packed detection records [images, D*6 + 2] of the last timed step (float32, what detect_batch unpacks):
+        per image D detections of 6 floats, then the detection count and the overflow flag (engine.unpack_records)."""
+        if not args.dump_outputs or rank != 0:
+            return
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        rec = dump_step_outputs.pop(net).float().cpu().numpy()
+        np.save(os.path.join(args.dump_outputs, name + ".npy"), rec.astype(np.float32))
+        # the score threshold the records were filtered with (RetinaNet's is derived from this build's own rows)
+        np.save(os.path.join(args.dump_outputs, name + "_score_threshold.npy"),
+                np.array([net.tail.p.score_thr], dtype=np.float64))
 
     def time_e2e(model, images, sampler=None):
         """Public API, host buffers: pinned H2D of every step's images + D2H of every step's records inside
@@ -477,18 +499,9 @@ def main():
     e2e_value = world * BATCH * K / (ms_e2e / 1e3)
     h2d, d2h = e2e_bytes(net, images)
 
+    write_dump("ssd300_b%d_records" % BATCH, net)
     roofline = conv_roofline(net, tc_ms, ms_step, peaks, peak_src,
-                             "tcgen05 implicit-GEMM convolutions (conv_tc_kernel<1|2>, conv_tapn_kernel where planned)")
-    traffic, traffic_src = None, None
-    for cand in ("r02_conv_traffic.json", "r01_conv_traffic.json"):
-        tpath = os.path.join(ROOT, "profiles", cand)
-        if os.path.exists(tpath):  # committed ncu measurement of the same command (scripts/conv_traffic.py)
-            with open(tpath) as f:
-                tj = json.load(f)
-            if tj.get("launches_per_step") == roofline["launches_per_step"]:
-                traffic, traffic_src = tj["dram_bytes_per_launch_avg"], "profiles/%s (ncu dram__bytes_read+write)" % cand
-                break
-    roofline["traffic"], roofline["traffic_source"] = traffic, traffic_src
+                             "wgmma implicit-GEMM convolutions (conv_tc_kernel<BN>, conv_tapn_kernel where planned)")
     floor_us = tail_launch_floor_us()
     ssd_tail_rf = tail_roofline(net, dec_ms, nms_ms, peaks, floor_us)
 
@@ -535,6 +548,7 @@ def main():
         rs1.start()
         r_ms_total = time_resident(rnet, rg, rs1)
         r_clocks = rs1.stop()
+        write_dump("retinanet800_b%d_records" % RETINA_BATCH, rnet)
         r_ms_step = r_ms_total / K
         r_tc_ms, r_dec_ms, r_nms_ms = timed_ops(rnet, is_tc)
         rs2 = ClockSampler(local)
@@ -542,7 +556,7 @@ def main():
         r_e2e_ms = time_e2e(rmodel, rimg, rs2)
         r_e2e_clocks = rs2.stop()
         rh2d, rd2h = e2e_bytes(rnet, rimg)
-        rr = conv_roofline(rnet, r_tc_ms, r_ms_step, peaks, peak_src, "tcgen05 implicit-GEMM convolutions")
+        rr = conv_roofline(rnet, r_tc_ms, r_ms_step, peaks, peak_src, "wgmma implicit-GEMM convolutions")
         rr["note"] = ("tc_ms_per_step is the SERIALISED sum of the kernels' eager durations; the graph runs the FPN levels and the "
                       "two towers on parallel lanes, so share_of_step can exceed 1 and whole_step_frac_* is the figure for the step")
         line["workloads"] = {"retinanet800_b16": {

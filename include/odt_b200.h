@@ -1,5 +1,5 @@
 /*
- * odt_b200.h -- C ABI of the B200-native detection hot path.
+ * odt_b200.h -- C ABI of the H100-native (sm_90a) detection hot path.
  *
  * This is the drop-in boundary underneath the reference's Python surface
  * (SSD300.SSD300 / RetinaNet.RetinaNet / YOLOv3.YOLOv3 / FCOS.FCOS /
@@ -133,7 +133,7 @@ typedef struct {
   int out2_halo;
 } odt_conv_params;
 
-/* tcgen05 / TMA implicit-GEMM forward convolution, fp16 in, fp32 accumulate.
+/* wgmma / TMA implicit-GEMM forward convolution, fp16 in, fp32 accumulate.
  * Requires in_ld % 64 == 0, w_ld == in_ld, Cout_pad % 32 == 0.
  * ref: tf.nn.conv2d SSD300.py:519; tf.layers.conv2d SSD300.py:524,
  * RetinaNet.py:579,599,609, YOLOv3.py:495, FCOS.py:449,469,479; the fused
@@ -148,7 +148,7 @@ int odt_conv2d_direct(const void* in, const void* weights, int dtype, const odt_
 int odt_conv2d_stem(const float* images, const float* mean3_host, const void* weights, int dtype,
                     const odt_conv_params* p, void* stream);
 
-/* tcgen05 stem on the packed image of odt_pack_input_rgbx (p->in_ld = 4, p->in_halo = its pad: 1 for the
+/* Tensor-core (wgmma) stem on the packed image of odt_pack_input_rgbx (p->in_ld = 4, p->in_halo = its pad: 1 for the
  * 3x3/stride-1 stems with 64 / 32 outputs, 4 for the 7x7/stride-2 stem with 16 outputs and even W / left pad);
  * every filter row of an output pixel is one aligned span of the image, so the im2col rows are built with
  * wide loads and no arithmetic.  ODT_ERR_UNSUPPORTED for other shapes (use odt_conv2d_stem).

@@ -21,23 +21,11 @@ bool pdl_enabled() {
   }
   return v == 1;
 }
-bool bulk_enabled() {
-  const char* e = getenv("ODT_TC_BULK");
-  return !(e && e[0] == '0');
-}
 bool flat_enabled() {
   const char* e = getenv("ODT_TC_FLAT");  // read every call: lets one process compare both paths
   return !(e && e[0] == '0');
 }
-bool pair_enabled() {
-  const char* e = getenv("ODT_TC_PAIR");  // read every call: A/B inside one process
-  return !(e && e[0] == '0');
-}
-bool flat_pair_enabled() {
-  const char* e = getenv("ODT_TC_FLAT_PAIR");
-  return pair_enabled() && !(e && e[0] == '0');
-}
-// Defaults settled by the same-box A/B of round 2 (profiles/r02_ab_micro.md): all three on.
+// Defaults carried over from the previous target (all three on); not re-measured on the H100.
 bool kskip_enabled() {
   const char* e = getenv("ODT_TC_KSKIP");  // default on: all-zero K steps of thin layers are not issued (TcGeom::klast)
   return !(e && e[0] == '0');

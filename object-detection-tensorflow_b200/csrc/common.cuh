@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels behind include/odt_b200.h.
+// Shared helpers for the sm_90a kernels behind include/odt_b200.h.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -37,7 +37,7 @@ void set_error(const char* fmt, ...);
     }                                                                            \
   } while (0)
 
-constexpr int kNumSMs = 148;
+constexpr int kNumSMs = 132;  // H100 SXM
 
 template <typename T>
 struct Elem;
@@ -69,10 +69,7 @@ __device__ __forceinline__ void pdl_launch_dependents() {
 }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 bool pdl_enabled();   // ODT_PDL=0 disables the launch attribute (api.cu)
-bool bulk_enabled();  // ODT_TC_BULK=0 disables the smem-staged bulk-store epilogue
 bool flat_enabled();  // ODT_TC_FLAT=0 disables the halo-flat 3x3 path (A/B measurements)
-bool pair_enabled();  // ODT_TC_PAIR=0 disables the CTA-pair (cta_group::2) launch of large im2col-mode convs
-bool flat_pair_enabled();  // ODT_TC_FLAT_PAIR=0: no CTA pairs in the halo-flat modes
 bool kskip_enabled();  // ODT_TC_KSKIP=1: do not issue the all-zero 16-deep K steps of thin layers (Cin padded to 64)
 int thin_mode();       // ODT_TC_THIN: 1 = very thin layers (Cin, Cout <= 32, few multiply-adds per pixel) go through the
                        // CUDA-core kernel of conv_thin.cu, 2 = wherever the layer qualifies, 0 / unset = never

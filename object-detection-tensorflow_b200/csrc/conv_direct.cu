@@ -1,7 +1,7 @@
 // CUDA-core implicit-GEMM convolution: any filter / stride / dilation / channel
 // count, fp32 accumulate.  Used for (i) the reference-precision fp32 path that
 // backs the 1e-4 box parity claim, (ii) the Cin=3 stems (mean subtraction fused
-// into the operand load) and (iii) as the on-device cross-check of the tcgen05
+// into the operand load) and (iii) as the on-device cross-check of the wgmma
 // kernel.  ref: tf.nn.conv2d SSD300.py:519, tf.layers.conv2d SSD300.py:524.
 #include "epilogue.cuh"
 

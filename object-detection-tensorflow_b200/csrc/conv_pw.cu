@@ -359,9 +359,8 @@ static int pw_plan(const void* in, const odt_conv_params* p, bool force, PwGeom*
       (p->out1 && (long long)p->B * p->out1_img_stride >= lim) || (p->out2 && (long long)p->B * p->out2_img_stride >= lim))
     return ODT_ERR_UNSUPPORTED;
   // The kernel itself takes layers up to 4096 multiply-adds per pixel (beyond that the arithmetic no longer hides
-  // under the traffic).  Default planner (mode 1) = where the same-box A/B of round 2 shows a gain over conv_thin /
-  // the tensor-core path (profiles/r02_ncu_conv_pw.md): the 8-channel-input expand layers of large maps (7->28 at
-  // 200x200x16: 76 -> 64 us); every other narrow 1x1 layer is as fast or faster through the other kernels.
+  // under the traffic).  Default planner (mode 1): the 8-channel-input expand layers of large maps only (7->28 of
+  // RetinaNet); a rule carried over from the previous target, not re-measured on the H100.
   if ((long long)ci8 * 8 * passes * cot > 4096 && !force) return ODT_ERR_UNSUPPORTED;
   if (!force && !(ci8 == 1 && co8 >= 3 && M >= (1 << 18))) return ODT_ERR_UNSUPPORTED;
   PwGeom g;

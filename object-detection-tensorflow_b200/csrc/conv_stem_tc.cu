@@ -1,14 +1,15 @@
-// tcgen05 stem convolution (Cin = 3): the first layer of every backbone.
+// wgmma stem convolution (Cin = 3): the first layer of every backbone.
 //
-// K = KS*KS*3 is far below one TMA/UMMA channel chunk, so instead of im2col TMA
+// K = KS*KS*3 is far below one TMA/wgmma channel chunk, so instead of im2col TMA
 // the A operand is BUILT in shared memory: two groups of 4 producer warps (one thread per
 // output pixel of a 128-row tile, the groups take alternate tiles) gather the KS*KS*3 fp32 pixels, subtract the
 // RGB mean, convert to fp16 and store 16-byte chunks straight into the
-// 128B-swizzled K-major layout the UMMA descriptor expects (chunk c of row m at
+// 128B-swizzled K-major layout the wgmma descriptor expects (chunk c of row m at
 // ((c ^ (m & 7)) << 4)); a fence.proxy.async + mbarrier arrive hands the stage to
-// the single MMA-issuing thread.  Weights [COUT x Kpad] sit in shared memory for
-// the whole kernel.  Accumulators are double-buffered in TMEM; 4 epilogue warps
-// apply bias/BN/activation and write fp16 NHWC rows.  The layer is HBM-bound
+// the consumer warpgroup.  Weights [COUT x Kpad] sit in shared memory for the
+// whole kernel.  The consumer warpgroup multiplies the two 64-row halves of a
+// tile (accumulators in registers), hands the stage back, applies bias/BN/
+// activation to its fragments and writes fp16 NHWC rows.  The layer is HBM-bound
 // (image read + activation write); the tensor pipe is idle most of the time.
 //
 //
@@ -39,7 +40,7 @@ struct StemGeom {
 constexpr int ST_MAX_STAGES = 4;
 constexpr int ST_PROD_GROUPS = 2;                    // producer groups of 4 warps, round-robin over the CTA's tiles
 constexpr int ST_PROD_WARPS = 4 * ST_PROD_GROUPS, ST_EPI_WARPS = 4;
-constexpr int ST_THREADS = 32 * (ST_PROD_WARPS + 1 + ST_EPI_WARPS);
+constexpr int ST_THREADS = 32 * (ST_PROD_WARPS + ST_EPI_WARPS);  // producers, one consumer warpgroup
 constexpr int ST_PITCH = 144;                  // staging row pitch (bytes)
 constexpr int ST_WARP_STAGE = 32 * ST_PITCH;   // staging bytes per epilogue warp
 
@@ -61,12 +62,11 @@ __global__ void __launch_bounds__(ST_THREADS)
   constexpr int ST_STAGES = StemK<KS, H4>::STAGES;
   constexpr int KREAL = StemK<KS, H4>::KREAL;
   constexpr int KSP = StemK<KS, H4>::KSP;
-  constexpr int KSTEPS = (KREAL + 15) / 16;        // UMMA k-steps issued
+  constexpr int KSTEPS = (KREAL + 15) / 16;        // wgmma k-steps issued
   constexpr int NCHUNK = KSTEPS * 2;               // 16-byte chunks written per row
   constexpr int NBLK = (KSTEPS * 16 + 63) / 64;    // 128-byte-row blocks per stage
   constexpr int A_BYTES = NBLK * 128 * 128;
   constexpr int B_BYTES = NBLK * COUT * 128;
-  constexpr int TMEM_COLS = (2 * COUT <= 32) ? 32 : (2 * COUT <= 64 ? 64 : (2 * COUT <= 128 ? 128 : 256));
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
@@ -76,10 +76,6 @@ __global__ void __launch_bounds__(ST_THREADS)
   const uint32_t bar_base = b_base + ((B_BYTES + 1023) & ~1023);
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (ST_STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * ST_STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * ST_STAGES + 2 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * ST_STAGES + 4);
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - raw));
   float* s_scale = reinterpret_cast<float*>(smem_raw + (bar_base + 128u - raw));
   float* s_shift = s_scale + COUT;
   // per-epilogue-warp store staging: 32 rows x 128 B at a 144 B pitch (ST_PITCH), so
@@ -89,7 +85,7 @@ __global__ void __launch_bounds__(ST_THREADS)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-  // ---- one-time setup: weights -> swizzled smem, params, barriers, TMEM ----
+  // ---- one-time setup: weights -> swizzled smem, params, barriers ----
   {
     uint8_t* bsm = gbase + (b_base - base);
     // zero the K padding once, then scatter the real weights
@@ -114,25 +110,12 @@ __global__ void __launch_bounds__(ST_THREADS)
   if (threadIdx.x == 0) {
     for (int s = 0; s < ST_STAGES; ++s) {
       mbar_init(full_bar(s), 128);  // one producer group (one thread per tile row)
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), ST_EPI_WARPS);
+      mbar_init(empty_bar(s), ST_EPI_WARPS);  // one arrival per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == ST_PROD_WARPS) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot),
-                 "n"(TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   fence_proxy_async_smem();  // weight tile written through the generic proxy
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
   pdl_launch_dependents();
   pdl_wait();
 
@@ -309,93 +292,69 @@ __global__ void __launch_bounds__(ST_THREADS)
       fence_proxy_async_smem();
       mbar_arrive(full_bar(stage));
     }
-  } else if (warp == ST_PROD_WARPS) {
-    // ===================== MMA issuer ==========================================
-    // warp-uniform loop, one elected lane issues (see conv_tc.cu)
-    const uint32_t idesc = make_idesc_f16(128, COUT);
-    int stage = 0, acc = 0;
-    uint32_t phase = 0, acc_phase0 = 0u, acc_phase1 = 0u;
+  } else {
+    // ===================== consumer warpgroup: MMA + epilogue ==================
+    // Warp w holds rows 16w .. 16w+15 of each 64-row half (wgmma fragment layout, tc_ptx.cuh).
+    const int w = warp - ST_PROD_WARPS;
+    int stage = 0;
+    uint32_t phase = 0;
+    // Stage the warp's 32 rows x COUT fp16 in shared memory (144-byte pitch: the fragment writes
+    // of one instruction hit 32 distinct banks), then store them with the lanes transposed:
+    // CPR consecutive lanes cover one row's COUT*2 bytes, so every STG.128 of the warp
+    // writes whole 32-byte sectors of 32/CPR rows -- in the dense and in the halo layout.
+    // Staging row h*16 + i holds tile row 64h + 16w + i.
+    uint8_t* warp_stage = smem_raw + (stage_out - raw) + (uint32_t)w * ST_WARP_STAGE;
     for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
-      mbar_wait(tempty_bar(acc), (acc ? acc_phase1 : acc_phase0) ^ 1u);
+      float acc[2][COUT / 2];
       mbar_wait(full_bar(stage), phase);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + (uint32_t)acc * COUT;
-      if (elect_one()) {
+      wg_fence();
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
 #pragma unroll
         for (int k = 0; k < KSTEPS; ++k) {
           const uint32_t blk = k >> 2, kin = k & 3;
           const uint64_t adesc =
-              make_desc_sw128(a_base + (uint32_t)stage * A_BYTES + blk * (128 * 128)) + (uint64_t)(2 * kin);
+              make_desc_sw128(a_base + (uint32_t)stage * A_BYTES + blk * (128 * 128) + (uint32_t)h * (64 * 128)) +
+              (uint64_t)(2 * kin);
           const uint64_t bdesc = make_desc_sw128(b_base + blk * (COUT * 128)) + (uint64_t)(2 * kin);
-          tc_mma_f16(d_tmem, adesc, bdesc, idesc, (uint32_t)(k != 0));
+          wg_mma_f16<COUT>(acc[h], adesc, bdesc, (uint32_t)(k != 0));
         }
-        tc_commit(empty_bar(stage));
-        tc_commit(tfull_bar(acc));
       }
+      wg_commit();
+      wg_wait<0>();
+      // the stage has been read: hand it back before the epilogue
       __syncwarp();
-      if (acc) acc_phase1 ^= 1u; else acc_phase0 ^= 1u;
-      acc ^= 1;
+      if (lane == 0) mbar_arrive(empty_bar(stage));
       if (++stage == ST_STAGES) {
         stage = 0;
         phase ^= 1u;
       }
-    }
-  } else {
-    // ===================== epilogue ============================================
-    const int quarter = warp & 3;
-    int acc = 0;
-    uint32_t acc_phase[2] = {0u, 0u};
-    for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
-      const long long m = (long long)tile * 128 + quarter * 32 + lane;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        uint8_t* r0 = warp_stage + (h * 16 + (lane >> 2)) * ST_PITCH;
+#pragma unroll
+        for (int i = 0; i < COUT / 8; ++i) {
+          const int c0 = 8 * i + 2 * (lane & 3);
+          const float sc0 = s_scale[c0], sc1 = s_scale[c0 + 1], sh0 = s_shift[c0], sh1 = s_shift[c0 + 1];
+          *reinterpret_cast<__half2*>(r0 + c0 * 2) =
+              __floats2half2_rn(apply_act(fmaf(acc[h][4 * i], sc0, sh0), e.act),
+                                apply_act(fmaf(acc[h][4 * i + 1], sc1, sh1), e.act));
+          *reinterpret_cast<__half2*>(r0 + 8 * ST_PITCH + c0 * 2) =
+              __floats2half2_rn(apply_act(fmaf(acc[h][4 * i + 2], sc0, sh0), e.act),
+                                apply_act(fmaf(acc[h][4 * i + 3], sc1, sh1), e.act));
+        }
+      }
+      __syncwarp();
+      const long long m = (long long)tile * 128 + (lane < 16 ? 16 * w + lane : 64 + 16 * w + lane - 16);
       const bool row_ok = m < g.M;
       const int b = row_ok ? (int)(m / g.ohw) : 0;
       const int pix = row_ok ? (int)(m - (long long)b * g.ohw) : 0;
-      mbar_wait(tfull_bar(acc), acc_phase[acc]);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (uint32_t)acc * COUT + ((uint32_t)(quarter * 32) << 16);
       long long opix = pix;
       if (g.out_halo) {
         const int oy = pix / g.OW, ox = pix - oy * g.OW;
         opix = (long long)(oy + 1) * (g.OW + 2) + ox + 1;
       }
-      // Stage the warp's 32 rows x COUT fp16 in shared memory (one row per lane, 144-byte
-      // pitch: conflict-free 16-byte writes), then store them with the lanes transposed:
-      // CPR consecutive lanes cover one row's COUT*2 bytes, so every STG.128 of the warp
-      // writes whole 32-byte sectors of 32/CPR rows -- in the dense and in the halo layout.
-      uint8_t* warp_stage = smem_raw + (stage_out - raw) + (uint32_t)(warp - ST_PROD_WARPS - 1) * ST_WARP_STAGE;
-      uint8_t* my_stage_ptr = warp_stage + lane * ST_PITCH;
       const long long my_off = row_ok ? (long long)b * e.out0_img_stride + opix * e.out0_pix_stride : -1;
-#pragma unroll
-      for (int j = 0; j < COUT / 16; ++j) {
-        uint32_t r[16];
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-            : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-              "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]),
-              "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-            : "r"(taddr + (uint32_t)(j * 16))
-            : "memory");
-        tc_wait_ld();
-        uint4 pk[2];
-        __half2* h = reinterpret_cast<__half2*>(pk);
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const int c0 = j * 16 + 2 * q;
-          const float v0 = apply_act(fmaf(__uint_as_float(r[2 * q]), s_scale[c0], s_shift[c0]), e.act);
-          const float v1 =
-              apply_act(fmaf(__uint_as_float(r[2 * q + 1]), s_scale[c0 + 1], s_shift[c0 + 1]), e.act);
-          h[q] = __floats2half2_rn(v0, v1);
-        }
-        *reinterpret_cast<uint4*>(my_stage_ptr + ((2 * j) << 4)) = pk[0];
-        *reinterpret_cast<uint4*>(my_stage_ptr + ((2 * j + 1) << 4)) = pk[1];
-      }
-      // the accumulator stage is drained: hand it back before the store phase
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));
-      acc_phase[acc] ^= 1u;
-      acc ^= 1;
       constexpr int CPR = COUT / 8;    // 16-byte chunks per row (the pad channels stay zero in HBM)
       constexpr int RPI = 32 / CPR;    // rows per store instruction
       const int sub_row = lane / CPR, chunk = lane % CPR;
@@ -408,14 +367,6 @@ __global__ void __launch_bounds__(ST_THREADS)
       }
       __syncwarp();  // staging rows are rewritten by the next tile
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == ST_PROD_WARPS) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS)
-                 : "memory");
   }
 }
 
@@ -431,7 +382,13 @@ static int launch_stem_tc(const void* img, const void* w, const StemGeom& g, con
     ODT_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr = true;
   }
-  const int per_sm = smem > 110000 ? 1 : 2;
+  // as many CTAs per SM as registers and shared memory allow (the 384-thread variants take one or two)
+  int per_sm = 0;
+  ODT_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, ST_THREADS, smem));
+  if (per_sm < 1) {
+    set_error("launch_stem_tc: the kernel does not fit on an SM (%d bytes of shared memory)", smem);
+    return ODT_ERR_CUDA;
+  }
   int grid = kNumSMs * per_sm;
   if (grid > g.num_tiles) grid = g.num_tiles;
   kern<<<grid, ST_THREADS, smem, st>>>(img, (const __half*)w, g, e);

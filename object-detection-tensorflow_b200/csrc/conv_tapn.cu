@@ -1,30 +1,25 @@
 // "Taps as N": the 3x3 / stride-1 halo convolution for NARROW outputs (Cout_pad <= 64) with the three
-// horizontal filter taps folded into the N dimension of the MMA.
-//
-// Why: a tcgen05.mma M128 x N x K16 fetches its operands from shared memory at ~64 B/clk, i.e.
-// 2*(32 + N/4) clk, while the tensor pipe itself needs N/2 clk (conv_tc.cu, DESIGN.md 3.1).  At N = 64 the
-// fetch (96 clk) is 3x the math (32 clk): conv1_2 of VGG and every thin RetinaNet layer sit on that floor
-// (36 MMAs x 96 clk per 128-pixel tile).  Each activation row that is fetched should therefore feed more
-// output columns.  Here one MMA multiplies the activation tile of filter row r by the weights of ALL THREE
-// horizontal taps:
+// horizontal filter taps folded into the N dimension of the MMA.  One MMA multiplies the activation tile of
+// filter row r by the weights of ALL THREE horizontal taps:
 //
 //   P[q, s*BN + n] = sum_{r, c} X[q + r*PW, c] * W[n, r, s, c]          (N = 3*BN, K = 3*Cin)
 //   out[p, n]      = P[p-1, 0*BN + n] + P[p, 1*BN + n] + P[p+1, 2*BN + n]
 //
-// so a tile costs 3*cchunks*4 MMAs of N = 192 (160 clk each) instead of 9*cchunks*4 of N = 64 (96 clk):
-// 1920 instead of 3456 clk at Cin = Cout = 64.  The shifted sum runs in the epilogue: a tile is 4 image rows
-// x 32 columns with the COLUMN index in the lane (one warp = one row), P[p-1] / P[p+1] come from the
-// neighbouring lanes (shfl), lanes 0 and 31 only serve as neighbours, tiles overlap by two columns (30 outputs
-// per row and tile).  The fused 2x2/2 max-pool pairs columns inside the warp and rows through a small
-// shared-memory exchange between the warps of an epilogue group.
+// so a tile takes 3*cchunks*4 MMAs of N = 3*BN instead of 9*cchunks*4 of N = BN: each activation row that is
+// fetched feeds three times as many output columns.  A tile is 4 image rows x 32 columns (shared-memory row
+// = 32*row + column); columns 0 and 31 only serve as neighbours, tiles overlap by two columns (30 outputs per
+// row and tile).  The shifted sum runs on the fp32 accumulator tile in shared memory; in the epilogue each
+// lane owns one column of one row.  The fused 2x2/2 max-pool pairs columns inside the warp and rows through
+// a small shared-memory exchange between the warps of an epilogue group.
 //
 // Roles / pipeline as in conv_tc.cu: w0 TMA producer (one [64 ch][32 x][4 rows] box per filter row and
-// channel chunk), w1 MMA issuer, w2..9 two epilogue groups draining alternate tiles from two TMEM stages;
-// the 9*cchunks weight tiles stay resident in shared memory.
+// channel chunk), w4..11 two consumer warpgroups (wgmma over the two 64-row halves of the tile, then the
+// epilogue: group g takes the 32-channel chunks j = g, g + 2, ...); the 9*cchunks weight tiles stay resident
+// in shared memory.
 //
-// OPT-IN (ODT_TC_TAPN=1) until it has been A/B-timed on a B200: written at the end of round 1; its eight parity
-// cases (tests/test_gpu_conv.py::test_conv_tapn_matches_reference) passed on a B200 with the last GPU seconds of
-// the round, no timing yet.  ref call sites: tf.nn.conv2d SSD300.py:519 (conv1_2), tf.layers.conv2d
+// On sm_90 a 128 x N x 16 MMA costs about N clocks whatever the operand layout, so folding the taps into N
+// saves no MMA time; the planner (ODT_TC_TAPN=1) takes the layer only where its tiles waste fewer positions
+// than the regular halo-flat tiles.  ref call sites: tf.nn.conv2d SSD300.py:519 (conv1_2), tf.layers.conv2d
 // RetinaNet.py:599-609, YOLOv3.py:495, FCOS.py:469-479.
 #include <string.h>
 
@@ -33,12 +28,11 @@
 
 namespace odt {
 
-constexpr int TN_THREADS = 320;      // TMA, MMA, 2 x 4 epilogue warps
+constexpr int TN_THREADS = 384;      // producer warpgroup (one active warp), two consumer warpgroups
 constexpr int TN_XV = 30;            // output columns per tile row (32 lanes - 2 neighbour lanes)
-constexpr int TN_ROWS = 4;           // image rows per tile (one per TMEM lane quarter)
+constexpr int TN_ROWS = 4;           // image rows per tile (one per epilogue warp of a group)
 constexpr int TN_A_BYTES = 128 * 128;
 constexpr int TN_MAX_STAGES = 8;
-constexpr int TN_ACC_STRIDE = 256;   // TMEM columns between the two accumulator stages (3*BN <= 192 used)
 constexpr int TN_PAR_FLOATS = 6 * 64;
 constexpr int TN_XCH_PITCH = 80;     // bytes per lane in the pooling exchange (64 payload, padded against bank conflicts)
 constexpr int TN_XCH_BYTES = 2 * 2 * 2 * 32 * TN_XCH_PITCH;  // [group][buffer][row pair][lane]
@@ -53,7 +47,9 @@ struct TnGeom {
   int out_halo;
 };
 
-template <int POOL>
+constexpr int tn_sum_bytes(int bn) { return 128 * (bn + 4) * 4; }  // fp32 tile of the shifted sum
+
+template <int BN, int POOL>
 __global__ void __launch_bounds__(TN_THREADS, 1)
     conv_tapn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                      const __grid_constant__ TnGeom g, const __grid_constant__ Epi e) {
@@ -63,42 +59,33 @@ __global__ void __launch_bounds__(TN_THREADS, 1)
   const int stages = g.stages;
   const uint32_t a_base = base;
   const uint32_t b_base = base + (uint32_t)stages * TN_A_BYTES;
-  const uint32_t wtile = 3u * (uint32_t)g.BN * 128u;  // weights of one (filter row, chunk): rows s*BN + n
+  const uint32_t wtile = 3u * (uint32_t)BN * 128u;  // weights of one (filter row, chunk): rows s*BN + n
   const uint32_t wbytes = 3u * (uint32_t)g.cchunks * wtile;
   const uint32_t bar_base = b_base + wbytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (TN_MAX_STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * TN_MAX_STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * TN_MAX_STAGES + 2 + a); };
-  const uint32_t wfull_bar = bar_base + 8u * (2 * TN_MAX_STAGES + 4);
-  const uint32_t tmem_slot = bar_base + 8u * (2 * TN_MAX_STAGES + 5);
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - raw));
+  const uint32_t wfull_bar = bar_base + 8u * (2 * TN_MAX_STAGES);
   float* par = reinterpret_cast<float*>(smem_raw + (bar_base + 256u - raw));  // [scale|shift|scale2|shift2|scale3|shift3][64]
   uint8_t* xch = smem_raw + (bar_base + 256u + TN_PAR_FLOATS * 4u - raw);
+  // out[p] = P_centre[p] + P_left[p-1] + P_right[p+1] accumulated in place, BN + 4 floats per row
+  constexpr int SUM_PITCH = BN + 4;
+  float* sum = reinterpret_cast<float*>(xch + (POOL ? TN_XCH_BYTES : 0));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
     for (int s = 0; s < stages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), 4);  // the four warps of the group that owns the stage
+      mbar_init(empty_bar(s), 8);  // one arrival per consumer warp
     }
     mbar_init(wfull_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(tmem_slot) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  if (warp >= 2) {
+  if (warp >= 4) {
     // per-channel epilogue parameters (constant data): one copy per CTA
-    for (int i = threadIdx.x - 64; i < TN_PAR_FLOATS; i += 256) {
+    for (int i = threadIdx.x - 128; i < TN_PAR_FLOATS; i += 256) {
       const int which = i >> 6, c = i & 63;
       const bool ok = c < e.Cout;
       const float* src = which == 0 ? e.scale : which == 1 ? e.shift : which == 2 ? e.scale2 : which == 3 ? e.shift2
@@ -106,10 +93,7 @@ __global__ void __launch_bounds__(TN_THREADS, 1)
       par[i] = (ok && src) ? __ldg(src + c) : ((which & 1) ? 0.f : 1.f);
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
   if (warp == 0) {
     // the filter bank is constant data: fetch it before waiting on the previous kernel
@@ -118,7 +102,7 @@ __global__ void __launch_bounds__(TN_THREADS, 1)
       for (int r = 0; r < 3; ++r)
         for (int cc = 0; cc < g.cchunks; ++cc)
           for (int s = 0; s < 3; ++s)
-            tma_load_2d(b_base + (uint32_t)(r * g.cchunks + cc) * wtile + (uint32_t)s * (uint32_t)g.BN * 128u, &tmB,
+            tma_load_2d(b_base + (uint32_t)(r * g.cchunks + cc) * wtile + (uint32_t)s * (uint32_t)BN * 128u, &tmB,
                         wfull_bar, ((r * 3 + s) * g.cchunks + cc) * 64, 0);
     }
     __syncwarp();
@@ -154,54 +138,74 @@ __global__ void __launch_bounds__(TN_THREADS, 1)
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =========================================
-    const uint32_t idesc = make_idesc_f16(128, 3 * g.BN);
+  } else if (warp >= 4) {
+    // ===================== consumer warpgroups ===============================
+    const int quarter = warp & 3;          // epilogue: image row inside the tile
+    const int group = (warp - 4) >> 2;     // MMA: rows 64*group .. +63 of the tile; epilogue: chunks group, group + 2
+    const int chunks = BN >> 5;            // 32-channel chunks per tile
+    int xbuf = 0;
     int stage = 0;
     uint32_t phase = 0;
-    int local_tile = 0;
+    float acc[3 * BN / 2];
     mbar_wait(wfull_bar, 0);
-    tc_fence_after();
-    for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x, ++local_tile) {
-      const int acc = local_tile & 1;
-      const uint32_t use = (uint32_t)(local_tile >> 1);
-      mbar_wait(tempty_bar(acc), (use & 1u) ^ 1u);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + (uint32_t)(acc * TN_ACC_STRIDE);
+    for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
+      int prev = -1;
       for (int r = 0; r < 3; ++r) {
         for (int cc = 0; cc < g.cchunks; ++cc) {
           mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          const uint64_t adesc = make_desc_sw128(a_base + (uint32_t)stage * TN_A_BYTES);
+          const uint64_t adesc = make_desc_sw128(a_base + (uint32_t)stage * TN_A_BYTES + (uint32_t)group * 64u * 128u);
           const uint64_t bdesc = make_desc_sw128(b_base + (uint32_t)(r * g.cchunks + cc) * wtile);
-          const int ksteps = (cc == g.cchunks - 1) ? g.klast : 4;  // all-zero K steps of a thin layer are not issued
-          const bool last = r == 2 && cc == g.cchunks - 1;
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              tc_mma_f16(d_tmem, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc,
-                         (uint32_t)((r | cc | k) != 0), (uint32_t)(k < ksteps));
-            tc_commit(empty_bar(stage));
-            if (last) tc_commit(tfull_bar(acc));
-          }
-          __syncwarp();
+          // all-zero K steps of a thin layer are not issued
+          const int ksteps = __shfl_sync(0xffffffffu, (cc == g.cchunks - 1) ? g.klast : 4, 0);
+          wg_fence();
+          wg_mma_chunk<3 * BN>(acc, adesc, bdesc, ksteps, (r | cc) == 0);
+          wg_commit();
+          wg_wait<1>();  // the previous stage's MMAs have retired
+          if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
+          prev = stage;
           if (++stage == stages) {
             stage = 0;
             phase ^= 1u;
           }
         }
       }
-    }
-  } else {
-    // ===================== epilogue warps =====================================
-    const int quarter = warp & 3;          // TMEM lane quarter = image row inside the tile
-    const int group = (warp - 2) >> 2;     // owns accumulator stage `group`
-    const int chunks = g.BN >> 5;          // 32-channel chunks per tile
-    int xbuf = 0;
-    int local_tile = 0;
-    for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x, ++local_tile) {
-      if ((local_tile & 1) != group) continue;
-      const uint32_t use = (uint32_t)(local_tile >> 1);
+      wg_wait<0>();
+      if (lane == 0) mbar_arrive(empty_bar(prev));
+      // shifted sum in shared memory: out[p] = (P_centre[p] + P_left[p-1]) + P_right[p+1]; row 32*y + 31 feeds
+      // row 32*(y+1), column 0, which only serves as a neighbour
+      asm volatile("bar.sync 3, 256;" ::: "memory");  // the previous tile's epilogue has read the sum
+      {
+        const int w = warp & 3;
+        const int row0 = 64 * group + 16 * w + (lane >> 2);
+#pragma unroll
+        for (int pass = 0; pass < 3; ++pass) {
+          const int s3 = pass == 0 ? 1 : (pass == 1 ? 0 : 2);  // centre, left, right
+          const int dr = s3 - 1;  // centre writes row p, left adds into p + 1, right into p - 1
+          if (pass) asm volatile("bar.sync 3, 256;" ::: "memory");
+#pragma unroll
+          for (int i = 0; i < BN / 8; ++i) {
+            const int c = 8 * i + 2 * (lane & 3);
+            const int f = (s3 * BN + 8 * i) / 8 * 4;  // fragment register of column s3*BN + 8i
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+              const int row = row0 + 8 * hh - dr;
+              if (row < 0 || row >= 128) continue;
+              float2* dst = reinterpret_cast<float2*>(sum + row * SUM_PITCH + c);
+              const float2 v = make_float2(acc[f + 2 * hh], acc[f + 2 * hh + 1]);
+              if (s3 == 1) {
+                *dst = v;
+              } else {
+                float2 o = *dst;
+                o.x += v.x;
+                o.y += v.y;
+                *dst = o;
+              }
+            }
+          }
+        }
+      }
+      asm volatile("bar.sync 3, 256;" ::: "memory");
+
       const int img = tile / per_img;
       const int rem = tile - img * per_img;
       const int yq = rem / g.xblocks, xq = rem - yq * g.xblocks;
@@ -221,30 +225,20 @@ __global__ void __launch_bounds__(TN_THREADS, 1)
         o1_row = aux_row(e.out1_img_stride, e.out1_pix_stride, e.out1_halo, g.W, img, pix);
         o2_row = aux_row(e.out2_img_stride, e.out2_pix_stride, e.out2_halo, g.W, img, pix);
       }
-      mbar_wait(tfull_bar(group), use & 1u);
-      tc_fence_after();
-      const uint32_t taddr0 = tmem_base + (uint32_t)(group * TN_ACC_STRIDE) + ((uint32_t)(quarter * 32) << 16);
-      for (int j = 0; j < chunks; ++j) {
+      const float* my_sum = sum + (quarter * 32 + lane) * SUM_PITCH;
+      for (int j = group; j < chunks; j += 2) {
         const int nb = j * 32;
-        uint32_t r0[32], r1[32], r2[32];
-        tc_ld32(taddr0 + (uint32_t)(0 * g.BN + nb), r0);
-        tc_ld32(taddr0 + (uint32_t)(1 * g.BN + nb), r1);
-        tc_ld32(taddr0 + (uint32_t)(2 * g.BN + nb), r2);
-        tc_wait_ld();
-        if (j == chunks - 1) {
-          // every TMEM read of this tile has completed: hand the stage back before the math
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(tempty_bar(group));
-        }
-        // out[p] = P_left[p-1] + P_centre[p] + P_right[p+1]  (lanes 0 / 31 produce unused values)
         const float4* ps = reinterpret_cast<const float4*>(par + nb);
         const float4* ph4 = reinterpret_cast<const float4*>(par + 64 + nb);
         float v[32];
 #pragma unroll
-        for (int i = 0; i < 32; ++i)
-          v[i] = __uint_as_float(r1[i]) + __uint_as_float(__shfl_up_sync(0xffffffffu, r0[i], 1)) +
-                 __uint_as_float(__shfl_down_sync(0xffffffffu, r2[i], 1));
+        for (int i = 0; i < 8; ++i) {
+          const float4 t = *reinterpret_cast<const float4*>(my_sum + nb + 4 * i);
+          v[4 * i + 0] = t.x;
+          v[4 * i + 1] = t.y;
+          v[4 * i + 2] = t.z;
+          v[4 * i + 3] = t.w;
+        }
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
           const float4 sc = ps[i], sh = ph4[i];
@@ -357,14 +351,6 @@ __global__ void __launch_bounds__(TN_THREADS, 1)
       }
     }
   }
-
-  // ---- teardown ----
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
-  }
 }
 
 static int g_tapn_launches = 0;  // debug: lets a test assert that the layer really took this path
@@ -409,35 +395,32 @@ int conv_tapn_try(const void* in, const void* weights, const odt_conv_params* p,
   g.num_tiles = (int)tiles;
   g.out_halo = p->out0_halo;
   if (tapn_mode() == 1) {
-    // same operand-fetch model as pick_tiling (conv_tc.cu): rounds of the slowest SM x MMAs per tile x clk per MMA
-    // (2*(32 + N/4), A and half of B with the CTA pairs the regular flat modes use), + a fixed cost per tile.
+    // rounds of the slowest SM x MMA clocks per tile + a fixed cost per tile; a 128 x N x 16 MMA takes ~N clk
+    // (2048 fp16 FMA/clk/SM), so both paths spend 9*cchunks*4*BN clk per tile and only the tile counts differ.
     // Small maps lose here: a 13-wide row still occupies a 32-lane tile row.
     const long long mm = 4ll * g.cchunks;
-    const long long c_tapn = (long long)ceil_div(tiles, kNumSMs) * (3 * mm * (64 + 3 * g.BN / 2) + 1200);
+    const long long c_tapn = (long long)ceil_div(tiles, kNumSMs) * (9 * mm * g.BN + 1200);
     long long t_reg;  // tiles of the regular path
-    bool pairs;
     if (pool) {
       const long long t2 = (long long)((p->H + 1) / 2) * ((p->W + 63) / 64), t4 = (long long)((p->H + 3) / 4) * ((p->W + 31) / 32);
       t_reg = (long long)p->B * (t4 < t2 ? t4 : t2);
-      pairs = true;
     } else {
       t_reg = ((long long)p->B * (p->H + 2) * (p->W + 2) + 127) / 128;
-      pairs = g.cchunks >= 2;
     }
-    const long long c_reg = (long long)ceil_div(t_reg, kNumSMs) * (9 * mm * (64 + (pairs ? g.BN / 4 : g.BN / 2)) + 1200);
+    const long long c_reg = (long long)ceil_div(t_reg, kNumSMs) * (9 * mm * g.BN + 1200);
     if (c_tapn >= c_reg) return ODT_ERR_UNSUPPORTED;
   }
   const int wbytes = 9 * g.cchunks * g.BN * 128;
-  const int fixed = wbytes + 256 + TN_PAR_FLOATS * 4 + (pool ? TN_XCH_BYTES : 0) + 1024;
+  const int fixed = wbytes + 256 + TN_PAR_FLOATS * 4 + (pool ? TN_XCH_BYTES : 0) + tn_sum_bytes(g.BN) + 1024;
   int stages = (TN_SMEM_LIMIT - fixed) / TN_A_BYTES;
   if (stages > TN_MAX_STAGES) stages = TN_MAX_STAGES;
-  if (stages < 3) return ODT_ERR_UNSUPPORTED;
+  if (stages < 2) return ODT_ERR_UNSUPPORTED;
   g.stages = stages;
 
   CUtensorMap tmA, tmB;
   {
     // [ld][W+2][H+2][B] view of the halo tensor; one {64, 32, 4, 1} box = the tile's rows of one filter row,
-    // column index fastest (shared-memory row = 32*row + column = TMEM lane)
+    // column index fastest (shared-memory row = 32*row + column)
     const cuuint64_t PH = (cuuint64_t)p->H + 2, PW = (cuuint64_t)p->W + 2;
     cuuint64_t dims[4] = {(cuuint64_t)p->in_ld, PW, PH, (cuuint64_t)p->B};
     cuuint64_t strides[3] = {(cuuint64_t)p->in_ld * 2, PW * p->in_ld * 2, PH * PW * p->in_ld * 2};
@@ -455,8 +438,10 @@ int conv_tapn_try(const void* in, const void* weights, const odt_conv_params* p,
   }
   static bool attr_set = false;
   if (!attr_set) {
-    ODT_CUDA_OK(cudaFuncSetAttribute(conv_tapn_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TN_SMEM_LIMIT));
-    ODT_CUDA_OK(cudaFuncSetAttribute(conv_tapn_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TN_SMEM_LIMIT));
+    ODT_CUDA_OK(cudaFuncSetAttribute(conv_tapn_kernel<32, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TN_SMEM_LIMIT));
+    ODT_CUDA_OK(cudaFuncSetAttribute(conv_tapn_kernel<32, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TN_SMEM_LIMIT));
+    ODT_CUDA_OK(cudaFuncSetAttribute(conv_tapn_kernel<64, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, TN_SMEM_LIMIT));
+    ODT_CUDA_OK(cudaFuncSetAttribute(conv_tapn_kernel<64, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TN_SMEM_LIMIT));
     attr_set = true;
   }
   Epi e = make_epi(*p);
@@ -470,10 +455,10 @@ int conv_tapn_try(const void* in, const void* weights, const odt_conv_params* p,
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  if (pool)
-    ODT_CUDA_OK(cudaLaunchKernelEx(&cfg, conv_tapn_kernel<1>, tmA, tmB, g, e));
-  else
-    ODT_CUDA_OK(cudaLaunchKernelEx(&cfg, conv_tapn_kernel<0>, tmA, tmB, g, e));
+  void (*kern)(CUtensorMap, CUtensorMap, TnGeom, Epi) =
+      g.BN == 32 ? (pool ? conv_tapn_kernel<32, 1> : conv_tapn_kernel<32, 0>)
+                 : (pool ? conv_tapn_kernel<64, 1> : conv_tapn_kernel<64, 0>);
+  ODT_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, g, e));
   ODT_LAUNCH_OK();
   ++g_tapn_launches;
   return ODT_OK;

@@ -1,7 +1,7 @@
-// tcgen05 / TMA implicit-GEMM forward convolution for sm_100a.
+// wgmma / TMA implicit-GEMM forward convolution for sm_90a.
 //
 //   D[m, n] = sum_{r,s,c} X[b, p*stride - pad + r*dil, q*stride - pad + s*dil, c] * W[n, r, s, c]
-//   m = (b, p, q) linearised over B*OH*OW, fp16 operands, fp32 accumulation in TMEM.
+//   m = (b, p, q) linearised over B*OH*OW, fp16 operands, fp32 accumulation in registers.
 //
 // * A operand (activations, NHWC), three feeding modes:
 //   - im2col-mode TMA: one load per (filter tap, 64-channel chunk) brings a [128 pixels x 64
@@ -9,18 +9,21 @@
 //     images, zero-filled where the tap falls into the SAME padding (any filter geometry);
 //   - halo-flat (3x3 / stride 1 / N <= 128, input stored with a zero halo): one [136 x 64] slab of
 //     consecutive padded positions per (filter row, chunk) feeds the three horizontal taps
-//     through row-shifted UMMA descriptors;
+//     through row-shifted wgmma descriptors;
 //   - row-block (the same shapes + fused 2x2/2 max-pool): RP rows x 128/RP columns per tile, a 4-D
 //     tiled box with the row dimension second, the pooling window in four lanes of one warp.
-// * B operand (weights, KRSC = K-major): tiled TMA loads [BN x 64] (half of it per CTA in a pair),
-//   optionally resident in shared memory for small filter banks.
-// * MMA: tcgen05.mma kind::f16, K=16, issued by one elected lane; M=128, N=BN<=256 per CTA
-//   (cta_group::1) or M=256 across the two SMs of a TPC (cta_group::2, conv_tc_kernel<2>);
-//   accumulators in TMEM (2 x 256 or 4 x <=128 columns) so epilogues overlap the next tiles' MMAs.
-// * Epilogue: tcgen05.ld -> folded bias/BN scale+shift, activation, residual, up to two extra
-//   pre-activated outputs, fused max-pool, fp32 head scatter; 128-bit / bulk global stores.
-// * Persistent: one CTA (or CTA pair) per SM, static round-robin tile schedule, warp roles:
-//   w0 = TMA producer, w1 = TMEM allocator + MMA issuer, w2..9 = epilogue (2 warps per TMEM lane quarter).
+// * B operand (weights, KRSC = K-major): tiled TMA loads [BN x 64], optionally resident in shared
+//   memory for small filter banks.
+// * MMA: wgmma m64nBNk16 (BN <= 128), both operands from shared memory; two consumer warpgroups,
+//   one per 64-row half of the 128-row tile.  A pipeline stage goes back to the producer as soon
+//   as the MMAs that read it have retired (one wgmma group kept in flight).
+// * Epilogue: the accumulators pass through an fp32 tile in shared memory so that every epilogue
+//   lane owns one pixel row, 32 channels at a time: folded bias/BN scale+shift, activation,
+//   residual, up to two extra pre-activated outputs, fused max-pool, fp32 head scatter; 128-bit
+//   global stores.
+// * Persistent: one CTA per SM, static round-robin tile schedule.  Warp 0 = TMA producer (runs
+//   ahead across tiles), warps 4..11 = the two consumer warpgroups (MMA, then the epilogue of the
+//   same tile; warps 1..3 only pad the producer warpgroup).
 //
 // ref call sites: tf.nn.conv2d SSD300.py:519; tf.layers.conv2d SSD300.py:524,
 // RetinaNet.py:579,599,609, YOLOv3.py:495, FCOS.py:449,469,479.
@@ -34,14 +37,15 @@ namespace odt {
 
 constexpr int TC_BM = 128;
 constexpr int TC_BK = 64;
+constexpr int TC_MAX_BN = 128;  // N tile (the wgmma accumulators of one 64-row half live in registers)
 constexpr int TC_EPI_WARPS = 8;
-constexpr int TC_THREADS = 32 * (2 + TC_EPI_WARPS);  // TMA, MMA, 8 epilogue warps
+constexpr int TC_THREADS = 128 + 32 * TC_EPI_WARPS;  // producer warpgroup, two consumer warpgroups
 constexpr int TC_EPI_PAR = 7 * 256;               // floats per parameter block: scale/shift/scale2/shift2/column offset/scale3/shift3
-constexpr int TC_EPI_SMEM = 2 * 2 * TC_EPI_PAR * 4;  // per epilogue group, double-buffered
-constexpr int TC_MAX_ACC = 4;  // TMEM accumulator stages (512 columns / BN, at most 4)
+constexpr int TC_EPI_SMEM = 2 * TC_EPI_PAR * 4;   // double-buffered
 constexpr int TC_MAX_STAGES = 8;
 constexpr int TC_A_BYTES = TC_BM * TC_BK * 2;  // 16 KiB
 constexpr int TC_SMEM_LIMIT = 232448;          // 227 KiB
+constexpr int tc_acc_bytes(int bn) { return TC_BM * (bn + 4) * 4; }  // staged fp32 accumulator tile
 
 struct TcGeom {
   long long M;  // B*OH*OW
@@ -56,16 +60,13 @@ struct TcGeom {
   int a_bytes, b_bytes;  // shared memory per pipeline stage
   // halo-flat mode (3x3, stride 1, input stored with a 1-pixel zero halo): M runs over
   // the padded-linear positions, one [136 x 64] slab per (filter row, channel chunk)
-  // feeds the three horizontal taps through row-shifted UMMA descriptors
+  // feeds the three horizontal taps through row-shifted wgmma descriptors
   int flat;
   int PW, PHW;     // padded row length W+2 and padded image size (H+2)*(W+2)
   int H, W;        // real input (= output) size in flat mode
   long long Q;     // B*(H+2)*(W+2)
   int out_halo;    // out0 / residual are stored with a 1-pixel halo
-  int bulk_store;  // tile rows are contiguous in out0: smem-staged cp.async.bulk stores
-  int nacc;        // accumulator stages in TMEM (2 or 4), BN columns each
-  int epi_split;   // 1: the two epilogue groups drain alternate tiles (N <= 128); 0: all 8 warps share a tile
-  int head_mode;   // fp32 scatter into candidate rows: 32x32 smem transpose per warp, coalesced stores
+  int head_mode;   // fp32 scatter into candidate rows: one row per store instruction, lanes on consecutive channels
   // row-block flat mode (flat == 2, fused 2x2/2 max pooling): a tile is RP image rows x XB
   // columns (RP*XB = 128); the slab of one filter row is a [XB+2 columns][RP rows][64 ch]
   // box, column-major over the tile so that tap s is the slab shifted by s*RP rows and the
@@ -75,18 +76,16 @@ struct TcGeom {
   // flat modes with a small filter bank: all 9*cchunks weight tiles [BN x 64] stay resident
   // in shared memory (loaded once per CTA); the pipeline stages then carry activations only
   int bres;
-  int pair;         // 1: launched as CTA pairs (conv_tc_kernel<2>)
   int klast;        // 16-deep K steps of the LAST 64-channel chunk that hold real input channels (1..4); with
                     // ODT_TC_KSKIP=1 the all-zero steps of a thin layer (Cin = 7..48 padded to 64 on both
-                    // operands) are not issued (predicated UTCHMMA, no branch); 4 otherwise
+                    // operands) are not issued (warpgroup-uniform branch); 4 otherwise
 };
-constexpr int TC_HEAD_STAGE = TC_EPI_WARPS * 32 * 33 * 4;  // per-warp [32][33] fp32 transpose tiles
 constexpr int TC_FLAT_ROWS = 136;                    // 128 + 2 neighbours, padded to 1024 B
 constexpr int TC_FLAT_A_BYTES = TC_FLAT_ROWS * 128;  // 17408
 
 // Optional per-role timeline of CTA 0 (compile with -DODT_TC_TIMELINE; off in the product build): lane 0 of
-// each role stamps clock64 at its hand-over points so that a tile's latency chain (TMA -> MMA -> commit ->
-// epilogue -> accumulator hand-back) can be read off directly.  Entries: (clock, role << 56 | event << 48 | tile).
+// each role stamps clock64 at its hand-over points so that a tile's latency chain (TMA -> MMA -> epilogue)
+// can be read off directly.  Entries: (clock, role << 56 | event << 48 | tile).
 #ifdef ODT_TC_TIMELINE
 __device__ unsigned long long* g_tl_buf = nullptr;
 __device__ unsigned int g_tl_cap = 0, g_tl_len = 0;
@@ -104,13 +103,7 @@ __device__ __forceinline__ void tl_stamp(int role, int event, int tile) {
 #endif
 
 // --------------------------------------------------------------- kernel ----
-// CG = 1: one CTA per tile.  CG = 2 (im2col mode only): the two CTAs of a cluster (one TPC)
-// share every MMA -- tcgen05.mma.cta_group::2, M = 256 = two M tiles, each CTA stages its own
-// 128 activation rows and HALF of the weight tile, so the shared-memory operand traffic per
-// SM and MMA drops from A+B to A+B/2 (the UMMA operand fetch, ~64 B/clk, is what bounds the
-// N = 256 layers at ~2/3 of the tensor peak with CG = 1).  Rank 0 issues the MMAs; its
-// commits are multicast to both CTAs' barriers.
-template <int CG>
+template <int BN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
     conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                    const __grid_constant__ TcGeom g, const __grid_constant__ Epi e) {
@@ -122,84 +115,48 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   const uint32_t a_bytes = (uint32_t)g.a_bytes, b_bytes = (uint32_t)g.b_bytes;
   const uint32_t a_base = base;
   const uint32_t b_base = base + (uint32_t)stages * a_bytes;
-  const uint32_t bn_cta = (uint32_t)(g.BN / CG);  // weight-tile rows staged by this CTA
-  const uint32_t wres_bytes = g.bres ? (uint32_t)(9 * g.cchunks) * bn_cta * 128u : 0u;
-  const uint32_t bar_base = b_base + (uint32_t)stages * b_bytes + wres_bytes;  // 8-byte aligned
-  // barriers: full[stages], empty[stages], tfull[2], tempty[2], then tmem ptr
+  const uint32_t wres_bytes = g.bres ? (uint32_t)(9 * g.cchunks) * (uint32_t)BN * 128u : 0u;
+  const uint32_t bar_base = b_base + (uint32_t)stages * b_bytes + wres_bytes;  // 1024-byte aligned
+  // barriers: full[stages], empty[stages], then the resident-weights barrier
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (TC_MAX_STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * TC_MAX_STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * TC_MAX_STAGES + TC_MAX_ACC + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * TC_MAX_STAGES + 2 * TC_MAX_ACC);
-  const uint32_t wfull_bar = tmem_slot + 8u;  // resident weights landed
-  uint32_t* tmem_slot_ptr =
-      reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - raw));
-  // per-tile epilogue parameters staged in smem: [buf][scale|shift|scale2|shift2][256]
+  const uint32_t wfull_bar = bar_base + 8u * (2 * TC_MAX_STAGES);  // resident weights landed
+  // per-tile epilogue parameters staged in smem: [buf][scale|shift|scale2|shift2|offset|scale3|shift3][256]
   float* epi_par = reinterpret_cast<float*>(smem_raw + (bar_base + 256u - raw));
-  // bulk-store staging: per TMEM lane quarter 32 rows x BN fp16 (only when g.bulk_store)
-  const uint32_t out_stage = bar_base + 256u + TC_EPI_SMEM;
+  // the tile's fp32 accumulators, one 128-row tile at a pitch of BN + 4 floats (row reads of float4 per
+  // lane hit distinct banks in every quarter-warp phase)
+  constexpr int ACC_PITCH = BN + 4;
+  float* acc_tile = reinterpret_cast<float*>(smem_raw + (bar_base + 256u + TC_EPI_SMEM - raw));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t cta_rank = CG == 2 ? cluster_ctarank() : 0u;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
     for (int s = 0; s < stages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int a = 0; a < TC_MAX_ACC; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), CG * (g.epi_split ? TC_EPI_WARPS / 2 : TC_EPI_WARPS));  // both CTAs' epilogues
+      mbar_init(empty_bar(s), TC_EPI_WARPS);  // one arrival per consumer warp
     }
     mbar_init(wfull_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    if (CG == 2) {  // warp 1 of both CTAs, same slot offset
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(tmem_slot)
-                   : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(tmem_slot)
-                   : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-  }
-  tc_fence_before();
-  if (CG == 2)
-    cluster_sync_all();  // barrier inits of both CTAs visible before any cross-CTA arrival
-  else
-    __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
+  __syncthreads();
   if (g.bres && warp == 0) {
     // the filter bank is constant data: fetch it before waiting on the previous kernel
     if (elect_one()) {
-      if (CG == 2) {  // both CTAs' halves are credited to rank 0's barrier (its MMA issuer waits there)
-        const uint32_t wb = mapa_u32(wfull_bar, 0);
-        if (cta_rank == 0) mbar_expect_tx(wfull_bar, 2u * wres_bytes);
-        for (int t = 0; t < 9 * g.cchunks; ++t)
-          tma_load_2d_cg2(b_base + (uint32_t)t * bn_cta * 128u, &tmB, wb, t * TC_BK, (int)(cta_rank * bn_cta));
-      } else {
-        mbar_expect_tx(wfull_bar, wres_bytes);
-        for (int t = 0; t < 9 * g.cchunks; ++t)
-          tma_load_2d(b_base + (uint32_t)t * (uint32_t)g.BN * 128u, &tmB, wfull_bar, t * TC_BK, 0);
-      }
+      mbar_expect_tx(wfull_bar, wres_bytes);
+      for (int t = 0; t < 9 * g.cchunks; ++t)
+        tma_load_2d(b_base + (uint32_t)t * (uint32_t)BN * 128u, &tmB, wfull_bar, t * TC_BK, 0);
     }
     __syncwarp();
   }
-  // Programmatic dependent launch: everything above (barrier init, TMEM allocation,
-  // descriptor prefetch) overlapped the tail of the previous kernel in the stream;
-  // from here on we touch memory it produced.
+  // Programmatic dependent launch: everything above (barrier init, descriptor prefetch, the
+  // resident filter bank) overlapped the tail of the previous kernel in the stream; from here
+  // on we touch memory it produced.
   pdl_launch_dependents();
   pdl_wait();
 
-  // CG = 2: a "tile" is a pair of M tiles (2*pair + rank) x one N tile, one pair per cluster
-  const int num_tiles = CG == 2 ? ((g.num_m_tiles + 1) / 2) * g.num_n_tiles : g.num_m_tiles * g.num_n_tiles;
-  const int tile_first = CG == 2 ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int tile_step = CG == 2 ? (int)(gridDim.x >> 1) : (int)gridDim.x;
+  const int num_tiles = g.num_m_tiles * g.num_n_tiles;
   const int kblocks = g.flat ? 3 * g.cchunks : g.R * g.S * g.cchunks;  // pipeline stages per tile
 
   if (warp == 0) {
@@ -208,13 +165,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     // uniform registers); one elected lane issues the TMA instructions.
     int stage = 0;
     uint32_t phase = 0;
-    const uint32_t full_rank0 = CG == 2 ? mapa_u32(bar_base, 0) : 0u;  // rank 0's barrier block
-    for (int tile = tile_first; tile < num_tiles; tile += tile_step) {
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int n_tile = tile % g.num_n_tiles;
-      int m_tile = CG == 2 ? 2 * (tile / g.num_n_tiles) + (int)cta_rank : tile / g.num_n_tiles;
-      if (CG == 2 && m_tile >= g.num_m_tiles) m_tile = g.num_m_tiles - 1;  // phantom half of the last pair: valid loads, no stores
+      const int m_tile = tile / g.num_n_tiles;
       const long long m0 = (long long)m_tile * TC_BM;
-      const int n0 = n_tile * g.BN;
+      const int n0 = n_tile * BN;
       tl_stamp(0, 0, tile);  // producer starts the tile's loads
       if (g.flat) {
         // one slab of 136 consecutive padded-linear rows per (filter row, chunk): rows
@@ -233,31 +188,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
             mbar_wait(empty_bar(stage), phase ^ 1u);
             if (elect_one()) {
               const uint32_t adst = a_base + (uint32_t)stage * a_bytes, bdst = b_base + (uint32_t)stage * b_bytes;
-              if (CG == 2) {
-                const uint32_t fb = full_rank0 + 8u * stage;
-                if (cta_rank == 0) mbar_expect_tx(full_bar(stage), 2u * ((uint32_t)g.a_tx + b_bytes));
-                if (g.flat == 2)
-                  tma_load_4d_cg2(adst, &tmA, fb, cc * TC_BK, g.RP * yq + r, g.XB * xq, bb);
-                else
-                  tma_load_2d_cg2(adst, &tmA, fb, cc * TC_BK, row0);
-                if (!g.bres) {
+              mbar_expect_tx(full_bar(stage), (uint32_t)g.a_tx + b_bytes);  // b_bytes == 0 when resident
+              if (g.flat == 2)  // padded rows RP*yq + r .., padded columns XB*xq .. (+2 for the taps)
+                tma_load_4d(adst, &tmA, full_bar(stage), cc * TC_BK, g.RP * yq + r, g.XB * xq, bb);
+              else
+                tma_load_2d(adst, &tmA, full_bar(stage), cc * TC_BK, row0);
+              if (!g.bres) {
 #pragma unroll
-                  for (int s = 0; s < 3; ++s)
-                    tma_load_2d_cg2(bdst + (uint32_t)s * bn_cta * 128u, &tmB, fb,
-                                    ((r * 3 + s) * g.cchunks + cc) * TC_BK, n0 + (int)(cta_rank * bn_cta));
-                }
-              } else {
-                mbar_expect_tx(full_bar(stage), (uint32_t)g.a_tx + b_bytes);  // b_bytes == 0 when resident
-                if (g.flat == 2)  // padded rows RP*yq + r .., padded columns XB*xq .. (+2 for the taps)
-                  tma_load_4d(adst, &tmA, full_bar(stage), cc * TC_BK, g.RP * yq + r, g.XB * xq, bb);
-                else
-                  tma_load_2d(adst, &tmA, full_bar(stage), cc * TC_BK, row0);
-                if (!g.bres) {
-#pragma unroll
-                  for (int s = 0; s < 3; ++s)
-                    tma_load_2d(bdst + (uint32_t)s * (uint32_t)g.BN * 128u, &tmB, full_bar(stage),
-                                ((r * 3 + s) * g.cchunks + cc) * TC_BK, n0);
-                }
+                for (int s = 0; s < 3; ++s)
+                  tma_load_2d(bdst + (uint32_t)s * (uint32_t)BN * 128u, &tmB, full_bar(stage),
+                              ((r * 3 + s) * g.cchunks + cc) * TC_BK, n0);
               }
             }
             __syncwarp();
@@ -279,22 +219,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
           for (int cc = 0; cc < g.cchunks; ++cc) {
             mbar_wait(empty_bar(stage), phase ^ 1u);
             if (elect_one()) {
-              if (CG == 2) {
-                // both CTAs' bytes are credited to rank 0's full barrier; this CTA loads its own
-                // 128 rows of A and its half (rank * BN/2 ...) of the weight tile
-                const uint32_t fb = full_rank0 + 8u * stage;
-                if (cta_rank == 0) mbar_expect_tx(full_bar(stage), 2u * (a_bytes + b_bytes));
-                tma_load_im2col_cg2(a_base + (uint32_t)stage * a_bytes, &tmA, fb, cc * TC_BK, cw, ch, img,
-                                    (uint16_t)(s * g.dil), (uint16_t)(r * g.dil));
-                tma_load_2d_cg2(b_base + (uint32_t)stage * b_bytes, &tmB, fb, kcol,
-                                n0 + (int)cta_rank * (g.BN / 2));
-              } else {
-                mbar_expect_tx(full_bar(stage), a_bytes + b_bytes);
-                tma_load_im2col(a_base + (uint32_t)stage * a_bytes, &tmA, full_bar(stage),
-                                cc * TC_BK, cw, ch, img, (uint16_t)(s * g.dil),
-                                (uint16_t)(r * g.dil));
-                tma_load_2d(b_base + (uint32_t)stage * b_bytes, &tmB, full_bar(stage), kcol, n0);
-              }
+              mbar_expect_tx(full_bar(stage), a_bytes + b_bytes);
+              tma_load_im2col(a_base + (uint32_t)stage * a_bytes, &tmA, full_bar(stage),
+                              cc * TC_BK, cw, ch, img, (uint16_t)(s * g.dil),
+                              (uint16_t)(r * g.dil));
+              tma_load_2d(b_base + (uint32_t)stage * b_bytes, &tmB, full_bar(stage), kcol, n0);
             }
             __syncwarp();
             kcol += TC_BK;
@@ -306,113 +235,65 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =========================================
-    // Warp-uniform loop; one elected lane issues tcgen05.mma / tcgen05.commit.  (With a
-    // single-lane branch around the whole loop ptxas has to bounce every descriptor
-    // through R2UR + an ELECT retry loop: ~170 cycles per MMA, measured.)
-    const uint32_t idesc = make_idesc_f16(CG * TC_BM, g.BN);
+  } else if (warp >= 4) {
+    // ===================== consumer warpgroups ===============================
+    // MMA: warpgroup `group` computes rows 64*group .. +63 of the tile over all BN columns.
+    // Epilogue: warp (group, quarter) owns pixel rows 32*quarter .. +31 (one per lane) and the
+    // 32-column chunks j = group, group + 2, ... of the staged accumulator tile.
+    const int quarter = warp & 3;
+    const int group = (warp - 4) >> 2;
+    const int et = threadIdx.x - 128;  // index among the 256 consumer threads
+    int staged_n_tile = -1, pbuf = 0;
     int stage = 0;
     uint32_t phase = 0;
-    int local_tile = 0;
     int cc_mma = 0;  // channel chunk of the current k-block (the k-block order ends with the chunk index)
-    if (g.bres && (CG == 1 || cta_rank == 0)) {  // the issuing CTA's barrier collects both halves
-      mbar_wait(wfull_bar, 0);
-      tc_fence_after();
-    }
-    for (int tile = (CG == 2 && cta_rank != 0) ? num_tiles : tile_first; tile < num_tiles;
-         tile += tile_step, ++local_tile) {
-      const int acc = local_tile % g.nacc;
-      const uint32_t use = (uint32_t)(local_tile / g.nacc);
-      mbar_wait(tempty_bar(acc), (use & 1u) ^ 1u);
-      tc_fence_after();
-      tl_stamp(1, 0, tile);  // accumulator stage free
-      const uint32_t d_tmem = tmem_base + (uint32_t)(acc * g.BN);
+    float acc[BN / 2];
+    if (g.bres) mbar_wait(wfull_bar, 0);
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int n_tile = tile % g.num_n_tiles;
+      const int m_tile = tile / g.num_n_tiles;
+      int prev = -1;
       for (int kb = 0; kb < kblocks; ++kb) {
         mbar_wait(full_bar(stage), phase);
-        tc_fence_after();
-        const uint64_t adesc = make_desc_sw128(a_base + (uint32_t)stage * a_bytes);
+        const uint64_t adesc = make_desc_sw128(a_base + (uint32_t)stage * a_bytes + (uint32_t)group * 64u * 128u);
         // resident bank: tile ((r*3 + s)*cchunks + cc) with kb = r*cchunks + cc
         const uint64_t bdesc = make_desc_sw128(
-            g.bres ? b_base + (uint32_t)((kb / g.cchunks) * 3 * g.cchunks + kb % g.cchunks) * bn_cta * 128u
+            g.bres ? b_base + (uint32_t)((kb / g.cchunks) * 3 * g.cchunks + kb % g.cchunks) * (uint32_t)BN * 128u
                    : b_base + (uint32_t)stage * b_bytes);
-        // 16-deep K steps of this chunk that hold real channels (predicated issue, see TcGeom::klast)
-        const int ksteps = (cc_mma == g.cchunks - 1) ? g.klast : TC_BK / 16;
+        // 16-deep K steps of this chunk that hold real channels (see TcGeom::klast)
+        // (broadcast from lane 0 so that ptxas sees a warp-uniform count)
+        const int ksteps = __shfl_sync(0xffffffffu, (cc_mma == g.cchunks - 1) ? g.klast : TC_BK / 16, 0);
         if (++cc_mma == g.cchunks) cc_mma = 0;
-        if (elect_one()) {
-          if (g.flat) {
-            // three horizontal taps from the same slab: operand rows s .. s+127, i.e. the
-            // descriptor start shifted by s*128 B inside the 1024 B swizzle pattern (the
-            // swizzle is a function of the absolute address: probed, scripts/probe_rowoffset.py)
-            const uint64_t bstep = (uint64_t)(((uint32_t)(g.bres ? g.cchunks : 1) * bn_cta * 128u) >> 4);
-            const uint64_t astep = (uint64_t)(g.flat == 2 ? 8 * g.RP : 8);  // rows per tap shift x 128 B >> 4
+        wg_fence();
+        if (g.flat) {
+          // three horizontal taps from the same slab: operand rows s .. s+63 of the half, i.e. the
+          // descriptor start shifted by s*128 B inside the 1024 B swizzle pattern
+          const uint64_t bstep = (uint64_t)(((uint32_t)(g.bres ? g.cchunks : 1) * (uint32_t)BN * 128u) >> 4);
+          const uint64_t astep = (uint64_t)(g.flat == 2 ? 8 * g.RP : 8);  // rows per tap shift x 128 B >> 4
 #pragma unroll
-            for (int s3 = 0; s3 < 3; ++s3) {
-#pragma unroll
-              for (int k = 0; k < TC_BK / 16; ++k) {
-                if (CG == 2)
-                  tc_mma_f16_cg2(d_tmem, adesc + astep * s3 + (uint64_t)(2 * k),
-                                 bdesc + bstep * s3 + (uint64_t)(2 * k), idesc, (uint32_t)((kb | s3 | k) != 0),
-                                 (uint32_t)(k < ksteps));
-                else
-                  tc_mma_f16(d_tmem, adesc + astep * s3 + (uint64_t)(2 * k),
-                             bdesc + bstep * s3 + (uint64_t)(2 * k), idesc, (uint32_t)((kb | s3 | k) != 0),
-                             (uint32_t)(k < ksteps));
-              }
-            }
-          } else {
-#pragma unroll
-            for (int k = 0; k < TC_BK / 16; ++k) {
-              // advance 16 elements (32 bytes) along K inside the swizzle atom
-              if (CG == 2)
-                tc_mma_f16_cg2(d_tmem, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc,
-                               (uint32_t)((kb | k) != 0), (uint32_t)(k < ksteps));
-              else
-                tc_mma_f16(d_tmem, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc,
-                           (uint32_t)((kb | k) != 0), (uint32_t)(k < ksteps));
-            }
-          }
-          if (CG == 2) {
-            tc_commit_cg2(empty_bar(stage), 3);  // both CTAs' smem slots
-            if (kb == kblocks - 1) tc_commit_cg2(tfull_bar(acc), 3);
-          } else {
-            tc_commit(empty_bar(stage));  // frees the smem slot when these MMAs retire
-            if (kb == kblocks - 1) tc_commit(tfull_bar(acc));  // accumulator complete -> epilogue
-          }
+          for (int s3 = 0; s3 < 3; ++s3)
+            wg_mma_chunk<BN>(acc, adesc + astep * s3, bdesc + bstep * s3, ksteps, (kb | s3) == 0);
+        } else {
+          wg_mma_chunk<BN>(acc, adesc, bdesc, ksteps, kb == 0);
         }
-        __syncwarp();
-        if (kb == 0) tl_stamp(1, 1, tile);            // first stage of the tile issued
-        if (kb == kblocks - 1) tl_stamp(1, 2, tile);  // last stage issued + committed
+        wg_commit();
+        wg_wait<1>();  // the previous k-block's MMAs have retired: its stage goes back to the producer
+        if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
+        prev = stage;
+        if (kb == 0 && quarter == 0) tl_stamp(1 + group, 0, tile);  // first stage of the tile issued
         if (++stage == stages) {
           stage = 0;
           phase ^= 1u;
         }
       }
-    }
-  } else {
-    // ===================== epilogue warps =====================================
-    // Two groups of four warps (one warp per TMEM lane quarter).  N <= 128 ("split"): the
-    // groups drain alternate tiles from four accumulator stages, so the latency of one
-    // epilogue pass (tcgen05.ld -> math -> stores -> fence -> arrive) is overlapped with the
-    // other group's pass instead of bounding the tile rate of short-K layers.  N > 128: both
-    // groups share every tile (even / odd 32-column chunks) over two 256-column stages.
-    const int quarter = warp & 3;
-    const int group = (warp - 2) >> 2;
-    const bool split = g.epi_split != 0;
-    const int et = split ? threadIdx.x - 64 - group * 128 : threadIdx.x - 64;  // index in the sync group
-    int staged_n_tile = -1, pbuf = 0;
-    float* gpar = epi_par + (split ? group * 2 * TC_EPI_PAR : 0);
-    const uint32_t row_bytes = (uint32_t)g.BN * 2u;
-    const uint32_t my_stage = out_stage + (uint32_t)(group * 4 + quarter) * 32u * row_bytes;
-    uint8_t* my_stage_ptr = smem_raw + (my_stage - raw) + lane * row_bytes;
-    int local_tile = 0;
-    const uint32_t tempty_rank0 = CG == 2 ? mapa_u32(tempty_bar(0), 0) : 0u;
-    for (int tile = tile_first; tile < num_tiles; tile += tile_step, ++local_tile) {
-      if (split && (local_tile & 1) != group) continue;
-      const int acc = local_tile % g.nacc;
-      const uint32_t use = (uint32_t)(local_tile / g.nacc);
-      const int n_tile = tile % g.num_n_tiles;
-      const int m_tile = CG == 2 ? 2 * (tile / g.num_n_tiles) + (int)cta_rank : tile / g.num_n_tiles;
+      wg_wait<0>();
+      if (lane == 0) mbar_arrive(empty_bar(prev));
+      if (quarter == 0) tl_stamp(1 + group, 1, tile);  // accumulators complete
+      // accumulators -> shared memory, once every consumer warp has finished reading the previous tile
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      wg_acc_to_smem<BN>(acc, acc_tile, ACC_PITCH, 64 * group);
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+
       const long long m = (long long)m_tile * TC_BM + quarter * 32 + lane;
       bool row_ok;
       int img, pix;
@@ -425,7 +306,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         const int yq = rem / g.xblocks, xq = rem - yq * g.xblocks;
         const int ml = quarter * 32 + lane;
         const int x = g.XB * xq + (ml >> g.lgRP), y = g.RP * yq + (ml & (g.RP - 1));
-        row_ok = x < g.W && y < g.H && m_tile < g.num_m_tiles;  // even sizes: a window is valid or invalid as a whole
+        row_ok = x < g.W && y < g.H;  // even sizes: a window is valid or invalid as a whole
         pix = 0;
         const int oh = g.out_halo;
         pool_row = (long long)img * e.out0_img_stride +
@@ -443,33 +324,26 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         img = row_ok ? (int)(m / g.ohw) : 0;
         pix = row_ok ? (int)(m - (long long)img * g.ohw) : 0;
       }
-      const int n0 = n_tile * g.BN;
-      // stage the per-channel parameters of this N tile once per group (broadcast reads
-      // later); consecutive tiles of single-N-tile layers reuse them
+      const int n0 = n_tile * BN;
+      // stage the per-channel parameters of this N tile once (broadcast reads later);
+      // consecutive tiles of single-N-tile layers reuse them
       if (n_tile != staged_n_tile) {
         staged_n_tile = n_tile;
         pbuf ^= 1;
-        float* wpar = gpar + pbuf * TC_EPI_PAR;
-#pragma unroll
-        for (int h2 = 0; h2 < 2; ++h2) {
-          const int c = split ? et + h2 * 128 : et;
-          if (!split && h2) break;
-          const int n = n0 + c;
-          const bool ok = c < g.BN && n < e.Cout;
-          wpar[c] = (ok && e.scale) ? __ldg(e.scale + n) : 1.f;
-          wpar[256 + c] = (ok && e.shift) ? __ldg(e.shift + n) : 0.f;
-          wpar[512 + c] = (ok && e.scale2) ? __ldg(e.scale2 + n) : 1.f;
-          wpar[768 + c] = (ok && e.shift2) ? __ldg(e.shift2 + n) : 0.f;
-          reinterpret_cast<int*>(wpar)[1024 + c] = ok ? regroup(e, n) : 0;
-          wpar[1280 + c] = (ok && e.scale3) ? __ldg(e.scale3 + n) : 1.f;
-          wpar[1536 + c] = (ok && e.shift3) ? __ldg(e.shift3 + n) : 0.f;
-        }
-        if (split)
-          asm volatile("bar.sync %0, 128;" ::"r"(1 + group) : "memory");
-        else
-          asm volatile("bar.sync 3, 256;" ::: "memory");
+        float* wpar = epi_par + pbuf * TC_EPI_PAR;
+        const int c = et;
+        const int n = n0 + c;
+        const bool ok = c < BN && n < e.Cout;
+        wpar[c] = (ok && e.scale) ? __ldg(e.scale + n) : 1.f;
+        wpar[256 + c] = (ok && e.shift) ? __ldg(e.shift + n) : 0.f;
+        wpar[512 + c] = (ok && e.scale2) ? __ldg(e.scale2 + n) : 1.f;
+        wpar[768 + c] = (ok && e.shift2) ? __ldg(e.shift2 + n) : 0.f;
+        reinterpret_cast<int*>(wpar)[1024 + c] = ok ? regroup(e, n) : 0;
+        wpar[1280 + c] = (ok && e.scale3) ? __ldg(e.scale3 + n) : 1.f;
+        wpar[1536 + c] = (ok && e.shift3) ? __ldg(e.shift3 + n) : 0.f;
+        asm volatile("bar.sync 3, 256;" ::: "memory");
       }
-      const float* par = gpar + pbuf * TC_EPI_PAR;
+      const float* par = epi_par + pbuf * TC_EPI_PAR;
       long long o0_row = (long long)img * e.out0_img_stride;
       if (g.out_halo) {
         const int oy = pix / g.OW, ox = pix - oy * g.OW;
@@ -479,21 +353,19 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
       }
       const long long o1_row = aux_row(e.out1_img_stride, e.out1_pix_stride, e.out1_halo, g.OW, img, pix);
       const long long o2_row = aux_row(e.out2_img_stride, e.out2_pix_stride, e.out2_halo, g.OW, img, pix);
-      if (g.bulk_store) {
-        // this warp's previous bulk store must have drained its staging rows
-        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-        __syncwarp();
-      }
-      mbar_wait(tfull_bar(acc), use & 1u);
-      tc_fence_after();
-      if (quarter == 0) tl_stamp(2 + group, 0, tile);  // accumulator complete (MMAs retired)
-      const uint32_t taddr0 = tmem_base + (uint32_t)(acc * g.BN) + ((uint32_t)(quarter * 32) << 16);
-      for (int j = split ? 0 : group; j < g.BN / 32; j += split ? 1 : 2) {
+      const float* my_acc = acc_tile + (quarter * 32 + lane) * ACC_PITCH;
+      for (int j = group; j < BN / 32; j += 2) {
         const int nb = n0 + j * 32;
-        if (nb >= e.Cout && !g.bulk_store) break;  // fully padded chunk (uniform)
+        if (nb >= e.Cout) break;  // fully padded chunk (uniform)
         uint32_t r[32];
-        tc_ld32(taddr0 + (uint32_t)(j * 32), r);
-        tc_wait_ld();
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const uint4 t = *reinterpret_cast<const uint4*>(my_acc + j * 32 + 4 * i);
+          r[4 * i + 0] = t.x;
+          r[4 * i + 1] = t.y;
+          r[4 * i + 2] = t.z;
+          r[4 * i + 3] = t.w;
+        }
         if (g.flat == 2) {
           // fused 2x2/2 max pooling: bias/BN + activation, round to fp16, then the maximum over
           // the window's four lanes (vertical neighbour = lane^1, horizontal = lane^RP); each
@@ -535,11 +407,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
             v[4 * i + 2] = apply_act(fmaf(__uint_as_float(r[4 * i + 2]), sc.z, sh.z), e.act);
             v[4 * i + 3] = apply_act(fmaf(__uint_as_float(r[4 * i + 3]), sc.w, sh.w), e.act);
           }
-          if (g.bulk_store && !row_ok) {  // halo / tail rows of the staged block are zeros
-            uint4* sp = reinterpret_cast<uint4*>(my_stage_ptr + j * 64);
-#pragma unroll
-            for (int qd = 0; qd < 4; ++qd) sp[qd] = make_uint4(0, 0, 0, 0);
-          }
           if (row_ok) {
             const long long o0 = o0_row + nb;
             if (e.residual) {
@@ -561,11 +428,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
             __half2* ph = reinterpret_cast<__half2*>(packed);
 #pragma unroll
             for (int i = 0; i < 16; ++i) ph[i] = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-            if (g.bulk_store) {
-              uint4* sp = reinterpret_cast<uint4*>(my_stage_ptr + j * 64);
-#pragma unroll
-              for (int qd = 0; qd < 4; ++qd) sp[qd] = packed[qd];
-            } else if (e.out0) {
+            if (e.out0) {
               uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<__half*>(e.out0) + o0);
 #pragma unroll
               for (int qd = 0; qd < 4; ++qd) op[qd] = packed[qd];
@@ -616,25 +479,20 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
           const int* pofs = reinterpret_cast<const int*>(par) + 1024 + j * 32;
           const int nvalid = min(32, e.Cout - nb);
           if (g.head_mode) {
-            // head convolutions: fp32 scatter into the candidate rows.  Each lane holds one
-            // pixel row; a 32x32 transpose through shared memory lets the warp write one
-            // row per instruction with the lanes on consecutive channels (4-5 sectors per
-            // request instead of 32).
-            float* tb = reinterpret_cast<float*>(smem_raw + (out_stage - raw)) + (warp - 2) * (32 * 33);
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              tb[lane * 33 + i] = apply_act(fmaf(__uint_as_float(r[i]), ps[i], ps[256 + i]), e.act);
-            __syncwarp();
+            // head convolutions: fp32 scatter into the candidate rows.  The staged accumulator
+            // tile is read column-wise, so the warp writes one row per instruction with the
+            // lanes on consecutive channels (4-5 sectors per request instead of 32).
+            const float* acol = acc_tile + (quarter * 32) * ACC_PITCH + j * 32 + lane;
+            const float sc = ps[lane], sh = ps[256 + lane];
             const int my_ofs = pofs[lane];
             const long long my_row = row_ok ? o0_row : -1;
             float* obase = reinterpret_cast<float*>(e.out0);
 #pragma unroll 4
             for (int rr = 0; rr < 32; ++rr) {
               const long long orow_r = __shfl_sync(0xffffffffu, my_row, rr);
-              const float val = tb[rr * 33 + lane];
+              const float val = apply_act(fmaf(acol[rr * ACC_PITCH], sc, sh), e.act);
               if (orow_r >= 0 && lane < nvalid) obase[orow_r + my_ofs] = val;
             }
-            __syncwarp();
           } else {
 #pragma unroll
             for (int i = 0; i < 32; ++i) {
@@ -662,49 +520,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
           }
         }
       }
-      // release the accumulator stage
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (CG == 2)
-          mbar_arrive_cluster(tempty_rank0 + 8u * acc);  // the MMA issuer (rank 0) waits for both CTAs
-        else
-          mbar_arrive(tempty_bar(acc));
-      }
-      if (quarter == 0) tl_stamp(2 + group, 1, tile);  // accumulator handed back
-      if (g.bulk_store) {
-        // the warp staged its 32 x BN block, contiguous in out0 (rows = consecutive pixels)
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          const long long first = (long long)m_tile * TC_BM + quarter * 32;
-          const long long left = (g.flat ? g.Q : g.M) - first;
-          if (left > 0) {
-            const uint32_t bytes = (uint32_t)(left < 32 ? left : 32) * row_bytes;
-            const __half* gdst = reinterpret_cast<const __half*>(e.out0) + first * e.out0_pix_stride;
-            asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst),
-                         "r"(my_stage), "r"(bytes)
-                         : "memory");
-            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-          }
-        }
-      }
+      if (quarter == 0) tl_stamp(1 + group, 2, tile);  // epilogue done
     }
-    if (g.bulk_store && lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-  }
-
-  // ---- teardown ----
-  tc_fence_before();
-  if (CG == 2)
-    cluster_sync_all();  // the peer's shared memory / TMEM stay alive until every MMA has retired
-  else
-    __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    if (CG == 2)
-      asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
-    else
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
   }
 }
 
@@ -782,37 +599,28 @@ int check_conv_params(const odt_conv_params* p) {
 
 using namespace odt;
 
-// N tile and launch shape of an im2col-mode layer from a two-term cost model:
-//   time ~ rounds * (kblocks * cost_kb + fixed),
-//   cost_kb = 256 + 2*BN cycles per 64-deep K block with one CTA per tile (UMMA operand
-//             fetch of A and B at ~64 B/clk -- the same figure as the per-SM L2->smem fill),
-//           = 256 +   BN with CTA pairs (each CTA stages half of the weight tile),
-//   rounds  = tiles per CTA (or pair-tiles per cluster) of the slowest SM.
+// N tile of an im2col-mode layer from a two-term cost model:
+//   time ~ rounds * (kblocks * (128 + 4*BN) + 2000 + 8*BN),
+//   4*BN    = clocks of the 128 x BN x 64 multiply-adds of one K block at the dense fp16 wgmma rate
+//             (2048 FMA/clk/SM), 128 = per-K-block barrier and issue overhead,
+//   2000 + 8*BN = the epilogue, which the consumer warpgroups run between two tiles,
+//   rounds  = tiles per CTA of the slowest SM.
 // Small-M layers (FPN P5-P7 towers, SSD extras) come out with narrow tiles spread over many
-// SMs, large ones with 256-wide pair tiles.
-static void pick_tiling(int cout_pad, int m_tiles, int kblocks, bool allow_pair, int* bn_out, int* pair_out) {
+// SMs, large ones with 128-wide tiles.
+static int pick_bn(int cout_pad, int m_tiles, int kblocks) {
   long long best = -1;
-  int best_bn = 32, best_pair = 0;
-  for (int bn = 256; bn >= 32; bn -= 32) {
+  int best_bn = 32;
+  for (int bn = TC_MAX_BN; bn >= 32; bn -= 32) {
     if (cout_pad % bn != 0) continue;
-    const long long n_tiles = cout_pad / bn;
-    for (int pair = allow_pair ? 1 : 0; pair >= 0; --pair) {
-      if (pair && (bn < 64 || m_tiles < 2)) continue;
-      const long long units = pair ? (long long)((m_tiles + 1) / 2) * n_tiles : (long long)m_tiles * n_tiles;
-      const long long slots = pair ? kNumSMs / 2 : kNumSMs;
-      const long long rounds = (units + slots - 1) / slots;
-      // + a per-launch constant for the cluster launch / cluster barriers of the pair kernel
-      const long long cost =
-          rounds * ((long long)kblocks * (256 + (pair ? bn : 2 * bn)) + 2000) + (pair ? 4000 : 0);
-      if (best < 0 || cost < best) {  // ties keep the wider tile / the pair launch (visited first)
-        best = cost;
-        best_bn = bn;
-        best_pair = pair;
-      }
+    const long long units = (long long)m_tiles * (cout_pad / bn);
+    const long long rounds = (units + kNumSMs - 1) / kNumSMs;
+    const long long cost = rounds * ((long long)kblocks * (128 + 4 * bn) + 2000 + 8 * bn);
+    if (best < 0 || cost < best) {  // ties keep the wider tile (visited first)
+      best = cost;
+      best_bn = bn;
     }
   }
-  *bn_out = best_bn;
-  *pair_out = best_pair;
+  return best_bn;
 }
 
 extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_conv_params* p,
@@ -863,8 +671,8 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
   g.lower_h = -p->pad_t + ih;
   g.cchunks = p->in_ld / 64;
   {
-    // opt-in until a same-box A/B settles it (parity-tested; 68 -> 62 us on a 7->7 RetinaNet layer under ncu,
-    // unresolved in whole-graph times): with the knob off every step is issued
+    // ODT_TC_KSKIP (default on, carried over from the previous target, not re-measured on the H100): with the knob
+    // off every step is issued
     const int rem = p->Cin - (g.cchunks - 1) * TC_BK;  // real channels in the last chunk
     g.klast = !kskip_enabled() || rem >= TC_BK ? TC_BK / 16 : (rem <= 0 ? 1 : (rem + 15) / 16);
   }
@@ -906,55 +714,34 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
     g.num_n_tiles = 1;
     g.a_bytes = TC_FLAT_A_BYTES;
     g.a_tx = (g.XB + 2) * g.RP * 128;
-    // CTA pairs (half of each tap tile per CTA): +21 % at Cin = 128 (conv2_2), +3 % at Cin = 64 in this
-    // pooled mode (conv1_2: the light pooled epilogue leaves room for the handshakes)
-    g.pair = (flat_pair_enabled() && g.num_m_tiles >= 2) ? 1 : 0;
-    g.b_bytes = 3 * (g.pair ? g.BN / 2 : g.BN) * 128;
+    g.b_bytes = 3 * g.BN * 128;
   } else if (g.flat) {
     g.a_tx = TC_FLAT_A_BYTES;
     g.num_m_tiles = (int)((g.Q + TC_BM - 1) / TC_BM);
     g.BN = p->Cout_pad;
     g.num_n_tiles = 1;
     g.a_bytes = TC_FLAT_A_BYTES;
-    // CTA pairs (half of each tap tile per CTA) pay off once a tile is long enough to hide the
-    // cross-CTA handshakes: measured +21 % at Cin = 128 (conv2_2), -10 % at Cin <= 64 (conv2_1)
-    g.pair = (flat_pair_enabled() && g.num_m_tiles >= 2 && g.cchunks >= 2) ? 1 : 0;
-    g.b_bytes = 3 * (g.pair ? g.BN / 2 : g.BN) * 128;
+    g.b_bytes = 3 * g.BN * 128;
   } else {
     g.num_m_tiles = (int)((g.M + TC_BM - 1) / TC_BM);
-    pick_tiling(p->Cout_pad, g.num_m_tiles, p->R * p->S * g.cchunks, pair_enabled(), &g.BN, &g.pair);
+    g.BN = pick_bn(p->Cout_pad, g.num_m_tiles, p->R * p->S * g.cchunks);
     g.num_n_tiles = (p->Cout_pad + g.BN - 1) / g.BN;
     g.a_bytes = TC_A_BYTES;
-    g.b_bytes = (g.pair ? g.BN / 2 : g.BN) * 128;
+    g.b_bytes = g.BN * 128;
   }
   stage_bytes = g.a_bytes + g.b_bytes;
-  // staged bulk stores: fp16 rows of exactly BN channels that are contiguous over the tile
-  // (flat mode writing a halo tensor of the same geometry, or im2col mode writing dense NHWC)
-  const bool linear_rows =
-      g.flat ? (p->out0_halo == 1 &&
-                p->out0_img_stride == (long long)(p->OH + 2) * (p->OW + 2) * p->out0_pix_stride)
-             : (p->out0_halo == 0 && p->out0_img_stride == (long long)p->OH * p->OW * p->out0_pix_stride);
-  g.bulk_store = (bulk_enabled() && g.flat != 2 && p->out0 && !p->out1 && !p->out2 && p->out0_dtype == ODT_F16 &&
-                  p->out0_group == 0 && g.num_n_tiles == 1 && g.BN <= 64 &&
-                  g.BN == p->out0_pix_stride && linear_rows && ((uintptr_t)p->out0 & 15) == 0 &&
-                  (!p->residual || ((uintptr_t)p->residual & 15) == 0))
-                     ? 1
-                     : 0;
   g.head_mode = (p->out0 && p->out0_dtype == ODT_F32 && !p->residual && !p->out1 && !p->out2) ? 1 : 0;
-  const int out_stage_bytes =
-      g.bulk_store ? TC_EPI_WARPS * 32 * g.BN * 2 : (g.head_mode ? TC_HEAD_STAGE : 0);  // per-warp staging
-  g.epi_split = g.BN <= 128 ? 1 : 0;
-  g.nacc = g.epi_split ? 4 : 2;
+  // barriers + 1024-byte alignment slack, epilogue parameters, staged accumulator tile
+  const int fixed_bytes = 2048 + TC_EPI_SMEM + tc_acc_bytes(g.BN);
   // small filter banks of the flat modes stay resident in shared memory if at least three
   // activation stages still fit beside them
-  const long long wres = 9ll * g.cchunks * (g.pair ? g.BN / 2 : g.BN) * 128;  // per CTA
-  if (g.flat && wres_enabled() && g.BN >= 128 &&  // measured: a win at N = 128 (conv2_1), a loss at N <= 64
-      wres + 3 * TC_FLAT_A_BYTES + 2048 + TC_EPI_SMEM + out_stage_bytes <= TC_SMEM_LIMIT) {
+  const long long wres = 9ll * g.cchunks * g.BN * 128;
+  if (g.flat && wres_enabled() && g.BN >= 128 && wres + 3 * TC_FLAT_A_BYTES + fixed_bytes <= TC_SMEM_LIMIT) {
     g.bres = 1;
     g.b_bytes = 0;
     stage_bytes = g.a_bytes;
   }
-  int stages = (TC_SMEM_LIMIT - 2048 - TC_EPI_SMEM - out_stage_bytes - (g.bres ? (int)wres : 0)) / stage_bytes;
+  int stages = (TC_SMEM_LIMIT - fixed_bytes - (g.bres ? (int)wres : 0)) / stage_bytes;
   if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
   ODT_CHECK_ARG(stages >= 2, "tile too large for shared memory");
   g.stages = stages;
@@ -1025,7 +812,7 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
     const cuuint64_t ktot = (cuuint64_t)p->R * p->S * p->w_ld;
     cuuint64_t dims[2] = {ktot, (cuuint64_t)p->Cout_pad};
     cuuint64_t strides[1] = {ktot * 2};
-    cuuint32_t box[2] = {TC_BK, (cuuint32_t)(g.pair ? g.BN / 2 : g.BN)};
+    cuuint32_t box[2] = {TC_BK, (cuuint32_t)g.BN};
     cuuint32_t estr[2] = {1, 1};
     CUresult cr = g_encode_tiled(&tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2,
                                  const_cast<void*>(weights), dims, strides, box, estr,
@@ -1038,14 +825,18 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
     }
   }
 
-  const int smem = stages * stage_bytes + (g.bres ? (int)wres : 0) + 2048 + TC_EPI_SMEM + out_stage_bytes;
-  static int smem_set = 0;
-  if (smem_set < smem) {
-    ODT_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     TC_SMEM_LIMIT));
-    ODT_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     TC_SMEM_LIMIT));
-    smem_set = TC_SMEM_LIMIT;
+  const int smem = stages * stage_bytes + (g.bres ? (int)wres : 0) + fixed_bytes;
+  void (*kern)(CUtensorMap, CUtensorMap, TcGeom, Epi) =
+      g.BN == 32 ? conv_tc_kernel<32> : g.BN == 64 ? conv_tc_kernel<64> : g.BN == 96 ? conv_tc_kernel<96>
+                                                                                    : conv_tc_kernel<128>;
+  ODT_CHECK_ARG(g.BN % 32 == 0 && g.BN <= TC_MAX_BN, "N tile");
+  static bool smem_set = false;
+  if (!smem_set) {
+    ODT_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
+    ODT_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
+    ODT_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<96>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
+    ODT_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
+    smem_set = true;
   }
   Epi e = make_epi(*p);
   cudaLaunchConfig_t cfg = {};
@@ -1054,25 +845,12 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
   cfg.attrs = attr;
-  if (g.pair) {
-    // one cluster (two CTAs on one TPC) per pair of M tiles; persistent over at most 74 clusters
-    const int num_pairs = ((g.num_m_tiles + 1) / 2) * g.num_n_tiles;
-    const int clusters = num_pairs < kNumSMs / 2 ? num_pairs : kNumSMs / 2;
-    cfg.gridDim = dim3(2 * clusters);
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.numAttrs = 1;
-    ODT_CUDA_OK(cudaLaunchKernelEx(&cfg, conv_tc_kernel<2>, tmA, tmB, g, e));
-  } else {
-    const int num_tiles = g.num_m_tiles * g.num_n_tiles;
-    cfg.gridDim = dim3(num_tiles < kNumSMs ? num_tiles : kNumSMs);
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.numAttrs = pdl_enabled() ? 1 : 0;
-    ODT_CUDA_OK(cudaLaunchKernelEx(&cfg, conv_tc_kernel<1>, tmA, tmB, g, e));
-  }
+  const int num_tiles = g.num_m_tiles * g.num_n_tiles;
+  cfg.gridDim = dim3(num_tiles < kNumSMs ? num_tiles : kNumSMs);
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  ODT_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, g, e));
   ODT_LAUNCH_OK();
   return ODT_OK;
 }

@@ -1,9 +1,8 @@
 // CUDA-core convolution for VERY thin layers (RetinaNet's 7*2^i bottlenecks: 16->7, 7->7, 7->28, 14->14 ...).
 //
 // Such a layer is not tensor-core work: 3x3 7->7 is 441 multiply-adds per pixel, the activations are stored in
-// 64-channel (128-byte) pixel rows of which 14 bytes are data, and the tcgen05 path pays an MMA operand fetch
-// (>= 64 clk per 16-deep K step, conv_tc.cu) and moves the whole 128-byte rows through TMA for it -- 68 us for
-// 640 k pixels whatever Cin / Cout are.  Here one thread owns one output pixel and all its (<= 32) output
+// 64-channel (128-byte) pixel rows of which 14 bytes are data, and the tensor-core path moves the whole 128-byte
+// rows through TMA and multiplies at least 16 zero-padded input channels per K step whatever Cin / Cout are.  Here one thread owns one output pixel and all its (<= 32) output
 // channels: it reads only the 16-byte sectors of the input rows that hold real channels, keeps the filter bank
 // in shared memory as fp32 [tap][cin][cout] (warp-broadcast 128-bit reads, 4 FMA per LDS), accumulates in
 // fp32 and writes only the 16-byte sectors that hold real output channels (the zero padding of the dedicated
@@ -225,9 +224,8 @@ static int thin_plan(const void* in, const odt_conv_params* p, bool force, ThinG
   if (!io_ok) return ODT_ERR_UNSUPPORTED;
   const long long M = (long long)p->B * p->OH * p->OW;
   if (M >= (1ll << 31) * THIN_THREADS) return ODT_ERR_UNSUPPORTED;
-  // default planner (mode 1): only 1x1 layers with few multiply-adds per pixel.  Same-box A/B of round 2
-  // (profiles/r02_ab_micro.md): 1x1 16->7 0.035 -> 0.027 ms, 28->7 0.052 -> 0.037 ms at 200x200x16, but every 3x3
-  // layer is faster through the taps-as-N tensor-core kernel (7->7: 0.041 vs 0.055 ms; 14->14: 0.015 vs 0.045 ms)
+  // default planner (mode 1): only 1x1 layers with few multiply-adds per pixel.  The rule is carried over from the
+  // previous target; it has not been re-measured on the H100.
   if (!force && (ks != 1 || ci8r * 8 * co8r * 8 > 1200)) return ODT_ERR_UNSUPPORTED;
   ThinGeom g;
   memset(&g, 0, sizeof(g));

@@ -37,7 +37,7 @@ struct Epi {
 
 int check_conv_params(const odt_conv_params* p);
 }  // namespace odt
-// internal: tcgen05 stem; ODT_ERR_UNSUPPORTED when no variant matches
+// internal: tensor-core stem; ODT_ERR_UNSUPPORTED when no variant matches
 int odt_conv2d_stem_tc_try(const float* images, const float* mean3_host, const void* weights,
                            const odt_conv_params* p, void* stream);
 namespace odt {

@@ -1,4 +1,4 @@
-// Inference tail of the five detectors on sm_100a: score activation, analytic
+// Inference tail of the five detectors on sm_90a: score activation, analytic
 // anchor/prior generation, box decode, thresholding, candidate compaction and
 // exact per-class TF NonMaxSuppressionV3 (iterative arg-max + IoU suppress).
 //
@@ -617,11 +617,10 @@ extern "C" int odt_decode_candidates(const float* head, const odt_tail_params* p
   if (const char* e = getenv("ODT_DECODE_BLOCKS_PER_SM")) per_sm = atoi(e) > 0 ? atoi(e) : per_sm;
   int maxb = kNumSMs * per_sm;
   if (blocks > maxb) blocks = maxb;
-  // Two builds per kind (A/B by ODT_DECODE_CFG, default from profiles/r02_tail.md): "3x2" = 3 CTAs / SM with 2 stages
-  // per warp (24 warps x 1 group in flight ahead), "2x4" = 2 CTAs / SM with 4 stages (16 warps x 3 groups ahead: more
-  // bytes in flight per SM, fewer warps to hide instruction latency)
-  // measured (profiles/r02_tail.md): 3x2 22.1 / 75.8 / 43.9 us against 2x4 26.0 / 79.3 / 56.7 us (SSD300 B=64 /
-  // RetinaNet-800 B=16 / YOLOv3 B=32): the kernel is bound by per-warp instruction issue, not by bytes in flight
+  // Two builds per kind (A/B by ODT_DECODE_CFG): "3x2" = 3 CTAs / SM with 2 stages per warp (24 warps x 1 group in
+  // flight ahead, the default), "2x4" = 2 CTAs / SM with 4 stages (16 warps x 3 groups ahead: more bytes in flight per
+  // SM, fewer warps to hide instruction latency).  The default is carried over from the previous target; it has not
+  // been re-measured on the H100.
   int deep = 0;
   if (const char* e = getenv("ODT_DECODE_CFG")) deep = strcmp(e, "2x4") == 0 ? 1 : 0;
 #define ODT_DECODE_LAUNCH(KIND_, OCC_, ST_)                                                                      \

@@ -1,3 +1,3 @@
-"""odt_b200: B200-native (sm_100a) detection hot path behind the reference's
+"""odt_b200: H100-native (sm_90a) detection hot path behind the reference's
 model API.  See DESIGN.md."""
 from .api import FCOS, SSD300, SSD512, RetinaNet, YOLOv3  # noqa: F401

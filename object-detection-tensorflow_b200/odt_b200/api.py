@@ -1,4 +1,4 @@
-"""The reference's public model surface on the B200 engine.
+"""The reference's public model surface on the H100 engine.
 
 Same class names, constructor signature `(config, data_provider)`, config keys,
 asserts and method names as the reference model scripts, so its test*.py

@@ -1,11 +1,11 @@
-"""Host runtime of the B200 detection path: a tiny static-graph builder whose
+"""Host runtime of the H100 detection path: a tiny static-graph builder whose
 ops are launches of the C-ABI kernels (include/odt_b200.h) on torch-owned
 device buffers.  PyTorch is plumbing only (allocation, streams, CUDA graphs).
 
 A model file (nets.py) describes its layers once through `Builder`; the builder
   * names variables the way TF1 variable scopes do (SURVEY.md App. D) so the
     same weight dict drives this path and the CPU oracle,
-  * pads fp16 activations to 64-channel multiples (TMA / UMMA K-chunk),
+  * pads fp16 activations to 64-channel multiples (TMA / wgmma K-chunk),
   * fuses what the reference expresses as separate TF ops into conv epilogues:
     bias / folded inference BN / ReLU / LeakyReLU / residual add / the
     consumer's pre-activation BN+ReLU (second output) / direct scatter of the
@@ -204,13 +204,13 @@ class ConvOp(Op):
             p.out2_halo = t.halo
         self.p = p
         self.flops = 2 * B * OH * OW * cout * R * S * cin
-        # stems: the tcgen05 variants read a packed fp16 RGBX copy of the image (mean subtracted, zero border of
+        # stems: the tensor-core variants read a packed fp16 RGBX copy of the image (mean subtracted, zero border of
         # `rgbx` pixels) so that every filter row is one aligned span -- see csrc/conv_stem_tc.cu
         self.rgbx = 0
         if (self.is_image and f16 and net.allow_tc and self.pre is None and self.head is None
                 and os.environ.get("ODT_STEM_RGBX", "1") != "0"):
-            # same-box A/B (profiles/r02_ab_micro.md): RetinaNet-800 stem 0.36 -> 0.205 ms, but the 3x3 / stride-1
-            # stems gain nothing (SSD300 conv1_1 0.254 -> 0.278 ms incl. the pack pass): ODT_STEM_RGBX=2 forces them
+            # the 7x7 / stride-2 stem takes the packed image by default, the 3x3 / stride-1 stems only with
+            # ODT_STEM_RGBX=2 (a choice carried over from the previous target, not re-measured on the H100)
             force3 = os.environ.get("ODT_STEM_RGBX") == "2"
             if (R, self.stride, cout) in ((3, 1, 64), (3, 1, 32)) and force3:
                 self.rgbx = 1
@@ -580,7 +580,7 @@ class Net:
     def assign_halos(self):
         """Give a zero 1-pixel halo to fp16 tensors that feed a flat-eligible 3x3 conv
         (stride 1, dilation 1, padded Cout <= 128) when every producer / consumer of the
-        tensor understands the layout (tensor-core convs, the tcgen05 stems, max-pool)."""
+        tensor understands the layout (tensor-core convs, the tensor-core stems, max-pool)."""
         if self.precision != "fp16" or not self.allow_tc:
             return
         readers, producer = {}, {}

@@ -1,5 +1,5 @@
 """Layer graphs of SSD300 / SSD512 / RetinaNet / YOLOv3 / FCOS expressed on the
-B200 engine (engine.Net).  Each builder mirrors the reference's layer creation
+H100 engine (engine.Net).  Each builder mirrors the reference's layer creation
 order so variables get the same TF1 names as in the reference checkpoints
 (SURVEY.md App. D); citations give the reference lines each block stands for.
 """

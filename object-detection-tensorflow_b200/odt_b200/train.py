@@ -3,7 +3,7 @@ per-image loss, backward, Momentum(0.9) + L2 weight decay -- what `train_one_epo
 (SSD300.py:129-155,345-453,473-484).
 
 Scope and honesty: this is the "PyTorch autograd first" stage the survey plans.  The forward / backward convolutions
-here are PyTorch's (library kernels), in fp32; the hand-written sm_100a kernels of this repository cover the
+here are PyTorch's (library kernels), in fp32; the hand-written sm_90a kernels of this repository cover the
 inference hot path and the loss FORWARD (csrc/loss.cu: the same value this module computes, used as a cross-check).
 dgrad / wgrad kernels are the next stage.  Restated from the reference, not copied:
 

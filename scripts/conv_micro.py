@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""One tensor-core conv in isolation (for ncu / A-B timing).
+"""One tensor-core conv in isolation (for A-B timing with CUDA events).
 usage: conv_micro.py B H W Cin Cout k stride [pool] [in_halo] [out_halo] [reps]"""
 import ctypes as C
 import os

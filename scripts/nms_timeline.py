@@ -26,7 +26,7 @@ def build_debug_lib():
     out = os.path.join(PKG, "odt_b200", "libodt_b200_nmstl.so")
     subprocess.check_call(["nvcc"] + ge.NVCC_FLAGS + ["-DODT_NMS_TIMELINE", "-c", "tail.cu", "-o", obj], cwd=csrc)
     objs = [os.path.join(csrc, s[:-3] + ".o") for s in ge.SRCS if s != "tail.cu"] + [obj]
-    subprocess.check_call(["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", out] + objs + ["-ldl"],
+    subprocess.check_call(["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", out] + objs + ["-ldl"],
                           cwd=csrc)
     return out
 

@@ -4,5 +4,5 @@ path; touching any attribute is an error."""
 
 
 def __getattr__(name):
-    raise AttributeError("tensorflow shim: the B200 path has no TensorFlow runtime (asked for tf.%s)"
+    raise AttributeError("tensorflow shim: the H100 path has no TensorFlow runtime (asked for tf.%s)"
                          % name)

@@ -15,7 +15,7 @@ pytestmark = pytest.mark.gpu
 
 def _conv_case(B, H, W, Cin, Cout, k, stride, dil, mode, act="relu", residual=False, pre=False,
                bn=True, f32_out=False, seed=0, in_halo=0, out_halo=0, pool=0, pre2=False, no_out0=False, aux_halo=0):
-    """mode: 'tc' (fp16 tcgen05), 'direct16', 'direct32'.  Returns (got, ref, got1, ref1)."""
+    """mode: 'tc' (fp16 wgmma), 'direct16', 'direct32'.  Returns (got, ref, got1, ref1)."""
     from odt_b200 import lib as L
     from odt_b200.engine import same_pad
     from oracle import tfops as T
@@ -326,8 +326,8 @@ def test_glue_kernels_vs_oracle_ops(built, dtype):
 @pytest.mark.parametrize("dtype", ["f16", "f32", "rgbx"])
 def test_stem_conv_vs_oracle(built, shape, dtype):
     """odt_conv2d_stem: fp32 image - RGB mean -> conv -> bias/BN -> ReLU.  fp16 takes the
-    tcgen05 stem (A tile built in swizzled smem), fp32 the CUDA-core stem; 'rgbx' = odt_pack_input_rgbx +
-    odt_conv2d_stem_rgbx (the tcgen05 stem on the packed fp16 image, the engine's default)."""
+    tensor-core stem (A tile built in swizzled smem), fp32 the CUDA-core stem; 'rgbx' = odt_pack_input_rgbx +
+    odt_conv2d_stem_rgbx (the tensor-core stem on the packed fp16 image, the engine's default)."""
     from odt_b200 import lib as L
     from odt_b200.engine import same_pad
     from oracle import tfops as T
@@ -460,36 +460,34 @@ def test_conv_tc_resident_filter_bank_is_bit_identical(built, monkeypatch, shape
     np.testing.assert_array_equal(a, b)
 
 
-PAIR_SHAPES = [
-    # >= 296 tiles -> CTA-pair launch (tcgen05 cta_group::2): B, H, W, Cin, Cout, k, stride, dil
-    (5, 88, 88, 128, 256, 3, 1, 1),    # 303 M tiles: odd count (phantom half pair) + ragged last tile
-    (4, 69, 69, 128, 512, 3, 1, 1),    # two N tiles of 256, 149 M tiles
-    (8, 75, 75, 256, 128, 1, 1, 1),    # 1x1, N = 128 (64 weight rows per CTA)
+LARGE_SHAPES = [
+    # hundreds of tiles, several rounds of the persistent grid: B, H, W, Cin, Cout, k, stride, dil
+    (5, 88, 88, 128, 256, 3, 1, 1),    # 303 M tiles: odd count + ragged last tile
+    (4, 69, 69, 128, 512, 3, 1, 1),    # four N tiles of 128, 149 M tiles
+    (8, 75, 75, 256, 128, 1, 1, 1),    # 1x1, N = 128
     (8, 150, 150, 64, 192, 3, 2, 1),   # stride 2, N = 192
     (6, 80, 80, 64, 96, 3, 1, 2),      # dilation 2, N = 96
 ]
 
 
-@pytest.mark.parametrize("shape", PAIR_SHAPES)
-def test_conv_tc_cta_pairs(built, monkeypatch, shape):
-    """cta_group::2 path against the fp32 reference and bit-identical to the one-CTA path
-    (same K order, same accumulator precision)."""
+@pytest.mark.parametrize("shape", LARGE_SHAPES)
+def test_conv_tc_large_tile_counts(built, shape):
+    """Layers of hundreds of tiles (odd tile counts, ragged last tiles, several N tiles, stride, dilation) against the
+    fp32 reference, and two launches bit-identical (static tile schedule, fixed K order)."""
     a, ref, a1, r1 = _conv_case(*shape, mode="tc", act="leaky", residual=True, pre=True, seed=sum(shape))
     tol = 2e-3 * max(np.abs(ref).max(), 1.0)
     assert np.abs(a - ref).max() <= tol and np.abs(a1 - r1).max() <= 2 * tol
-    monkeypatch.setenv("ODT_TC_PAIR", "0")
     b, _, b1, _ = _conv_case(*shape, mode="tc", act="leaky", residual=True, pre=True, seed=sum(shape))
     np.testing.assert_array_equal(a, b)
     np.testing.assert_array_equal(a1, b1)
 
 
-def test_conv_tc_cta_pairs_head_scatter_and_halo(built, monkeypatch):
-    # fp32 head rows (RetinaNet cls head shape class) and halo in/out layouts through the pair path
+def test_conv_tc_large_head_scatter_and_halo(built):
+    # fp32 head rows (RetinaNet cls head shape class) and halo in/out layouts at large tile counts
     g, ref, _, _ = _conv_case(4, 100, 100, 256, 189, 3, 1, 1, mode="tc", act=None, f32_out=True)
     assert np.abs(g - ref).max() <= 2e-3 * max(np.abs(ref).max(), 1.0)
     h, ref2, _, _ = _conv_case(4, 100, 100, 128, 256, 3, 1, 1, mode="tc", in_halo=1, out_halo=1)
     assert np.abs(h - ref2).max() <= 2e-3 * max(np.abs(ref2).max(), 1.0)
-    monkeypatch.setenv("ODT_TC_PAIR", "0")
     h0, _, _, _ = _conv_case(4, 100, 100, 128, 256, 3, 1, 1, mode="tc", in_halo=1, out_halo=1)
     np.testing.assert_array_equal(h, h0)
 
@@ -497,18 +495,17 @@ def test_conv_tc_cta_pairs_head_scatter_and_halo(built, monkeypatch):
 @pytest.mark.parametrize("shape,pool", [((2, 38, 38, 64, 64, 3, 1, 1), 0), ((3, 75, 75, 64, 128, 3, 1, 1), 0),
                                         ((2, 300, 300, 64, 64, 3, 1, 1), 2), ((2, 150, 150, 128, 128, 3, 1, 1), 2),
                                         ((1, 150, 150, 128, 128, 3, 1, 1), 0), ((1, 17, 23, 64, 28, 3, 1, 1), 0)])
-def test_conv_tc_flat_cta_pairs_bit_identical(built, monkeypatch, shape, pool):
-    """Halo-flat / row-block modes launched as CTA pairs vs one CTA per tile: same bits."""
+def test_conv_tc_flat_modes_bit_identical(built, shape, pool):
+    """Halo-flat / row-block modes against the fp32 reference, and two launches bit-identical."""
     a, ref, _, _ = _conv_case(*shape, mode="tc", in_halo=1, out_halo=1, pool=pool)
     assert np.abs(a - ref).max() <= 2e-3 * max(np.abs(ref).max(), 1.0)
-    monkeypatch.setenv("ODT_TC_FLAT_PAIR", "0")
     b, _, _, _ = _conv_case(*shape, mode="tc", in_halo=1, out_halo=1, pool=pool)
     np.testing.assert_array_equal(a, b)
 
 
 @pytest.mark.parametrize("shape,kw", [
     ((2, 38, 38, 128, 256, 3, 1, 1), {}),                       # im2col mode
-    ((8, 75, 75, 128, 256, 3, 1, 1), {"residual": True}),       # CTA pairs + residual
+    ((8, 75, 75, 128, 256, 3, 1, 1), {"residual": True}),       # two N tiles + residual
     ((2, 40, 40, 64, 96, 3, 1, 1), {"in_halo": 1}),             # halo-flat mode
     ((2, 26, 26, 512, 28, 1, 1, 1), {"no_out0": True}),         # ragged Cout, only the two pre-activations wanted
 ])
@@ -548,7 +545,7 @@ def test_conv_direct_two_preactivation_outputs(built):
     ((2, 40, 40, 7, 7, 3, 1, 1), {"in_halo": 1, "out_halo": 1}),     # thin flat layer: 1 of 4 K steps issued
     ((2, 40, 40, 28, 7, 1, 1, 1), {}),                               # thin 1x1: 2 of 4
     ((2, 26, 26, 40, 64, 3, 2, 1), {}),                              # 3 of 4, stride 2
-    ((8, 75, 75, 100, 256, 3, 1, 1), {}),                            # second chunk holds 36 channels, CTA pairs
+    ((8, 75, 75, 100, 256, 3, 1, 1), {}),                            # second chunk holds 36 channels, two N tiles
     ((2, 64, 64, 16, 28, 3, 1, 1), {"in_halo": 1, "pool": 2}),       # row-block pooled mode
 ])
 @pytest.mark.parametrize("kskip", ["0", "1"])
@@ -711,7 +708,7 @@ def test_conv_pw_matches_reference(built, monkeypatch, shape, kw):
 
 def test_conv_pw_is_bit_identical_to_the_tensor_core_path_on_exact_inputs(built, monkeypatch):
     """Small-integer activations and weights make every product and partial sum exact in fp16 / fp32, so the
-    CUDA-core pointwise kernel and the tcgen05 kernel must agree bit for bit (same epilogue rounding chain)."""
+    CUDA-core pointwise kernel and the wgmma kernel must agree bit for bit (same epilogue rounding chain)."""
     from odt_b200 import lib as L
     lib = L.load()
     g = torch.Generator(device="cuda").manual_seed(3)

@@ -3,7 +3,7 @@ thread id) executed on the CPU, block by block, warp by warp and phase by phase,
 (tests/native/pw_host.cu) and compared with the oracle's convolution + the epilogue chain of epilogue.cuh:
 staging indices (halo / dense inputs, ragged last group), the round-robin of pixel groups over warps, the
 output-channel passes, fp16 rounding order, residual, the two extra pre-activated outputs (dense and halo layouts), untouched
-padding lanes and halo rings.  The device launch itself needs a B200 (tests/test_gpu_conv.py::test_conv_pw_*)."""
+padding lanes and halo rings.  The device launch itself needs an H100 (tests/test_gpu_conv.py::test_conv_pw_*)."""
 import ctypes as C
 
 import pytest

@@ -2,7 +2,7 @@
 a direct 3x3 SAME convolution: tile = 4 rows x 32 columns (30 outputs per row), one [128 x Cin] activation tile
 per filter row, N = (tap s, channel n), out[p] = P[p-1, s=0] + P[p, s=1] + P[p+1, s=2]; optional 2x2/2 max-pool
 pairing (odd lane, next lane) x (even row, next row).  CPU only: the CUDA kernel itself is opt-in until it has
-run on a B200."""
+run on an H100."""
 import numpy as np
 import pytest
 

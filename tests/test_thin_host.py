@@ -2,7 +2,7 @@
 on the CPU through a test-only harness (tests/native/thin_host.cu, built here with nvcc) and compared with the
 oracle's TF-SAME convolution + the epilogue chain of epilogue.cuh: index arithmetic (halo / no halo, stride 2),
 fp16 rounding order, residual, the two extra pre-activated outputs, untouched padding lanes and halo ring.
-The device launch itself still needs a B200 (tests/test_gpu_conv.py::test_conv_thin_matches_reference)."""
+The device launch itself still needs an H100 (tests/test_gpu_conv.py::test_conv_thin_matches_reference)."""
 import ctypes as C
 import os
 import shutil
@@ -30,7 +30,7 @@ def build_host_harness(name, kernel_src, entry):
     if not os.path.exists(out) or any(os.path.getmtime(f) > os.path.getmtime(out) for f in deps):
         # -fno-strict-aliasing: the kernel reinterprets uint4 registers as __half2 (fine for nvcc's device code,
         # undefined behaviour for the host compiler's optimiser)
-        subprocess.check_call([nvcc, "-O2", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler",
+        subprocess.check_call([nvcc, "-O2", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler",
                                "-fPIC,-fno-strict-aliasing", "-shared", "-o", out, src])
     from odt_b200 import lib as L
     lib = C.CDLL(out)

@@ -1,7 +1,7 @@
 """Index arithmetic of the thin-layer CUDA-core convolution (csrc/conv_thin.cu) restated in numpy: one output
 pixel per "thread", taps addressed as iy = oy*stride - pad_t + r inside a tensor stored with or without a one-pixel
 zero halo, anything outside the stored extent read as zero.  Checked against the oracle's TF-SAME convolution.
-CPU only: the CUDA kernel is opt-in until it has run on a B200."""
+CPU only; the CUDA kernel itself is checked on the GPU (tests/test_gpu_conv.py)."""
 import numpy as np
 import pytest
 
