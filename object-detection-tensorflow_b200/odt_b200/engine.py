@@ -1027,12 +1027,15 @@ class RowsHarness:
         anc = self.tail.det_anchor.cpu().numpy()
         return [anc[b, :cnt[b]].copy() for b in range(self.batch)]
 
-    def loss(self, kind, ground_truth, **kw):
+    def loss(self, kind, ground_truth, return_info=False, **kw):
         """Training-loss forward kernels on the same rows: kind in 'retina' | 'ssd' | 'fcos' | 'yolo'.
-        ground_truth [B,G,5] (y,x,h,w,id) padded with -1.  Returns float32 [B]."""
+        ground_truth [B,G,5] (y,x,h,w,id) padded with -1.  Returns float32 [B]; for 'ssd' with
+        return_info=True also int32 [B,3] = (#positives, #negatives, #mined negatives) per image."""
         gt = torch.as_tensor(np.ascontiguousarray(ground_truth, dtype=np.float32)).to(self.device)
         B, G = gt.shape[0], gt.shape[1]
         assert B == self.batch
+        if return_info and kind != "ssd":
+            raise ValueError("return_info: only the SSD loss reports (#pos, #neg, #mined)")
         st = torch.cuda.current_stream().cuda_stream
         out = torch.zeros(B, dtype=torch.float32, device=self.device)
         p = C.byref(self.tail.p)
@@ -1047,6 +1050,10 @@ class RowsHarness:
                                   device=self.device)
             L.check(self.lib.odt_ssd_loss_fwd(self.head_buf.data_ptr(), p, B, gt.data_ptr(), G, scratch.data_ptr(),
                                               out.data_ptr(), st), "ssd_loss")
+            if return_info:
+                off = self.lib.odt_ssd_loss_info_offset(p, B)
+                info = scratch.view(torch.int32)[off // 4: off // 4 + 3 * B].cpu().numpy().reshape(B, 3)
+                return out.cpu().numpy(), info
         elif kind == "fcos":
             scratch = torch.zeros((self.lib.odt_fcos_loss_scratch_bytes(B) + 3) // 4, dtype=torch.int32,
                                   device=self.device)
