@@ -14,16 +14,19 @@
 //     tiled box with the row dimension second, the pooling window in four lanes of one warp.
 // * B operand (weights, KRSC = K-major): tiled TMA loads [BN x 64], optionally resident in shared
 //   memory for small filter banks.
-// * MMA: wgmma m64nBNk16 (BN <= 128), both operands from shared memory; two consumer warpgroups,
-//   one per 64-row half of the 128-row tile.  A pipeline stage goes back to the producer as soon
-//   as the MMAs that read it have retired (one wgmma group kept in flight).
-// * Epilogue: the accumulators pass through an fp32 tile in shared memory so that every epilogue
-//   lane owns one pixel row, 32 channels at a time: folded bias/BN scale+shift, activation,
-//   residual, up to two extra pre-activated outputs, fused max-pool, fp32 head scatter; 128-bit
-//   global stores.
+// * MMA: wgmma m64nBNk16 (BN <= 128), both operands from shared memory.  Two consumer warpgroups
+//   in a ping-pong schedule: each owns whole 128-row tiles (two m64 accumulator sets, one per
+//   64-row half) and they take alternate tiles of the CTA's list.  An ordering barrier pair makes
+//   their mainloops strictly alternate, so one warpgroup's epilogue runs while the other's MMAs
+//   keep the tensor pipe busy.  A pipeline stage goes back to the producer as soon as the MMAs
+//   that read it have retired (one wgmma group kept in flight).
+// * Epilogue: the accumulators pass, one 32-column slice at a time, through a per-warpgroup fp32
+//   buffer in shared memory so that every epilogue lane owns one pixel row: folded bias/BN
+//   scale+shift, activation, residual, up to two extra pre-activated outputs, fused max-pool,
+//   fp32 head scatter; 128-bit global stores.
 // * Persistent: one CTA per SM, static round-robin tile schedule.  Warp 0 = TMA producer (runs
-//   ahead across tiles), warps 4..11 = the two consumer warpgroups (MMA, then the epilogue of the
-//   same tile; warps 1..3 only pad the producer warpgroup).
+//   ahead across tiles; warps 1..3 only pad the producer warpgroup, which hands most of its
+//   registers to the consumers with setmaxnreg), warps 4..11 = the two consumer warpgroups.
 //
 // ref call sites: tf.nn.conv2d SSD300.py:519; tf.layers.conv2d SSD300.py:524,
 // RetinaNet.py:579,599,609, YOLOv3.py:495, FCOS.py:449,469,479.
@@ -37,15 +40,23 @@ namespace odt {
 
 constexpr int TC_BM = 128;
 constexpr int TC_BK = 64;
-constexpr int TC_MAX_BN = 128;  // N tile (the wgmma accumulators of one 64-row half live in registers)
-constexpr int TC_EPI_WARPS = 8;
-constexpr int TC_THREADS = 128 + 32 * TC_EPI_WARPS;  // producer warpgroup, two consumer warpgroups
-constexpr int TC_EPI_PAR = 7 * 256;               // floats per parameter block: scale/shift/scale2/shift2/column offset/scale3/shift3
-constexpr int TC_EPI_SMEM = 2 * TC_EPI_PAR * 4;   // double-buffered
+constexpr int TC_MAX_BN = 128;  // N tile (a consumer warpgroup holds the 128 x BN fp32 accumulators in registers)
+constexpr int TC_THREADS = 3 * 128;  // producer warpgroup, two consumer warpgroups
+// setmaxnreg split of the 64K-register file: 128 * 40 + 256 * 232 <= 65536
+constexpr int TC_PRODUCER_REGS = 40;
+constexpr int TC_CONSUMER_REGS = 232;
+constexpr int TC_EPI_PAR = 7 * TC_MAX_BN;  // floats per parameter block: scale/shift/scale2/shift2/column offset/scale3/shift3
+// one 32-column slice of a tile's fp32 accumulators at a pitch of 36 floats (row reads of float4 per lane
+// hit distinct banks in every quarter-warp phase)
+constexpr int TC_SLICE_PITCH = 36;
+constexpr int TC_SLICE_FLOATS = TC_BM * TC_SLICE_PITCH;
+constexpr int TC_EPI_SMEM = 2 * (TC_EPI_PAR + TC_SLICE_FLOATS) * 4;  // per consumer warpgroup: parameters + slice
 constexpr int TC_MAX_STAGES = 8;
 constexpr int TC_A_BYTES = TC_BM * TC_BK * 2;  // 16 KiB
 constexpr int TC_SMEM_LIMIT = 232448;          // 227 KiB
-constexpr int tc_acc_bytes(int bn) { return TC_BM * (bn + 4) * 4; }  // staged fp32 accumulator tile
+// named barriers: 1 + g = the 128 threads of consumer warpgroup g; 3 + g = "warpgroup g may start its mainloop"
+constexpr int TC_BAR_EPI = 1;
+constexpr int TC_BAR_ORDER = 3;
 
 struct TcGeom {
   long long M;  // B*OH*OW
@@ -121,12 +132,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (TC_MAX_STAGES + s); };
   const uint32_t wfull_bar = bar_base + 8u * (2 * TC_MAX_STAGES);  // resident weights landed
-  // per-tile epilogue parameters staged in smem: [buf][scale|shift|scale2|shift2|offset|scale3|shift3][256]
-  float* epi_par = reinterpret_cast<float*>(smem_raw + (bar_base + 256u - raw));
-  // the tile's fp32 accumulators, one 128-row tile at a pitch of BN + 4 floats (row reads of float4 per
-  // lane hit distinct banks in every quarter-warp phase)
-  constexpr int ACC_PITCH = BN + 4;
-  float* acc_tile = reinterpret_cast<float*>(smem_raw + (bar_base + 256u + TC_EPI_SMEM - raw));
+  // per consumer warpgroup: the epilogue parameters of its current N tile
+  // [scale|shift|scale2|shift2|offset|scale3|shift3][TC_MAX_BN], then its accumulator slice
+  float* epi_smem = reinterpret_cast<float*>(smem_raw + (bar_base + 256u - raw));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -135,7 +143,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
     for (int s = 0; s < stages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), TC_EPI_WARPS);  // one arrival per consumer warp
+      mbar_init(empty_bar(s), 4);  // one arrival per warp of the consuming warpgroup
     }
     mbar_init(wfull_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -159,7 +167,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   const int num_tiles = g.num_m_tiles * g.num_n_tiles;
   const int kblocks = g.flat ? 3 * g.cchunks : g.R * g.S * g.cchunks;  // pipeline stages per tile
 
-  if (warp == 0) {
+  if (warp < 4) {
+    wg_reg_dealloc<TC_PRODUCER_REGS>();
+    if (warp != 0) return;
     // ===================== TMA producer ======================================
     // The whole warp runs the loop (warp-uniform control flow, operands stay in
     // uniform registers); one elected lane issues the TMA instructions.
@@ -235,27 +245,43 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         }
       }
     }
-  } else if (warp >= 4) {
+  } else {
+    wg_reg_alloc<TC_CONSUMER_REGS>();
     // ===================== consumer warpgroups ===============================
-    // MMA: warpgroup `group` computes rows 64*group .. +63 of the tile over all BN columns.
-    // Epilogue: warp (group, quarter) owns pixel rows 32*quarter .. +31 (one per lane) and the
-    // 32-column chunks j = group, group + 2, ... of the staged accumulator tile.
+    // Warpgroup `group` owns the tiles i = group, group + 2, ... of the CTA's list, all 128 rows
+    // (acc[h] = rows 64*h .. +63).  Its mainloop starts once the other warpgroup has issued every
+    // MMA of the previous tile, so the k-blocks reach the ring's stages in the producer's order.
+    // Epilogue: warp `quarter` of the group owns pixel rows 32*quarter .. +31 (one per lane).
     const int quarter = warp & 3;
     const int group = (warp - 4) >> 2;
-    const int et = threadIdx.x - 128;  // index among the 256 consumer threads
-    int staged_n_tile = -1, pbuf = 0;
+    const int et = threadIdx.x - 128 * (1 + group);  // index among the warpgroup's 128 threads
+    const int epi_bar = TC_BAR_EPI + group;
+    float* par = epi_smem + group * (TC_EPI_PAR + TC_SLICE_FLOATS);
+    float* slice = par + TC_EPI_PAR;
+    constexpr int P = TC_MAX_BN;  // parameter block stride
+    int staged_n_tile = -1;
     int stage = 0;
     uint32_t phase = 0;
     int cc_mma = 0;  // channel chunk of the current k-block (the k-block order ends with the chunk index)
-    float acc[BN / 2];
+    float acc[2][BN / 2];
     if (g.bres) mbar_wait(wfull_bar, 0);
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    int i = 0;  // position of `tile` in the CTA's list
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++i) {
+      if ((i & 1) != group) {  // the other warpgroup's tile: its k-blocks pass through the ring
+        const int adv = stage + kblocks;
+        stage = adv % stages;
+        phase ^= (uint32_t)(adv / stages) & 1u;
+        continue;
+      }
       const int n_tile = tile % g.num_n_tiles;
       const int m_tile = tile / g.num_n_tiles;
+      if (i > 0) named_bar_sync(TC_BAR_ORDER + group, 256);
+      if (quarter == 0) tl_stamp(1 + group, 0, tile);  // mainloop start
       int prev = -1;
       for (int kb = 0; kb < kblocks; ++kb) {
         mbar_wait(full_bar(stage), phase);
-        const uint64_t adesc = make_desc_sw128(a_base + (uint32_t)stage * a_bytes + (uint32_t)group * 64u * 128u);
+        const uint32_t a_stage = a_base + (uint32_t)stage * a_bytes;
+        const uint64_t adesc0 = make_desc_sw128(a_stage), adesc1 = make_desc_sw128(a_stage + 64u * 128u);
         // resident bank: tile ((r*3 + s)*cchunks + cc) with kb = r*cchunks + cc
         const uint64_t bdesc = make_desc_sw128(
             g.bres ? b_base + (uint32_t)((kb / g.cchunks) * 3 * g.cchunks + kb % g.cchunks) * (uint32_t)BN * 128u
@@ -272,27 +298,25 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
           const uint64_t astep = (uint64_t)(g.flat == 2 ? 8 * g.RP : 8);  // rows per tap shift x 128 B >> 4
 #pragma unroll
           for (int s3 = 0; s3 < 3; ++s3)
-            wg_mma_chunk<BN>(acc, adesc + astep * s3, bdesc + bstep * s3, ksteps, (kb | s3) == 0);
+            wg_mma_chunk2<BN>(acc[0], acc[1], adesc0 + astep * s3, adesc1 + astep * s3, bdesc + bstep * s3, ksteps,
+                              (kb | s3) == 0);
         } else {
-          wg_mma_chunk<BN>(acc, adesc, bdesc, ksteps, kb == 0);
+          wg_mma_chunk2<BN>(acc[0], acc[1], adesc0, adesc1, bdesc, ksteps, kb == 0);
         }
         wg_commit();
         wg_wait<1>();  // the previous k-block's MMAs have retired: its stage goes back to the producer
         if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
         prev = stage;
-        if (kb == 0 && quarter == 0) tl_stamp(1 + group, 0, tile);  // first stage of the tile issued
         if (++stage == stages) {
           stage = 0;
           phase ^= 1u;
         }
       }
+      // every MMA of this tile is issued: the other warpgroup's mainloop may start
+      if (tile + (int)gridDim.x < num_tiles) named_bar_arrive(TC_BAR_ORDER + (group ^ 1), 256);
       wg_wait<0>();
       if (lane == 0) mbar_arrive(empty_bar(prev));
       if (quarter == 0) tl_stamp(1 + group, 1, tile);  // accumulators complete
-      // accumulators -> shared memory, once every consumer warp has finished reading the previous tile
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      wg_acc_to_smem<BN>(acc, acc_tile, ACC_PITCH, 64 * group);
-      asm volatile("bar.sync 1, 256;" ::: "memory");
 
       const long long m = (long long)m_tile * TC_BM + quarter * 32 + lane;
       bool row_ok;
@@ -325,25 +349,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         pix = row_ok ? (int)(m - (long long)img * g.ohw) : 0;
       }
       const int n0 = n_tile * BN;
-      // stage the per-channel parameters of this N tile once (broadcast reads later);
+      // the per-channel parameters of this N tile are staged once (broadcast reads later);
       // consecutive tiles of single-N-tile layers reuse them
-      if (n_tile != staged_n_tile) {
-        staged_n_tile = n_tile;
-        pbuf ^= 1;
-        float* wpar = epi_par + pbuf * TC_EPI_PAR;
-        const int c = et;
-        const int n = n0 + c;
-        const bool ok = c < BN && n < e.Cout;
-        wpar[c] = (ok && e.scale) ? __ldg(e.scale + n) : 1.f;
-        wpar[256 + c] = (ok && e.shift) ? __ldg(e.shift + n) : 0.f;
-        wpar[512 + c] = (ok && e.scale2) ? __ldg(e.scale2 + n) : 1.f;
-        wpar[768 + c] = (ok && e.shift2) ? __ldg(e.shift2 + n) : 0.f;
-        reinterpret_cast<int*>(wpar)[1024 + c] = ok ? regroup(e, n) : 0;
-        wpar[1280 + c] = (ok && e.scale3) ? __ldg(e.scale3 + n) : 1.f;
-        wpar[1536 + c] = (ok && e.shift3) ? __ldg(e.shift3 + n) : 0.f;
-        asm volatile("bar.sync 3, 256;" ::: "memory");
-      }
-      const float* par = epi_par + pbuf * TC_EPI_PAR;
+      const bool new_par = n_tile != staged_n_tile;
+      staged_n_tile = n_tile;
       long long o0_row = (long long)img * e.out0_img_stride;
       if (g.out_halo) {
         const int oy = pix / g.OW, ox = pix - oy * g.OW;
@@ -353,14 +362,30 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
       }
       const long long o1_row = aux_row(e.out1_img_stride, e.out1_pix_stride, e.out1_halo, g.OW, img, pix);
       const long long o2_row = aux_row(e.out2_img_stride, e.out2_pix_stride, e.out2_halo, g.OW, img, pix);
-      const float* my_acc = acc_tile + (quarter * 32 + lane) * ACC_PITCH;
-      for (int j = group; j < BN / 32; j += 2) {
+      const float* my_acc = slice + (quarter * 32 + lane) * TC_SLICE_PITCH;
+      for (int j = 0; j < BN / 32; ++j) {
         const int nb = n0 + j * 32;
         if (nb >= e.Cout) break;  // fully padded chunk (uniform)
+        // every lane of the warpgroup has finished reading the previous slice and, on a new tile, the parameters
+        named_bar_sync(epi_bar, 128);
+        if (j == 0 && new_par) {
+          const int n = n0 + et;
+          const bool ok = et < BN && n < e.Cout;
+          par[et] = (ok && e.scale) ? __ldg(e.scale + n) : 1.f;
+          par[P + et] = (ok && e.shift) ? __ldg(e.shift + n) : 0.f;
+          par[2 * P + et] = (ok && e.scale2) ? __ldg(e.scale2 + n) : 1.f;
+          par[3 * P + et] = (ok && e.shift2) ? __ldg(e.shift2 + n) : 0.f;
+          reinterpret_cast<int*>(par)[4 * P + et] = ok ? regroup(e, n) : 0;
+          par[5 * P + et] = (ok && e.scale3) ? __ldg(e.scale3 + n) : 1.f;
+          par[6 * P + et] = (ok && e.shift3) ? __ldg(e.shift3 + n) : 0.f;
+        }
+        wg_acc_slice_to_smem<BN>(acc[0], j, slice, TC_SLICE_PITCH, 0);
+        wg_acc_slice_to_smem<BN>(acc[1], j, slice, TC_SLICE_PITCH, 64);
+        named_bar_sync(epi_bar, 128);
         uint32_t r[32];
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          const uint4 t = *reinterpret_cast<const uint4*>(my_acc + j * 32 + 4 * i);
+          const uint4 t = *reinterpret_cast<const uint4*>(my_acc + 4 * i);
           r[4 * i + 0] = t.x;
           r[4 * i + 1] = t.y;
           r[4 * i + 2] = t.z;
@@ -371,7 +396,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
           // the window's four lanes (vertical neighbour = lane^1, horizontal = lane^RP); each
           // of the four lanes stores one 8-channel quarter of the pooled pixel
           const float4* ps = reinterpret_cast<const float4*>(par + j * 32);
-          const float4* ph4 = reinterpret_cast<const float4*>(par + 256 + j * 32);
+          const float4* ph4 = reinterpret_cast<const float4*>(par + P + j * 32);
           uint4 packed[4];
           __half2* ph = reinterpret_cast<__half2*>(packed);
 #pragma unroll
@@ -397,7 +422,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
             *reinterpret_cast<uint4*>(reinterpret_cast<__half*>(e.out0) + pool_row + nb + 8 * pool_q) = sel;
         } else if (g.fast_store && nb + 32 <= g.fast_cols) {
           const float4* ps = reinterpret_cast<const float4*>(par + j * 32);
-          const float4* ph4 = reinterpret_cast<const float4*>(par + 256 + j * 32);
+          const float4* ph4 = reinterpret_cast<const float4*>(par + P + j * 32);
           float v[32];
 #pragma unroll
           for (int i = 0; i < 8; ++i) {
@@ -434,8 +459,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
               for (int qd = 0; qd < 4; ++qd) op[qd] = packed[qd];
             }
             if (e.out1) {
-              const float4* ps2 = reinterpret_cast<const float4*>(par + 512 + j * 32);
-              const float4* ph2 = reinterpret_cast<const float4*>(par + 768 + j * 32);
+              const float4* ps2 = reinterpret_cast<const float4*>(par + 2 * P + j * 32);
+              const float4* ph2 = reinterpret_cast<const float4*>(par + 3 * P + j * 32);
               uint4 packed1[4];
               __half2* p1 = reinterpret_cast<__half2*>(packed1);
 #pragma unroll
@@ -453,8 +478,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
               for (int qd = 0; qd < 4; ++qd) op[qd] = packed1[qd];
             }
             if (e.out2) {
-              const float4* ps3 = reinterpret_cast<const float4*>(par + 1280 + j * 32);
-              const float4* ph3 = reinterpret_cast<const float4*>(par + 1536 + j * 32);
+              const float4* ps3 = reinterpret_cast<const float4*>(par + 5 * P + j * 32);
+              const float4* ph3 = reinterpret_cast<const float4*>(par + 6 * P + j * 32);
               uint4 packed2[4];
               __half2* p2 = reinterpret_cast<__half2*>(packed2);
 #pragma unroll
@@ -476,21 +501,21 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
           // generic path: fp32 head outputs scattered into the candidate rows,
           // channel regrouping, ragged Cout; parameters come from shared memory
           const float* ps = par + j * 32;
-          const int* pofs = reinterpret_cast<const int*>(par) + 1024 + j * 32;
+          const int* pofs = reinterpret_cast<const int*>(par) + 4 * P + j * 32;
           const int nvalid = min(32, e.Cout - nb);
           if (g.head_mode) {
             // head convolutions: fp32 scatter into the candidate rows.  The staged accumulator
-            // tile is read column-wise, so the warp writes one row per instruction with the
+            // slice is read column-wise, so the warp writes one row per instruction with the
             // lanes on consecutive channels (4-5 sectors per request instead of 32).
-            const float* acol = acc_tile + (quarter * 32) * ACC_PITCH + j * 32 + lane;
-            const float sc = ps[lane], sh = ps[256 + lane];
+            const float* acol = slice + (quarter * 32) * TC_SLICE_PITCH + lane;
+            const float sc = ps[lane], sh = ps[P + lane];
             const int my_ofs = pofs[lane];
             const long long my_row = row_ok ? o0_row : -1;
             float* obase = reinterpret_cast<float*>(e.out0);
 #pragma unroll 4
             for (int rr = 0; rr < 32; ++rr) {
               const long long orow_r = __shfl_sync(0xffffffffu, my_row, rr);
-              const float val = apply_act(fmaf(acol[rr * ACC_PITCH], sc, sh), e.act);
+              const float val = apply_act(fmaf(acol[rr * TC_SLICE_PITCH], sc, sh), e.act);
               if (orow_r >= 0 && lane < nvalid) obase[orow_r + my_ofs] = val;
             }
           } else {
@@ -498,7 +523,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
             for (int i = 0; i < 32; ++i) {
               if (i >= nvalid) break;
               const int n = nb + i;
-              float v = apply_act(fmaf(__uint_as_float(r[i]), ps[i], ps[256 + i]), e.act);
+              float v = apply_act(fmaf(__uint_as_float(r[i]), ps[i], ps[P + i]), e.act);
               const long long o0 = o0_row + pofs[i];
               if (e.residual) v += __half2float(reinterpret_cast<const __half*>(e.residual)[o0]);
               if (e.out0) {
@@ -512,10 +537,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
               }
               if (e.out1)
                 reinterpret_cast<__half*>(e.out1)[o1_row + n] =
-                    __float2half_rn(apply_act(fmaf(v, ps[512 + i], ps[768 + i]), e.act2));
+                    __float2half_rn(apply_act(fmaf(v, ps[2 * P + i], ps[3 * P + i]), e.act2));
               if (e.out2)
                 reinterpret_cast<__half*>(e.out2)[o2_row + n] =
-                    __float2half_rn(apply_act(fmaf(v, ps[1280 + i], ps[1536 + i]), e.act3));
+                    __float2half_rn(apply_act(fmaf(v, ps[5 * P + i], ps[6 * P + i]), e.act3));
             }
           }
         }
@@ -600,11 +625,14 @@ int check_conv_params(const odt_conv_params* p) {
 using namespace odt;
 
 // N tile of an im2col-mode layer from a two-term cost model:
-//   time ~ rounds * (kblocks * (128 + 4*BN) + 2000 + 8*BN),
+//   time ~ rounds * max(mma, epi) + epi,   mma = kblocks * (128 + 4*BN),   epi = 2000 + 8*BN,
 //   4*BN    = clocks of the 128 x BN x 64 multiply-adds of one K block at the dense fp16 wgmma rate
 //             (2048 FMA/clk/SM), 128 = per-K-block barrier and issue overhead,
-//   2000 + 8*BN = the epilogue, which the consumer warpgroups run between two tiles,
+//   epi     = the epilogue of one tile; with the ping-pong consumers it runs under the other
+//             warpgroup's mainloop, so a round costs the longer of the two and only the CTA's
+//             last epilogue is exposed,
 //   rounds  = tiles per CTA of the slowest SM.
+// The constants are estimates from the instruction counts, not measured on the H100.
 // Small-M layers (FPN P5-P7 towers, SSD extras) come out with narrow tiles spread over many
 // SMs, large ones with 128-wide tiles.
 static int pick_bn(int cout_pad, int m_tiles, int kblocks) {
@@ -614,7 +642,8 @@ static int pick_bn(int cout_pad, int m_tiles, int kblocks) {
     if (cout_pad % bn != 0) continue;
     const long long units = (long long)m_tiles * (cout_pad / bn);
     const long long rounds = (units + kNumSMs - 1) / kNumSMs;
-    const long long cost = rounds * ((long long)kblocks * (128 + 4 * bn) + 2000 + 8 * bn);
+    const long long mma = (long long)kblocks * (128 + 4 * bn), epi = 2000 + 8 * bn;
+    const long long cost = rounds * (mma > epi ? mma : epi) + epi;
     if (best < 0 || cost < best) {  // ties keep the wider tile (visited first)
       best = cost;
       best_bn = bn;
@@ -731,8 +760,8 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
   }
   stage_bytes = g.a_bytes + g.b_bytes;
   g.head_mode = (p->out0 && p->out0_dtype == ODT_F32 && !p->residual && !p->out1 && !p->out2) ? 1 : 0;
-  // barriers + 1024-byte alignment slack, epilogue parameters, staged accumulator tile
-  const int fixed_bytes = 2048 + TC_EPI_SMEM + tc_acc_bytes(g.BN);
+  // barriers + 1024-byte alignment slack, per consumer warpgroup: epilogue parameters + accumulator slice
+  const int fixed_bytes = 2048 + TC_EPI_SMEM;
   // small filter banks of the flat modes stay resident in shared memory if at least three
   // activation stages still fit beside them
   const long long wres = 9ll * g.cchunks * g.BN * 128;

@@ -189,17 +189,63 @@ __device__ __forceinline__ void wg_mma_chunk(float* d, uint64_t adesc, uint64_t 
   }
 }
 
-// The warpgroup's m64 x N fragment -> fp32 rows row0 .. row0+63 of a shared-memory tile (`pitch` floats per row)
+// The same K steps for the two 64-row halves of a 128-row tile (accumulators d0 / d1, A descriptors a0 / a1, one
+// B operand), interleaved step by step so that the tensor pipe always has an MMA whose accumulator is not the
+// one it is still writing.  Each half sees exactly the K order of wg_mma_chunk.
 template <int N>
-__device__ __forceinline__ void wg_acc_to_smem(const float* d, float* tile, int pitch, int row0) {
+__device__ __forceinline__ void wg_mma_chunk2(float* d0, float* d1, uint64_t a0, uint64_t a1, uint64_t bdesc,
+                                              int ksteps, bool first) {
+  if (ksteps == 4) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      wg_mma_f16<N>(d0, a0 + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (uint32_t)(!first || k != 0));
+      wg_mma_f16<N>(d1, a1 + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (uint32_t)(!first || k != 0));
+    }
+  } else {
+    for (int k = 0; k < ksteps; ++k) {
+      wg_mma_f16<N>(d0, a0 + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (uint32_t)(!first || k != 0));
+      wg_mma_f16<N>(d1, a1 + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (uint32_t)(!first || k != 0));
+    }
+  }
+}
+
+// Columns 32*j .. 32*j+31 of the warpgroup's m64 x N fragment -> columns 0..31 of rows row0 .. row0+63 of a
+// shared-memory slice.  `j` may be a run-time value: the fragment registers are selected by an unrolled
+// compare, so they never go through local memory.
+template <int N>
+__device__ __forceinline__ void wg_acc_slice_to_smem(const float* d, int j, float* slice, int pitch, int row0) {
   const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
-  float* r0 = tile + (row0 + 16 * w + (l >> 2)) * pitch + 2 * (l & 3);
+  float* r0 = slice + (row0 + 16 * w + (l >> 2)) * pitch + 2 * (l & 3);
   float* r8 = r0 + 8 * pitch;
 #pragma unroll
-  for (int i = 0; i < N / 8; ++i) {
-    *reinterpret_cast<float2*>(r0 + 8 * i) = make_float2(d[4 * i], d[4 * i + 1]);
-    *reinterpret_cast<float2*>(r8 + 8 * i) = make_float2(d[4 * i + 2], d[4 * i + 3]);
+  for (int jj = 0; jj < N / 32; ++jj) {
+    if (jj == j) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const float* f = d + 4 * (4 * jj + i);
+        *reinterpret_cast<float2*>(r0 + 8 * i) = make_float2(f[0], f[1]);
+        *reinterpret_cast<float2*>(r8 + 8 * i) = make_float2(f[2], f[3]);
+      }
+    }
   }
+}
+
+// Register reallocation between warpgroups (every warp of the warpgroup executes it)
+template <int R>
+__device__ __forceinline__ void wg_reg_dealloc() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+}
+template <int R>
+__device__ __forceinline__ void wg_reg_alloc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
+}
+
+// Named barriers (ids 1..15; `count` threads, a multiple of 32)
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
 // K-major, 128-byte swizzle shared-memory matrix descriptor (sm_90 wgmma format): 8-row core-matrix groups

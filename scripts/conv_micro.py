@@ -12,8 +12,8 @@ from odt_b200 import lib as L  # noqa: E402
 from odt_b200.engine import same_pad  # noqa: E402
 
 
-def main():
-    a = [int(v) for v in sys.argv[1:]]
+def setup(a):
+    """Inputs and parameters of one layer; returns (lib, launch(), FLOP per launch, reps)."""
     B, H, W, Cin, Cout, k, stride = a[:7]
     pool = a[7] if len(a) > 7 else 0
     ih = a[8] if len(a) > 8 else 1
@@ -62,17 +62,31 @@ def main():
     if "n" in extra:
         p.out0 = None
     st = torch.cuda.current_stream().cuda_stream
-    for _ in range(3):
+
+    def launch():
         L.check(lib.odt_conv2d_f16_tc(x.data_ptr(), w.data_ptr(), C.byref(p), st), "conv")
+
+    launch.keep = (x, w, y, shift, keep)
+    return lib, launch, 2.0 * B * OH * OW * Cout * k * k * Cin, reps
+
+
+def main():
+    a = [int(v) for v in sys.argv[1:]]
+    lib, launch, fl, reps = setup(a)
+    pool = a[7] if len(a) > 7 else 0
+    ih = a[8] if len(a) > 8 else 1
+    oh = a[9] if len(a) > 9 else 1
+    extra = os.environ.get("ODT_MICRO_EXTRA", "")
+    for _ in range(3):
+        launch()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     torch.cuda.synchronize()
     e0.record()
     for _ in range(reps):
-        L.check(lib.odt_conv2d_f16_tc(x.data_ptr(), w.data_ptr(), C.byref(p), st), "conv")
+        launch()
     e1.record()
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / reps
-    fl = 2.0 * B * OH * OW * Cout * k * k * Cin
     print("conv %s pool=%d halo=%d/%d extra=%r thin/tapn launches %d/%d: %.4f ms  %.1f TFLOP/s" % (
         a[:7], pool, ih, oh, extra, lib.odt_debug_thin_launches(), lib.odt_debug_tapn_launches(), ms, fl / ms / 1e9))
 

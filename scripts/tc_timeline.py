@@ -1,0 +1,95 @@
+#!/usr/bin/env python
+"""Per-warpgroup timeline of CTA 0 of conv_tc_kernel (debug build, -DODT_TC_TIMELINE): each consumer warpgroup's
+mainloop (first MMA issue -> accumulators complete) and epilogue (-> last store issued), and the share of the kernel
+during which no warpgroup has MMAs in flight, i.e. the epilogue time the ping-pong schedule leaves exposed.
+usage (on a GPU box): tc_timeline.py B H W Cin Cout k stride [pool] [in_halo] [out_halo]   (conv_micro.py's arguments)"""
+import os
+import subprocess
+import sys
+
+import numpy as np
+import torch
+
+ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
+PKG = os.path.join(ROOT, "object-detection-tensorflow_b200")
+sys.path.insert(0, ROOT)
+sys.path.insert(0, PKG)
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import __graft_entry__ as ge  # noqa: E402
+
+EVENTS = ("mainloop start", "accumulators complete", "epilogue done")
+
+
+def build_debug_lib():
+    ge.build()
+    csrc = os.path.join(PKG, "csrc")
+    obj = os.path.join(csrc, "conv_tc_tl.o")
+    out = os.path.join(PKG, "odt_b200", "libodt_b200_tl.so")
+    subprocess.check_call(["nvcc"] + ge.NVCC_FLAGS + ["-DODT_TC_TIMELINE", "-c", "conv_tc.cu", "-o", obj], cwd=csrc)
+    objs = [os.path.join(csrc, s[:-3] + ".o") for s in ge.SRCS if s != "conv_tc.cu"] + [obj]
+    subprocess.check_call(["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", out] + objs + ["-ldl"],
+                          cwd=csrc)
+    return out
+
+
+def union_length(intervals):
+    total, end = 0, None
+    for a, b in sorted(intervals):
+        if end is None or a > end:
+            total += b - a
+            end = b
+        elif b > end:
+            total += b - end
+            end = b
+    return total
+
+
+def main():
+    import ctypes as C
+    from odt_b200 import lib as L
+    L.LIB_PATH = build_debug_lib()
+    L._lib = None  # __graft_entry__.build() has loaded the product library: bind the debug build instead
+    import conv_micro
+    args = [int(v) for v in sys.argv[1:]]
+    lib, launch, fl, _ = conv_micro.setup(args)
+    lib.odt_debug_tc_timeline.restype = C.c_int
+    lib.odt_debug_tc_timeline.argtypes = [C.c_void_p, C.c_int]
+    for _ in range(3):
+        launch()
+    torch.cuda.synchronize()
+    cap = 1 << 16
+    buf = torch.zeros(2 * cap, dtype=torch.int64, device="cuda")
+    L.check(lib.odt_debug_tc_timeline(buf.data_ptr(), cap), "timeline")
+    launch()
+    torch.cuda.synchronize()
+    L.check(lib.odt_debug_tc_timeline(None, 0), "timeline off")
+    raw = buf.cpu().numpy().view(np.uint64).reshape(-1, 2)
+    raw = raw[raw[:, 0] != 0]
+    clk = raw[:, 0].astype(np.int64)
+    role = (raw[:, 1] >> np.uint64(56)).astype(int)
+    ev = ((raw[:, 1] >> np.uint64(48)) & np.uint64(0xFF)).astype(int)
+    tile = (raw[:, 1] & np.uint64(0xFFFFFFFF)).astype(int)
+    t0, t1 = int(clk.min()), int(clk.max())
+    print("conv %s: CTA 0, clocks since its first stamp; kernel span %d clk" % (args[:7], t1 - t0))
+    stamps = {}
+    for c, r, e, t in zip(clk, role, ev, tile):
+        stamps[(r, t, e)] = int(c) - t0
+    busy = []
+    for g in (0, 1):
+        tiles = sorted({t for (r, t, _) in stamps if r == 1 + g})
+        print("-- warpgroup %d: %d tiles" % (g, len(tiles)))
+        for t in tiles:
+            a, b, c = (stamps.get((1 + g, t, e)) for e in range(3))
+            print("tile %6d: mainloop %8s .. %8s (%6s clk)  epilogue .. %8s (%6s clk)" % (
+                t, a, b, (b - a) if None not in (a, b) else "-", c, (c - b) if None not in (b, c) else "-"))
+            if None not in (a, b):
+                busy.append((a, b))
+    first = min(a for a, _ in busy) if busy else 0
+    span = (t1 - t0) - first
+    idle = span - union_length(busy)
+    print("no warpgroup with MMAs in flight: %d of %d clk after the first mainloop start (%.1f %%)" % (
+        idle, span, 100.0 * idle / max(span, 1)))
+
+
+if __name__ == "__main__":
+    main()
