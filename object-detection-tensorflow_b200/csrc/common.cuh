@@ -43,16 +43,16 @@ template <typename T>
 struct Elem;
 template <>
 struct Elem<float> {
-  static __device__ __forceinline__ float ld(const float* p) { return *p; }
-  static __device__ __forceinline__ void st(float* p, float v) { *p = v; }
+  static __host__ __device__ __forceinline__ float ld(const float* p) { return *p; }
+  static __host__ __device__ __forceinline__ void st(float* p, float v) { *p = v; }
 };
 template <>
 struct Elem<__half> {
-  static __device__ __forceinline__ float ld(const __half* p) { return __half2float(*p); }
-  static __device__ __forceinline__ void st(__half* p, float v) { *p = __float2half_rn(v); }
+  static __host__ __device__ __forceinline__ float ld(const __half* p) { return __half2float(*p); }
+  static __host__ __device__ __forceinline__ void st(__half* p, float v) { *p = __float2half_rn(v); }
 };
 
-__device__ __forceinline__ float apply_act(float v, int act) {
+__host__ __device__ __forceinline__ float apply_act(float v, int act) {
   if (act == ODT_ACT_RELU) return fmaxf(v, 0.f);
   if (act == ODT_ACT_LEAKY) return fmaxf(v, 0.1f * v);
   return v;
@@ -69,6 +69,24 @@ __device__ __forceinline__ void pdl_launch_dependents() {
 }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 bool pdl_enabled();   // ODT_PDL=0 disables the launch attribute (api.cu)
+
+// Launch with the programmatic-serialisation attribute unless ODT_PDL=0.  For kernels that call pdl_wait() before
+// they touch what the previous kernel in the stream wrote.
+template <typename... KArgs, typename... Args>
+cudaError_t launch_pdl(void (*kern)(KArgs...), unsigned grid, int block, int smem, cudaStream_t st, Args... args) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(block);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  return cudaLaunchKernelEx(&cfg, kern, args...);
+}
+
 bool flat_enabled();  // ODT_TC_FLAT=0 disables the halo-flat 3x3 path (A/B measurements)
 bool kskip_enabled();  // ODT_TC_KSKIP=1: do not issue the all-zero 16-deep K steps of thin layers (Cin padded to 64)
 int thin_mode();       // ODT_TC_THIN: 1 = very thin layers (Cin, Cout <= 32, few multiply-adds per pixel) go through the

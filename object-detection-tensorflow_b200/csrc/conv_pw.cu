@@ -14,9 +14,9 @@
 //      issued before the first use;
 //   2. compute, COT output channels per pass: lane = pixel, the filter bank as fp32 [cin][cout] in shared memory
 //      (filled once per block) read by warp-broadcast 128-bit loads (4 FMA per LDS), fp32 accumulation;
-//   3. the accumulators are parked in the warp's slice and the epilogue (epilogue.cuh semantics: scale / shift / act,
-//      residual, fp16 rounding, up to two extra pre-activated outputs) runs with consecutive lanes on consecutive
-//      16-byte sectors again, so residual loads and all stores are full-sector and row-contiguous.
+//   3. the accumulators are parked in the warp's slice and epilogue.cuh's fused fp16 output step (epi_store_f16<1>)
+//      runs with consecutive lanes on consecutive 16-byte sectors again, so residual loads and all stores are
+//      full-sector and row-contiguous.
 // The grid is persistent (<= 2 blocks per SM, groups dealt round-robin to the warps).  The filter bank and the affine
 // parameters are constants of the network: they are filled BEFORE griddepcontrol.wait, i.e. under the tail of the
 // producer kernel (programmatic dependent launch).
@@ -27,12 +27,6 @@
 #include <string.h>
 
 #include "epilogue.cuh"
-
-#ifdef __CUDA_ARCH__
-#define ODT_PW_LDG(p) __ldg(p)
-#else
-#define ODT_PW_LDG(p) (*(p))
-#endif
 
 namespace odt {
 
@@ -60,12 +54,6 @@ struct PwGeom {
   int off_par, off_warps, slice_bytes, off_x, off_y, smem_bytes;
 };
 
-__host__ __device__ __forceinline__ float pw_act(float v, int act) {  // = apply_act (common.cuh), host-callable
-  if (act == ODT_ACT_RELU) return fmaxf(v, 0.f);
-  if (act == ODT_ACT_LEAKY) return fmaxf(v, 0.1f * v);
-  return v;
-}
-
 // One warp's private staging area.  Row offsets are kept in units of 16-byte sectors (8 fp16 elements).
 struct PwSlice {
   int* rows;  // [4][32]: sector offset of the pixel's row in in / out0 (= residual) / out1 / out2; in < 0: no pixel
@@ -82,7 +70,7 @@ __host__ __device__ __forceinline__ PwSlice pw_slice(unsigned char* base, const 
   return s;
 }
 
-// block prologue (before the grid dependency resolves): filter bank fp32 [cin][cop] and affine parameters [6][cop]
+// block prologue (before the grid dependency resolves): filter bank fp32 [cin][cop] and epi_param's six rows [6][cop]
 __host__ __device__ __forceinline__ void pw_fill(int tid, unsigned char* base, const __half* wgt, const PwGeom& g,
                                                  const Epi& e) {
   float* ws = reinterpret_cast<float*>(base);
@@ -90,17 +78,12 @@ __host__ __device__ __forceinline__ void pw_fill(int tid, unsigned char* base, c
   for (int i = tid; i < g.ci8 * g.cop; i += PW_THREADS) {
     const int n = i % g.cop, c8 = i / g.cop;  // consecutive threads: consecutive filters (conflict-free stores)
     uint4 raw = make_uint4(0u, 0u, 0u, 0u);
-    if (n < g.Cout) raw = ODT_PW_LDG(reinterpret_cast<const uint4*>(wgt + (long long)n * g.w_ld) + c8);
+    if (n < g.Cout) raw = ODT_LDG(reinterpret_cast<const uint4*>(wgt + (long long)n * g.w_ld) + c8);
     const __half* h = reinterpret_cast<const __half*>(&raw);
 #pragma unroll
     for (int j = 0; j < 8; ++j) ws[(c8 * 8 + j) * g.cop + n] = (c8 * 8 + j < g.Cin) ? __half2float(h[j]) : 0.f;
   }
-  for (int i = tid; i < 6 * g.cop; i += PW_THREADS) {
-    const int which = i / g.cop, n = i % g.cop;
-    const float* src = which == 0 ? e.scale : which == 1 ? e.shift : which == 2 ? e.scale2 : which == 3 ? e.shift2
-                       : which == 4 ? e.scale3 : e.shift3;
-    par[i] = (n < g.Cout && src) ? ODT_PW_LDG(src + n) : ((which & 1) ? 0.f : 1.f);
-  }
+  for (int i = tid; i < 6 * g.cop; i += PW_THREADS) par[i] = epi_param(e, i / g.cop, i % g.cop);
 }
 
 // phase 1: where the group's pixels live in the four tensors (lane = pixel); 32-bit arithmetic (pw_plan bounds M)
@@ -140,7 +123,7 @@ __host__ __device__ __forceinline__ void pw_load(int lane, const PwSlice& s, con
         const int px = (i * g.ci8_inv) >> 16, ch = i - px * g.ci8;  // exact for i < 512 (pw_plan)
         const int r = s.rows[px];
         dst[u] = px * g.xs16 + ch;
-        if (r >= 0) v[u] = ODT_PW_LDG(in16 + r + ch);
+        if (r >= 0) v[u] = ODT_LDG(in16 + r + ch);
       }
     }
 #pragma unroll
@@ -215,7 +198,7 @@ __host__ __device__ __forceinline__ void pw_items(int lane, int pass, const PwSl
     int sec = 0;
     const int px = pw_item(lane, u, spp, s.rows, &sec);
     it.rs[u] = make_uint4(0u, 0u, 0u, 0u);
-    if (px >= 0 && res16) it.rs[u] = ODT_PW_LDG(res16 + s.rows[32 + px] + pass * SPP + sec);
+    if (px >= 0 && res16) it.rs[u] = ODT_LDG(res16 + s.rows[32 + px] + pass * SPP + sec);
   }
 }
 
@@ -230,61 +213,16 @@ __host__ __device__ __forceinline__ void pw_store(int lane, int pass, const PwSl
                                                   const PwGeom& g, const Epi& e, const PwItems<COT>& it) {
   constexpr int SPP = COT / 8;
   const int spp = (g.co8 - pass * SPP) < SPP ? (g.co8 - pass * SPP) : SPP;
-  const float *sc1 = par, *sh1 = par + g.cop, *sc2 = par + 2 * g.cop, *sh2 = par + 3 * g.cop, *sc3 = par + 4 * g.cop,
-              *sh3 = par + 5 * g.cop;
 #pragma unroll
   for (int u = 0; u < SPP; ++u) {
     int sec = 0;
     const int px = pw_item(lane, u, spp, s.rows, &sec);
     if (px < 0) continue;
     const int n8 = pass * SPP + sec;
-    const int c0 = n8 * 8;  // first channel of the sector
-    float v[8], sc[8], sh[8];
-    pw_ld8(s.y + px * (COT + 4) + (c0 - pass * COT), v);
-    pw_ld8(sc1 + c0, sc);
-    pw_ld8(sh1 + c0, sh);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = pw_act(fmaf(v[i], sc[i], sh[i]), e.act);
-    if (e.residual) {
-      const __half2* h = reinterpret_cast<const __half2*>(&it.rs[u]);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float2 f = __half22float2(h[i]);
-        v[2 * i] += f.x;
-        v[2 * i + 1] += f.y;
-      }
-    }
-    uint4 packed;
-    __half2* ph = reinterpret_cast<__half2*>(&packed);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) ph[i] = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-    if (e.out0) reinterpret_cast<uint4*>(e.out0)[s.rows[32 + px] + n8] = packed;
-    if (e.out1) {
-      pw_ld8(sc2 + c0, sc);
-      pw_ld8(sh2 + c0, sh);
-      uint4 p1;
-      __half2* q = reinterpret_cast<__half2*>(&p1);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float2 f = __half22float2(ph[i]);  // the consumer sees the rounded value
-        q[i] = __floats2half2_rn(pw_act(fmaf(f.x, sc[2 * i], sh[2 * i]), e.act2),
-                                 pw_act(fmaf(f.y, sc[2 * i + 1], sh[2 * i + 1]), e.act2));
-      }
-      reinterpret_cast<uint4*>(e.out1)[s.rows[64 + px] + n8] = p1;
-    }
-    if (e.out2) {
-      pw_ld8(sc3 + c0, sc);
-      pw_ld8(sh3 + c0, sh);
-      uint4 p2;
-      __half2* q = reinterpret_cast<__half2*>(&p2);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float2 f = __half22float2(ph[i]);
-        q[i] = __floats2half2_rn(pw_act(fmaf(f.x, sc[2 * i], sh[2 * i]), e.act3),
-                                 pw_act(fmaf(f.y, sc[2 * i + 1], sh[2 * i + 1]), e.act3));
-      }
-      reinterpret_cast<uint4*>(e.out2)[s.rows[96 + px] + n8] = p2;
-    }
+    float v[8];
+    pw_ld8(s.y + px * (COT + 4) + (n8 * 8 - pass * COT), v);
+    epi_store_f16<1>(e, v, par + n8 * 8, g.cop, [&](int) { return it.rs[u]; }, 8ll * (s.rows[32 + px] + n8),
+                     8ll * (s.rows[64 + px] + n8), 8ll * (s.rows[96 + px] + n8));
   }
 }
 
@@ -337,18 +275,8 @@ static int pw_plan(const void* in, const odt_conv_params* p, bool force, PwGeom*
   if (ci8 > 16 || co8 > 32) return ODT_ERR_UNSUPPORTED;
   const int cot = co8 <= 1 ? 8 : co8 <= 2 ? 16 : 32;
   const int passes = (co8 * 8 + cot - 1) / cot;
-  auto aligned = [&](const void* ptr, long long img, int pix) {
-    return ((uintptr_t)ptr & 15) == 0 && img % 8 == 0 && pix % 8 == 0 && pix >= co8 * 8;
-  };
   const bool io_ok = ((uintptr_t)in & 15) == 0 && p->in_ld % 8 == 0 && p->in_ld >= ci8 * 8 && p->w_ld % 8 == 0 &&
-                     p->w_ld >= ci8 * 8 && (p->out0 || p->out1 || p->out2) &&
-                     (!p->out0 || (p->out0_dtype == ODT_F16 && aligned(p->out0, p->out0_img_stride, p->out0_pix_stride))) &&
-                     (!p->out1 || aligned(p->out1, p->out1_img_stride, p->out1_pix_stride)) &&
-                     (!p->out2 || aligned(p->out2, p->out2_img_stride, p->out2_pix_stride)) &&
-                     // the residual shares out0's addressing (strides / halo), whether or not out0 itself is stored
-                     (!p->residual || (((uintptr_t)p->residual & 15) == 0 && p->out0_img_stride % 8 == 0 &&
-                                       p->out0_pix_stride % 8 == 0 && p->out0_pix_stride >= co8 * 8 &&
-                                       (p->out0 || p->out0_dtype == ODT_F16)));
+                     p->w_ld >= ci8 * 8 && (p->out0 || p->out1 || p->out2) && f16_sector_outputs_ok(p, co8 * 8);
   if (!io_ok) return ODT_ERR_UNSUPPORTED;
   const long long M = (long long)p->B * p->H * p->W;
   if (M + 64 >= (1ll << 31)) return ODT_ERR_UNSUPPORTED;  // pixel indices are 32-bit
@@ -413,24 +341,16 @@ int conv_pw_try(const void* in, const void* weights, const odt_conv_params* p, v
   const Epi e = make_epi(*p);
   const long long want = (g.groups + PW_WARPS - 1) / PW_WARPS;  // blocks that give every warp one group
   const long long cap = (long long)kNumSMs * (g.smem_bytes <= PW_SMEM_SHARE ? PW_BLOCKS_PER_SM : g.smem_bytes <= 113 * 1024 ? 2 : 1);
-  cudaLaunchConfig_t cfg = {};
-  cfg.blockDim = dim3(PW_THREADS);
-  cfg.gridDim = dim3((unsigned)(want < cap ? want : cap));
-  cfg.dynamicSmemBytes = g.smem_bytes;
-  cfg.stream = (cudaStream_t)stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  const unsigned grid = (unsigned)(want < cap ? want : cap);
   const __half* inh = reinterpret_cast<const __half*>(in);
   const __half* wh = reinterpret_cast<const __half*>(weights);
+  cudaStream_t st = (cudaStream_t)stream;
   if (cot == 8)
-    ODT_CUDA_OK(cudaLaunchKernelEx(&cfg, conv_pw_kernel<8>, inh, wh, g, e));
+    ODT_CUDA_OK(launch_pdl(conv_pw_kernel<8>, grid, PW_THREADS, g.smem_bytes, st, inh, wh, g, e));
   else if (cot == 16)
-    ODT_CUDA_OK(cudaLaunchKernelEx(&cfg, conv_pw_kernel<16>, inh, wh, g, e));
+    ODT_CUDA_OK(launch_pdl(conv_pw_kernel<16>, grid, PW_THREADS, g.smem_bytes, st, inh, wh, g, e));
   else
-    ODT_CUDA_OK(cudaLaunchKernelEx(&cfg, conv_pw_kernel<32>, inh, wh, g, e));
+    ODT_CUDA_OK(launch_pdl(conv_pw_kernel<32>, grid, PW_THREADS, g.smem_bytes, st, inh, wh, g, e));
   ODT_LAUNCH_OK();
   ++g_pw_launches;
   return ODT_OK;

@@ -85,13 +85,7 @@ __global__ void __launch_bounds__(TN_THREADS, 1)
   }
   if (warp >= 4) {
     // per-channel epilogue parameters (constant data): one copy per CTA
-    for (int i = threadIdx.x - 128; i < TN_PAR_FLOATS; i += 256) {
-      const int which = i >> 6, c = i & 63;
-      const bool ok = c < e.Cout;
-      const float* src = which == 0 ? e.scale : which == 1 ? e.shift : which == 2 ? e.scale2 : which == 3 ? e.shift2
-                         : which == 4 ? e.scale3 : e.shift3;
-      par[i] = (ok && src) ? __ldg(src + c) : ((which & 1) ? 0.f : 1.f);
-    }
+    for (int i = threadIdx.x - 128; i < TN_PAR_FLOATS; i += 256) par[i] = epi_param(e, i >> 6, i & 63);
   }
   __syncthreads();
 
@@ -228,8 +222,6 @@ __global__ void __launch_bounds__(TN_THREADS, 1)
       const float* my_sum = sum + (quarter * 32 + lane) * SUM_PITCH;
       for (int j = group; j < chunks; j += 2) {
         const int nb = j * 32;
-        const float4* ps = reinterpret_cast<const float4*>(par + nb);
-        const float4* ph4 = reinterpret_cast<const float4*>(par + 64 + nb);
         float v[32];
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
@@ -239,21 +231,11 @@ __global__ void __launch_bounds__(TN_THREADS, 1)
           v[4 * i + 2] = t.z;
           v[4 * i + 3] = t.w;
         }
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float4 sc = ps[i], sh = ph4[i];
-          v[4 * i + 0] = apply_act(fmaf(v[4 * i + 0], sc.x, sh.x), e.act);
-          v[4 * i + 1] = apply_act(fmaf(v[4 * i + 1], sc.y, sh.y), e.act);
-          v[4 * i + 2] = apply_act(fmaf(v[4 * i + 2], sc.z, sh.z), e.act);
-          v[4 * i + 3] = apply_act(fmaf(v[4 * i + 3], sc.w, sh.w), e.act);
-        }
         if (POOL) {
           // 2x2/2 max-pool of the rounded values: columns (odd lane, next lane), rows (even warp, next warp)
           uint4 packed[4];
-          __half2* ph = reinterpret_cast<__half2*>(packed);
+          epi_act_f16<4>(v, par + nb, 64, e.act, packed);
           uint32_t* pw = reinterpret_cast<uint32_t*>(packed);
-#pragma unroll
-          for (int i = 0; i < 16; ++i) ph[i] = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
 #pragma unroll
           for (int i = 0; i < 16; ++i) {
             uint32_t o = __shfl_down_sync(0xffffffffu, pw[i], 1);
@@ -286,67 +268,8 @@ __global__ void __launch_bounds__(TN_THREADS, 1)
           xbuf ^= 1;  // the next chunk's writers may run ahead of this chunk's readers by one barrier only
         } else if (row_ok) {
           const long long o0 = o0_row + nb;
-          if (e.residual) {
-            const uint4* rp = reinterpret_cast<const uint4*>(reinterpret_cast<const __half*>(e.residual) + o0);
-#pragma unroll
-            for (int qd = 0; qd < 4; ++qd) {
-              uint4 t = __ldg(rp + qd);
-              const __half2* h = reinterpret_cast<const __half2*>(&t);
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                float2 f = __half22float2(h[i]);
-                v[qd * 8 + 2 * i] += f.x;
-                v[qd * 8 + 2 * i + 1] += f.y;
-              }
-            }
-          }
-          uint4 packed[4];
-          __half2* ph = reinterpret_cast<__half2*>(packed);
-#pragma unroll
-          for (int i = 0; i < 16; ++i) ph[i] = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-          if (e.out0) {
-            uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<__half*>(e.out0) + o0);
-#pragma unroll
-            for (int qd = 0; qd < 4; ++qd) op[qd] = packed[qd];
-          }
-          if (e.out1) {
-            const float4* ps2 = reinterpret_cast<const float4*>(par + 128 + nb);
-            const float4* ph2 = reinterpret_cast<const float4*>(par + 192 + nb);
-            uint4 packed1[4];
-            __half2* p1 = reinterpret_cast<__half2*>(packed1);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const float4 sc = ps2[i], sh = ph2[i];
-              const float2 fa = __half22float2(ph[2 * i]);  // the consumer sees the rounded value
-              const float2 fb = __half22float2(ph[2 * i + 1]);
-              p1[2 * i] = __floats2half2_rn(apply_act(fmaf(fa.x, sc.x, sh.x), e.act2),
-                                            apply_act(fmaf(fa.y, sc.y, sh.y), e.act2));
-              p1[2 * i + 1] = __floats2half2_rn(apply_act(fmaf(fb.x, sc.z, sh.z), e.act2),
-                                                apply_act(fmaf(fb.y, sc.w, sh.w), e.act2));
-            }
-            uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<__half*>(e.out1) + o1_row + nb);
-#pragma unroll
-            for (int qd = 0; qd < 4; ++qd) op[qd] = packed1[qd];
-          }
-          if (e.out2) {
-            const float4* ps3 = reinterpret_cast<const float4*>(par + 256 + nb);
-            const float4* ph3 = reinterpret_cast<const float4*>(par + 320 + nb);
-            uint4 packed2[4];
-            __half2* p2 = reinterpret_cast<__half2*>(packed2);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const float4 sc = ps3[i], sh = ph3[i];
-              const float2 fa = __half22float2(ph[2 * i]);
-              const float2 fb = __half22float2(ph[2 * i + 1]);
-              p2[2 * i] = __floats2half2_rn(apply_act(fmaf(fa.x, sc.x, sh.x), e.act3),
-                                            apply_act(fmaf(fa.y, sc.y, sh.y), e.act3));
-              p2[2 * i + 1] = __floats2half2_rn(apply_act(fmaf(fb.x, sc.z, sh.z), e.act3),
-                                                apply_act(fmaf(fb.y, sc.w, sh.w), e.act3));
-            }
-            uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<__half*>(e.out2) + o2_row + nb);
-#pragma unroll
-            for (int qd = 0; qd < 4; ++qd) op[qd] = packed2[qd];
-          }
+          const uint4* rp = reinterpret_cast<const uint4*>(reinterpret_cast<const __half*>(e.residual) + o0);
+          epi_store_f16<4>(e, v, par + nb, 64, [&](int q) { return __ldg(rp + q); }, o0, o1_row + nb, o2_row + nb);
         }
       }
     }
@@ -362,15 +285,12 @@ int conv_tapn_try(const void* in, const void* weights, const odt_conv_params* p,
                         p->in_ld % 64 == 0 && p->in_ld / 64 <= 2 && p->w_ld == p->in_ld;
   if (!shape_ok) return ODT_ERR_UNSUPPORTED;
   const bool pool = p->out0_pool == 2;
-  auto aligned = [](const void* ptr, long long img, int pix, int need) {
-    return ((uintptr_t)ptr & 15) == 0 && img % 8 == 0 && pix % 8 == 0 && pix >= need;
-  };
+  const int need = p->Cout_pad;
   bool out_ok = p->out0_group == 0 && (!p->out0 || p->out0_dtype == ODT_F16) &&
-                (!p->out0 || aligned(p->out0, p->out0_img_stride, p->out0_pix_stride, p->Cout_pad)) &&
-                (!p->out1 || aligned(p->out1, p->out1_img_stride, p->out1_pix_stride, p->Cout_pad)) &&
-                (!p->out2 || aligned(p->out2, p->out2_img_stride, p->out2_pix_stride, p->Cout_pad)) &&
-                (!p->residual || (((uintptr_t)p->residual & 15) == 0 && p->out0_img_stride % 8 == 0 &&
-                                  p->out0_pix_stride % 8 == 0 && p->out0_pix_stride >= p->Cout_pad));
+                (!p->out0 || f16_rows_aligned(p->out0, p->out0_img_stride, p->out0_pix_stride, need)) &&
+                (!p->out1 || f16_rows_aligned(p->out1, p->out1_img_stride, p->out1_pix_stride, need)) &&
+                (!p->out2 || f16_rows_aligned(p->out2, p->out2_img_stride, p->out2_pix_stride, need)) &&
+                (!p->residual || f16_rows_aligned(p->residual, p->out0_img_stride, p->out0_pix_stride, need));
   if (pool)
     out_ok = out_ok && p->out0 && !p->residual && !p->out1 && !p->out2 && p->OH % 2 == 0 && p->OW % 2 == 0;
   else
@@ -402,8 +322,8 @@ int conv_tapn_try(const void* in, const void* weights, const odt_conv_params* p,
     const long long c_tapn = (long long)ceil_div(tiles, kNumSMs) * (9 * mm * g.BN + 1200);
     long long t_reg;  // tiles of the regular path
     if (pool) {
-      const long long t2 = (long long)((p->H + 1) / 2) * ((p->W + 63) / 64), t4 = (long long)((p->H + 3) / 4) * ((p->W + 31) / 32);
-      t_reg = (long long)p->B * (t4 < t2 ? t4 : t2);
+      tc_rowblock_rp(p->H, p->W, &t_reg);
+      t_reg *= p->B;
     } else {
       t_reg = ((long long)p->B * (p->H + 2) * (p->W + 2) + 127) / 128;
     }
@@ -444,21 +364,11 @@ int conv_tapn_try(const void* in, const void* weights, const odt_conv_params* p,
     ODT_CUDA_OK(cudaFuncSetAttribute(conv_tapn_kernel<64, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TN_SMEM_LIMIT));
     attr_set = true;
   }
-  Epi e = make_epi(*p);
-  cudaLaunchConfig_t cfg = {};
-  cfg.blockDim = dim3(TN_THREADS);
-  cfg.gridDim = dim3(g.num_tiles < kNumSMs ? g.num_tiles : kNumSMs);
-  cfg.dynamicSmemBytes = stages * TN_A_BYTES + fixed;
-  cfg.stream = (cudaStream_t)stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
   void (*kern)(CUtensorMap, CUtensorMap, TnGeom, Epi) =
       g.BN == 32 ? (pool ? conv_tapn_kernel<32, 1> : conv_tapn_kernel<32, 0>)
                  : (pool ? conv_tapn_kernel<64, 1> : conv_tapn_kernel<64, 0>);
-  ODT_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, g, e));
+  ODT_CUDA_OK(launch_pdl(kern, g.num_tiles < kNumSMs ? g.num_tiles : kNumSMs, TN_THREADS, stages * TN_A_BYTES + fixed,
+                         (cudaStream_t)stream, tmA, tmB, g, make_epi(*p)));
   ODT_LAUNCH_OK();
   ++g_tapn_launches;
   return ODT_OK;

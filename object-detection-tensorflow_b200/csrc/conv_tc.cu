@@ -45,7 +45,7 @@ constexpr int TC_THREADS = 3 * 128;  // producer warpgroup, two consumer warpgro
 // setmaxnreg split of the 64K-register file: 128 * 40 + 256 * 232 <= 65536
 constexpr int TC_PRODUCER_REGS = 40;
 constexpr int TC_CONSUMER_REGS = 232;
-constexpr int TC_EPI_PAR = 7 * TC_MAX_BN;  // floats per parameter block: scale/shift/scale2/shift2/column offset/scale3/shift3
+constexpr int TC_EPI_PAR = 7 * TC_MAX_BN;  // floats per parameter block: epi_param's six rows, then the column offsets
 // one 32-column slice of a tile's fp32 accumulators at a pitch of 36 floats (row reads of float4 per lane
 // hit distinct banks in every quarter-warp phase)
 constexpr int TC_SLICE_PITCH = 36;
@@ -133,7 +133,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   auto empty_bar = [&](int s) { return bar_base + 8u * (TC_MAX_STAGES + s); };
   const uint32_t wfull_bar = bar_base + 8u * (2 * TC_MAX_STAGES);  // resident weights landed
   // per consumer warpgroup: the epilogue parameters of its current N tile
-  // [scale|shift|scale2|shift2|offset|scale3|shift3][TC_MAX_BN], then its accumulator slice
+  // [scale|shift|scale2|shift2|scale3|shift3|offset][TC_MAX_BN], then its accumulator slice
   float* epi_smem = reinterpret_cast<float*>(smem_raw + (bar_base + 256u - raw));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -369,44 +369,29 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         // every lane of the warpgroup has finished reading the previous slice and, on a new tile, the parameters
         named_bar_sync(epi_bar, 128);
         if (j == 0 && new_par) {
-          const int n = n0 + et;
-          const bool ok = et < BN && n < e.Cout;
-          par[et] = (ok && e.scale) ? __ldg(e.scale + n) : 1.f;
-          par[P + et] = (ok && e.shift) ? __ldg(e.shift + n) : 0.f;
-          par[2 * P + et] = (ok && e.scale2) ? __ldg(e.scale2 + n) : 1.f;
-          par[3 * P + et] = (ok && e.shift2) ? __ldg(e.shift2 + n) : 0.f;
-          reinterpret_cast<int*>(par)[4 * P + et] = ok ? regroup(e, n) : 0;
-          par[5 * P + et] = (ok && e.scale3) ? __ldg(e.scale3 + n) : 1.f;
-          par[6 * P + et] = (ok && e.shift3) ? __ldg(e.shift3 + n) : 0.f;
+          const int n = et < BN ? n0 + et : e.Cout;  // columns past the tile: identity
+#pragma unroll
+          for (int row = 0; row < 6; ++row) par[row * P + et] = epi_param(e, row, n);
+          reinterpret_cast<int*>(par)[6 * P + et] = n < e.Cout ? regroup(e, n) : 0;
         }
         wg_acc_slice_to_smem<BN>(acc[0], j, slice, TC_SLICE_PITCH, 0);
         wg_acc_slice_to_smem<BN>(acc[1], j, slice, TC_SLICE_PITCH, 64);
         named_bar_sync(epi_bar, 128);
-        uint32_t r[32];
+        float v[32];
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          const uint4 t = *reinterpret_cast<const uint4*>(my_acc + 4 * i);
-          r[4 * i + 0] = t.x;
-          r[4 * i + 1] = t.y;
-          r[4 * i + 2] = t.z;
-          r[4 * i + 3] = t.w;
+          const float4 t = *reinterpret_cast<const float4*>(my_acc + 4 * i);
+          v[4 * i + 0] = t.x;
+          v[4 * i + 1] = t.y;
+          v[4 * i + 2] = t.z;
+          v[4 * i + 3] = t.w;
         }
         if (g.flat == 2) {
           // fused 2x2/2 max pooling: bias/BN + activation, round to fp16, then the maximum over
           // the window's four lanes (vertical neighbour = lane^1, horizontal = lane^RP); each
           // of the four lanes stores one 8-channel quarter of the pooled pixel
-          const float4* ps = reinterpret_cast<const float4*>(par + j * 32);
-          const float4* ph4 = reinterpret_cast<const float4*>(par + P + j * 32);
           uint4 packed[4];
-          __half2* ph = reinterpret_cast<__half2*>(packed);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 sc = ps[i], sh = ph4[i];
-            ph[2 * i] = __floats2half2_rn(apply_act(fmaf(__uint_as_float(r[4 * i + 0]), sc.x, sh.x), e.act),
-                                          apply_act(fmaf(__uint_as_float(r[4 * i + 1]), sc.y, sh.y), e.act));
-            ph[2 * i + 1] = __floats2half2_rn(apply_act(fmaf(__uint_as_float(r[4 * i + 2]), sc.z, sh.z), e.act),
-                                              apply_act(fmaf(__uint_as_float(r[4 * i + 3]), sc.w, sh.w), e.act));
-          }
+          epi_act_f16<4>(v, par + j * 32, P, e.act, packed);
           uint32_t* pw = reinterpret_cast<uint32_t*>(packed);
 #pragma unroll
           for (int i = 0; i < 16; ++i) {
@@ -421,87 +406,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
           if (row_ok && nb + 8 * pool_q < g.fast_cols)
             *reinterpret_cast<uint4*>(reinterpret_cast<__half*>(e.out0) + pool_row + nb + 8 * pool_q) = sel;
         } else if (g.fast_store && nb + 32 <= g.fast_cols) {
-          const float4* ps = reinterpret_cast<const float4*>(par + j * 32);
-          const float4* ph4 = reinterpret_cast<const float4*>(par + P + j * 32);
-          float v[32];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 sc = ps[i], sh = ph4[i];
-            v[4 * i + 0] = apply_act(fmaf(__uint_as_float(r[4 * i + 0]), sc.x, sh.x), e.act);
-            v[4 * i + 1] = apply_act(fmaf(__uint_as_float(r[4 * i + 1]), sc.y, sh.y), e.act);
-            v[4 * i + 2] = apply_act(fmaf(__uint_as_float(r[4 * i + 2]), sc.z, sh.z), e.act);
-            v[4 * i + 3] = apply_act(fmaf(__uint_as_float(r[4 * i + 3]), sc.w, sh.w), e.act);
-          }
           if (row_ok) {
             const long long o0 = o0_row + nb;
-            if (e.residual) {
-              const uint4* rp =
-                  reinterpret_cast<const uint4*>(reinterpret_cast<const __half*>(e.residual) + o0);
-#pragma unroll
-              for (int qd = 0; qd < 4; ++qd) {
-                uint4 t = __ldg(rp + qd);
-                const __half2* h = reinterpret_cast<const __half2*>(&t);
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  float2 f = __half22float2(h[i]);
-                  v[qd * 8 + 2 * i] += f.x;
-                  v[qd * 8 + 2 * i + 1] += f.y;
-                }
-              }
-            }
-            uint4 packed[4];
-            __half2* ph = reinterpret_cast<__half2*>(packed);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) ph[i] = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-            if (e.out0) {
-              uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<__half*>(e.out0) + o0);
-#pragma unroll
-              for (int qd = 0; qd < 4; ++qd) op[qd] = packed[qd];
-            }
-            if (e.out1) {
-              const float4* ps2 = reinterpret_cast<const float4*>(par + 2 * P + j * 32);
-              const float4* ph2 = reinterpret_cast<const float4*>(par + 3 * P + j * 32);
-              uint4 packed1[4];
-              __half2* p1 = reinterpret_cast<__half2*>(packed1);
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float4 sc = ps2[i], sh = ph2[i];
-                const float2 fa = __half22float2(ph[2 * i]);      // consumer sees the rounded value
-                const float2 fb = __half22float2(ph[2 * i + 1]);
-                p1[2 * i] = __floats2half2_rn(apply_act(fmaf(fa.x, sc.x, sh.x), e.act2),
-                                              apply_act(fmaf(fa.y, sc.y, sh.y), e.act2));
-                p1[2 * i + 1] = __floats2half2_rn(apply_act(fmaf(fb.x, sc.z, sh.z), e.act2),
-                                                  apply_act(fmaf(fb.y, sc.w, sh.w), e.act2));
-              }
-              uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<__half*>(e.out1) + o1_row + nb);
-#pragma unroll
-              for (int qd = 0; qd < 4; ++qd) op[qd] = packed1[qd];
-            }
-            if (e.out2) {
-              const float4* ps3 = reinterpret_cast<const float4*>(par + 5 * P + j * 32);
-              const float4* ph3 = reinterpret_cast<const float4*>(par + 6 * P + j * 32);
-              uint4 packed2[4];
-              __half2* p2 = reinterpret_cast<__half2*>(packed2);
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float4 sc = ps3[i], sh = ph3[i];
-                const float2 fa = __half22float2(ph[2 * i]);
-                const float2 fb = __half22float2(ph[2 * i + 1]);
-                p2[2 * i] = __floats2half2_rn(apply_act(fmaf(fa.x, sc.x, sh.x), e.act3),
-                                              apply_act(fmaf(fa.y, sc.y, sh.y), e.act3));
-                p2[2 * i + 1] = __floats2half2_rn(apply_act(fmaf(fb.x, sc.z, sh.z), e.act3),
-                                                  apply_act(fmaf(fb.y, sc.w, sh.w), e.act3));
-              }
-              uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<__half*>(e.out2) + o2_row + nb);
-#pragma unroll
-              for (int qd = 0; qd < 4; ++qd) op[qd] = packed2[qd];
-            }
+            const uint4* rp = reinterpret_cast<const uint4*>(reinterpret_cast<const __half*>(e.residual) + o0);
+            epi_store_f16<4>(e, v, par + j * 32, P, [&](int q) { return __ldg(rp + q); }, o0, o1_row + nb,
+                             o2_row + nb);
           }
         } else if (row_ok || g.head_mode) {
           // generic path: fp32 head outputs scattered into the candidate rows,
           // channel regrouping, ragged Cout; parameters come from shared memory
           const float* ps = par + j * 32;
-          const int* pofs = reinterpret_cast<const int*>(par) + 4 * P + j * 32;
+          const int* pofs = reinterpret_cast<const int*>(par) + 6 * P + j * 32;
           const int nvalid = min(32, e.Cout - nb);
           if (g.head_mode) {
             // head convolutions: fp32 scatter into the candidate rows.  The staged accumulator
@@ -523,24 +438,24 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
             for (int i = 0; i < 32; ++i) {
               if (i >= nvalid) break;
               const int n = nb + i;
-              float v = apply_act(fmaf(__uint_as_float(r[i]), ps[i], ps[P + i]), e.act);
+              float x = apply_act(fmaf(v[i], ps[i], ps[P + i]), e.act);
               const long long o0 = o0_row + pofs[i];
-              if (e.residual) v += __half2float(reinterpret_cast<const __half*>(e.residual)[o0]);
+              if (e.residual) x += __half2float(reinterpret_cast<const __half*>(e.residual)[o0]);
               if (e.out0) {
                 if (e.out0_dtype == ODT_F32) {
-                  reinterpret_cast<float*>(e.out0)[o0] = v;
+                  reinterpret_cast<float*>(e.out0)[o0] = x;
                 } else {
-                  const __half hv = __float2half_rn(v);
+                  const __half hv = __float2half_rn(x);
                   reinterpret_cast<__half*>(e.out0)[o0] = hv;
-                  v = __half2float(hv);
+                  x = __half2float(hv);
                 }
               }
               if (e.out1)
                 reinterpret_cast<__half*>(e.out1)[o1_row + n] =
-                    __float2half_rn(apply_act(fmaf(v, ps[2 * P + i], ps[3 * P + i]), e.act2));
+                    __float2half_rn(apply_act(fmaf(x, ps[2 * P + i], ps[3 * P + i]), e.act2));
               if (e.out2)
                 reinterpret_cast<__half*>(e.out2)[o2_row + n] =
-                    __float2half_rn(apply_act(fmaf(v, ps[5 * P + i], ps[6 * P + i]), e.act3));
+                    __float2half_rn(apply_act(fmaf(x, ps[4 * P + i], ps[5 * P + i]), e.act3));
             }
           }
         }
@@ -598,6 +513,29 @@ int tc_encode_tiled(CUtensorMap* map, const void* base, int rank, const cuuint64
     return ODT_ERR_CUDA;
   }
   return ODT_OK;
+}
+
+int tc_encode_im2col(CUtensorMap* map, const void* base, const cuuint64_t* dims, const cuuint64_t* strides,
+                     const int* lower, const int* upper, cuuint32_t channels, cuuint32_t pixels, int stride) {
+  int rc = resolve_driver();
+  if (rc) return rc;
+  cuuint32_t estr[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
+  CUresult cr = g_encode_im2col(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, lower,
+                                upper, channels, pixels, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                                CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (cr != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeIm2col failed (%d): dims %d %d %d %d lower %d %d upper %d %d stride %d", (int)cr,
+              (int)dims[0], (int)dims[1], (int)dims[2], (int)dims[3], lower[0], lower[1], upper[0], upper[1], stride);
+    return ODT_ERR_CUDA;
+  }
+  return ODT_OK;
+}
+
+int tc_rowblock_rp(int OH, int OW, long long* tiles) {
+  const long long t2 = (long long)((OH + 1) / 2) * ((OW + 63) / 64);
+  const long long t4 = (long long)((OH + 3) / 4) * ((OW + 31) / 32);
+  *tiles = t4 < t2 ? t4 : t2;
+  return t4 < t2 ? 4 : 2;
 }
 
 int conv_tapn_try(const void* in, const void* weights, const odt_conv_params* p, void* stream);  // conv_tapn.cu
@@ -662,8 +600,6 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
   ODT_CHECK_ARG(p->Cout_pad % 32 == 0, "Cout_pad must be a multiple of 32");
   ODT_CHECK_ARG(((uintptr_t)in & 15) == 0 && ((uintptr_t)weights & 15) == 0, "16-byte alignment");
   ODT_CHECK_ARG(p->stride <= 8, "stride > 8 unsupported by TMA traversal stride");
-  rc = resolve_driver();
-  if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
 
   // TF SAME upper pads
@@ -729,16 +665,14 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
   g.a_tx = TC_A_BYTES;
   int stage_bytes;
   if (g.flat == 2) {
-    // tile = RP rows x XB columns; take the split that wastes fewer tile positions
-    const long long t2 = (long long)((p->OH + 1) / 2) * ((p->OW + 63) / 64);
-    const long long t4 = (long long)((p->OH + 3) / 4) * ((p->OW + 31) / 32);
-    g.RP = t4 < t2 ? 4 : 2;
+    long long tiles_per_img;
+    g.RP = tc_rowblock_rp(p->OH, p->OW, &tiles_per_img);
     g.lgRP = g.RP == 4 ? 2 : 1;
     g.XB = TC_BM / g.RP;
     g.yblocks = (p->OH + g.RP - 1) / g.RP;
     g.xblocks = (p->OW + g.XB - 1) / g.XB;
-    ODT_CHECK_ARG((long long)p->B * g.yblocks * g.xblocks < (1ll << 31), "too many tiles");
-    g.num_m_tiles = p->B * g.yblocks * g.xblocks;
+    ODT_CHECK_ARG(p->B * tiles_per_img < (1ll << 31), "too many tiles");
+    g.num_m_tiles = (int)(p->B * tiles_per_img);
     g.BN = p->Cout_pad;
     g.num_n_tiles = 1;
     g.a_bytes = TC_FLAT_A_BYTES;
@@ -794,29 +728,13 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
     cuuint64_t dims[4] = {(cuuint64_t)p->in_ld, PH, PW, (cuuint64_t)p->B};
     cuuint64_t strides[3] = {PW * p->in_ld * 2, (cuuint64_t)p->in_ld * 2, PH * PW * p->in_ld * 2};
     cuuint32_t box[4] = {TC_BK, (cuuint32_t)g.RP, (cuuint32_t)(g.XB + 2), 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult cr = g_encode_tiled(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(in), dims,
-                                 strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                 CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) {
-      set_error("cuTensorMapEncodeTiled(row-block activations) failed (%d)", (int)cr);
-      return ODT_ERR_CUDA;
-    }
+    rc = tc_encode_tiled(&tmA, in, 4, dims, strides, box, false);
   } else if (g.flat) {
     // flat [Q][ld] view of the halo tensor, slabs of 136 consecutive padded-linear pixels
     cuuint64_t dims[2] = {(cuuint64_t)p->in_ld, (cuuint64_t)g.Q};
     cuuint64_t strides[1] = {(cuuint64_t)p->in_ld * 2};
     cuuint32_t box[2] = {TC_BK, TC_FLAT_ROWS};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult cr = g_encode_tiled(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(in), dims,
-                                 strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                 CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) {
-      set_error("cuTensorMapEncodeTiled(flat activations) failed (%d)", (int)cr);
-      return ODT_ERR_CUDA;
-    }
+    rc = tc_encode_tiled(&tmA, in, 2, dims, strides, box, false);
   } else {
     const int IW = p->W + 2 * ih, IH = p->H + 2 * ih;
     cuuint64_t dims[4] = {(cuuint64_t)p->in_ld, (cuuint64_t)IW, (cuuint64_t)IH, (cuuint64_t)p->B};
@@ -825,33 +743,16 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
     // the halo shifts the image origin by one pixel inside the stored tensor
     int lower[2] = {-p->pad_l + ih, -p->pad_t + ih};
     int upper[2] = {pad_r - (p->S - 1) * p->dil - ih, pad_b - (p->R - 1) * p->dil - ih};
-    cuuint32_t estr[4] = {1, (cuuint32_t)p->stride, (cuuint32_t)p->stride, 1};
-    CUresult cr = g_encode_im2col(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(in),
-                                  dims, strides, lower, upper, TC_BK, TC_BM, estr,
-                                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                  CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) {
-      set_error("cuTensorMapEncodeIm2col failed (%d): dims %d %d %d %d lower %d %d upper %d %d stride %d",
-                (int)cr, p->in_ld, IW, IH, p->B, lower[0], lower[1], upper[0], upper[1], p->stride);
-      return ODT_ERR_CUDA;
-    }
+    rc = tc_encode_im2col(&tmA, in, dims, strides, lower, upper, TC_BK, TC_BM, p->stride);
   }
+  if (rc) return rc;
   {
     const cuuint64_t ktot = (cuuint64_t)p->R * p->S * p->w_ld;
     cuuint64_t dims[2] = {ktot, (cuuint64_t)p->Cout_pad};
     cuuint64_t strides[1] = {ktot * 2};
     cuuint32_t box[2] = {TC_BK, (cuuint32_t)g.BN};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult cr = g_encode_tiled(&tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2,
-                                 const_cast<void*>(weights), dims, strides, box, estr,
-                                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                 CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) {
-      set_error("cuTensorMapEncodeTiled(weights) failed (%d)", (int)cr);
-      return ODT_ERR_CUDA;
-    }
+    rc = tc_encode_tiled(&tmB, weights, 2, dims, strides, box, true);
+    if (rc) return rc;
   }
 
   const int smem = stages * stage_bytes + (g.bres ? (int)wres : 0) + fixed_bytes;
@@ -867,19 +768,9 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
     ODT_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
     smem_set = true;
   }
-  Epi e = make_epi(*p);
-  cudaLaunchConfig_t cfg = {};
-  cfg.blockDim = dim3(TC_THREADS);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  cfg.attrs = attr;
   const int num_tiles = g.num_m_tiles * g.num_n_tiles;
-  cfg.gridDim = dim3(num_tiles < kNumSMs ? num_tiles : kNumSMs);
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  ODT_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, g, e));
+  ODT_CUDA_OK(launch_pdl(kern, num_tiles < kNumSMs ? num_tiles : kNumSMs, TC_THREADS, smem, st, tmA, tmB, g,
+                         make_epi(*p)));
   ODT_LAUNCH_OK();
   return ODT_OK;
 }

@@ -9,8 +9,7 @@
 // activation buffers is never touched).  Traffic for 200x200x16 images, 7->7: ~20 MB read + ~10 MB written
 // instead of 82 + 41 MB; ~800 instructions per pixel.
 //
-// Epilogue semantics = epilogue.cuh (scale/shift/act, residual, fp16 rounding, up to two extra pre-activated
-// outputs).  OPT-IN (ODT_TC_THIN=1: where the per-pixel work is small enough; =2: wherever the layer
+// The output is epilogue.cuh's fused fp16 step, one 16-byte sector at a time (epi_store_f16<1>).  OPT-IN (ODT_TC_THIN=1: where the per-pixel work is small enough; =2: wherever the layer
 // qualifies) -- written after the last GPU minute of round 1: the device launch has not run yet, the body has (below).
 // ref call sites: tf.layers.conv2d RetinaNet.py:579,599,609 (bottleneck 1x1 / 3x3 with 7..28 filters).
 //
@@ -22,19 +21,7 @@
 
 #include "epilogue.cuh"
 
-#ifdef __CUDA_ARCH__
-#define ODT_THIN_LDG(p) __ldg(p)
-#else
-#define ODT_THIN_LDG(p) (*(p))
-#endif
-
 namespace odt {
-
-__host__ __device__ __forceinline__ float thin_act(float v, int act) {  // = apply_act (common.cuh), host-callable
-  if (act == ODT_ACT_RELU) return fmaxf(v, 0.f);
-  if (act == ODT_ACT_LEAKY) return fmaxf(v, 0.1f * v);
-  return v;
-}
 
 struct ThinGeom {
   int B, H, W, OH, OW;
@@ -47,7 +34,7 @@ struct ThinGeom {
 constexpr int THIN_THREADS = 256;
 
 // KS: filter size (1 or 3); CI8 / CO8: input / output channels in units of 8.
-// ws: fp32 filter bank [tap][cin][cout]; par: [scale | shift | scale2 | shift2 | scale3 | shift3][cout].
+// ws: fp32 filter bank [tap][cin][cout]; par: epi_param's six rows [6][cout].
 template <int KS, int CI8, int CO8>
 __host__ __device__ __forceinline__ void thin_fill(int tid, float* ws, float* par, const __half* wgt, const ThinGeom& g,
                                                    const Epi& e) {
@@ -58,12 +45,7 @@ __host__ __device__ __forceinline__ void thin_fill(int tid, float* ws, float* pa
     if (n < g.Cout && c < g.Cin) v = __half2float(wgt[((long long)n * TAPS + tap) * g.w_ld + c]);
     ws[i] = v;
   }
-  for (int i = tid; i < 6 * CO; i += THIN_THREADS) {
-    const int which = i / CO, n = i % CO;
-    const float* src = which == 0 ? e.scale : which == 1 ? e.shift : which == 2 ? e.scale2 : which == 3 ? e.shift2
-                       : which == 4 ? e.scale3 : e.shift3;
-    par[i] = (n < g.Cout && src) ? ODT_THIN_LDG(src + n) : ((which & 1) ? 0.f : 1.f);
-  }
+  for (int i = tid; i < 6 * CO; i += THIN_THREADS) par[i] = epi_param(e, i / CO, i % CO);
 }
 
 template <int KS, int CI8, int CO8>
@@ -94,7 +76,7 @@ __host__ __device__ __forceinline__ void thin_pixel(long long m, const float* ws
 #pragma unroll
       for (int c8 = 0; c8 < CI8; ++c8) {
         uint4 raw = make_uint4(0u, 0u, 0u, 0u);
-        if (inside) raw = ODT_THIN_LDG(reinterpret_cast<const uint4*>(src) + c8);
+        if (inside) raw = ODT_LDG(reinterpret_cast<const uint4*>(src) + c8);
         const __half2* h2 = reinterpret_cast<const __half2*>(&raw);
         float x[8];
 #pragma unroll
@@ -125,52 +107,11 @@ __host__ __device__ __forceinline__ void thin_pixel(long long m, const float* ws
                            (oh ? (long long)((oy + 1) * (g.OW + 2) + ox + 1) : (long long)pix) * e.out0_pix_stride;
   const long long o1_row = aux_row(e.out1_img_stride, e.out1_pix_stride, e.out1_halo, g.OW, b, pix);
   const long long o2_row = aux_row(e.out2_img_stride, e.out2_pix_stride, e.out2_halo, g.OW, b, pix);
-  const float* sc1 = par, *sh1 = par + CO, *sc2 = par + 2 * CO, *sh2 = par + 3 * CO, *sc3 = par + 4 * CO,
-             *sh3 = par + 5 * CO;
+  const uint4* rp = reinterpret_cast<const uint4*>(reinterpret_cast<const __half*>(e.residual) + o0_row);
 #pragma unroll
-  for (int n8 = 0; n8 < CO8; ++n8) {
-    float v[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = thin_act(fmaf(acc[8 * n8 + i], sc1[8 * n8 + i], sh1[8 * n8 + i]), e.act);
-    if (e.residual) {
-      const uint4 t =
-          ODT_THIN_LDG(reinterpret_cast<const uint4*>(reinterpret_cast<const __half*>(e.residual) + o0_row) + n8);
-      const __half2* h = reinterpret_cast<const __half2*>(&t);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float2 f = __half22float2(h[i]);
-        v[2 * i] += f.x;
-        v[2 * i + 1] += f.y;
-      }
-    }
-    uint4 packed;
-    __half2* ph = reinterpret_cast<__half2*>(&packed);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) ph[i] = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-    if (e.out0) reinterpret_cast<uint4*>(reinterpret_cast<__half*>(e.out0) + o0_row)[n8] = packed;
-    if (e.out1) {
-      uint4 p1;
-      __half2* q = reinterpret_cast<__half2*>(&p1);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float2 f = __half22float2(ph[i]);  // the consumer sees the rounded value
-        q[i] = __floats2half2_rn(thin_act(fmaf(f.x, sc2[8 * n8 + 2 * i], sh2[8 * n8 + 2 * i]), e.act2),
-                                 thin_act(fmaf(f.y, sc2[8 * n8 + 2 * i + 1], sh2[8 * n8 + 2 * i + 1]), e.act2));
-      }
-      reinterpret_cast<uint4*>(reinterpret_cast<__half*>(e.out1) + o1_row)[n8] = p1;
-    }
-    if (e.out2) {
-      uint4 p2;
-      __half2* q = reinterpret_cast<__half2*>(&p2);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float2 f = __half22float2(ph[i]);
-        q[i] = __floats2half2_rn(thin_act(fmaf(f.x, sc3[8 * n8 + 2 * i], sh3[8 * n8 + 2 * i]), e.act3),
-                                 thin_act(fmaf(f.y, sc3[8 * n8 + 2 * i + 1], sh3[8 * n8 + 2 * i + 1]), e.act3));
-      }
-      reinterpret_cast<uint4*>(reinterpret_cast<__half*>(e.out2) + o2_row)[n8] = p2;
-    }
-  }
+  for (int n8 = 0; n8 < CO8; ++n8)
+    epi_store_f16<1>(e, acc + 8 * n8, par + 8 * n8, CO, [&](int) { return ODT_LDG(rp + n8); }, o0_row + 8 * n8,
+                     o1_row + 8 * n8, o2_row + 8 * n8);
 }
 
 template <int KS, int CI8, int CO8>
@@ -210,17 +151,8 @@ static int thin_plan(const void* in, const odt_conv_params* p, bool force, ThinG
   const int ci8 = (p->Cin + 7) / 8, co8 = (p->Cout + 7) / 8;
   const int ci8r = ci8 <= 1 ? 1 : ci8 <= 2 ? 2 : 4, co8r = co8 <= 1 ? 1 : co8 <= 2 ? 2 : 4;
   if (ci8 > 4 || co8 > 4 || (ks == 3 && (ci8 > 2 || co8 > 2))) return ODT_ERR_UNSUPPORTED;
-  auto aligned = [&](const void* ptr, long long img, int pix) {
-    return ((uintptr_t)ptr & 15) == 0 && img % 8 == 0 && pix % 8 == 0 && pix >= co8r * 8;
-  };
   const bool io_ok = ((uintptr_t)in & 15) == 0 && p->in_ld % 8 == 0 && p->in_ld >= ci8r * 8 &&
-                     (!p->out0 || (p->out0_dtype == ODT_F16 && aligned(p->out0, p->out0_img_stride, p->out0_pix_stride))) &&
-                     (!p->out1 || aligned(p->out1, p->out1_img_stride, p->out1_pix_stride)) &&
-                     (!p->out2 || aligned(p->out2, p->out2_img_stride, p->out2_pix_stride)) &&
-                     // the residual shares out0's addressing (strides / halo), whether or not out0 itself is stored
-                     (!p->residual || (((uintptr_t)p->residual & 15) == 0 && p->out0_img_stride % 8 == 0 &&
-                                       p->out0_pix_stride % 8 == 0 && p->out0_pix_stride >= co8r * 8 &&
-                                       (p->out0 || p->out0_dtype == ODT_F16)));
+                     f16_sector_outputs_ok(p, co8r * 8);
   if (!io_ok) return ODT_ERR_UNSUPPORTED;
   const long long M = (long long)p->B * p->OH * p->OW;
   if (M >= (1ll << 31) * THIN_THREADS) return ODT_ERR_UNSUPPORTED;

@@ -275,9 +275,16 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
-// host: cuTensorMapEncodeTiled for an fp16 tensor with the 128-byte swizzle and zero fill (conv_tc.cu);
-// 0 or an ODT_ERR_* code with the message set
+// host (conv_tc.cu): the tensor maps of the tensor-core kernels, fp16 with the 128-byte swizzle and zero fill;
+// 0 or an ODT_ERR_* code with the message set.  L2 promotion: 256 B for weights, 128 B for activations.
 int tc_encode_tiled(CUtensorMap* map, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides,
                     const cuuint32_t* box, bool l2_promote_256);
+// rank-4 NHWC activations, `channels` x `pixels` boxes, traversal stride `stride` along W and H
+int tc_encode_im2col(CUtensorMap* map, const void* base, const cuuint64_t* dims, const cuuint64_t* strides,
+                     const int* lower, const int* upper, cuuint32_t channels, cuuint32_t pixels, int stride);
+
+// host (conv_tc.cu): the row-block split of a pooled 3x3 layer (conv_tc's flat == 2 mode).  A tile is RP image rows x
+// 128/RP columns; RP = 4 where that needs fewer tiles than RP = 2.  Returns RP; *tiles = tiles per image.
+int tc_rowblock_rp(int OH, int OW, long long* tiles);
 
 }  // namespace odt
