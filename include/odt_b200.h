@@ -260,32 +260,29 @@ int odt_nms_per_class(const float* head, const odt_tail_params* p, int B,
 /* bytes of sel_scratch needed by odt_nms_per_class */
 long long odt_nms_scratch_bytes(const odt_tail_params* p, int B);
 
-/* RetinaNet softmax focal loss + smooth-L1 (anchor/GT matching included),
- * forward only.  cls/reg come from the same [B,N,25] head buffer; gt: f32
- * [B,G,5] rows (y,x,h,w,id) padded with -1 (G <= 128).  loss_out: f32 [B]
- * per-image loss (the reference averages them over the batch and adds weight
- * decay on the host side of the graph).  partial_scratch: f32
- * [odt_retina_loss_scratch_floats(B)]; match_scratch: i32 [B*G].
+/* Training-loss forwards, one per family.  All four share one calling convention:
+ *   head: the [B,N,25] candidate rows the inference tail reads; gt: f32 [B,G,5] rows (y,x,h,w,id)
+ *   padded with -1 (G <= 128); loss_out: f32 [B] per-image loss (the reference averages them over the
+ *   batch and adds weight decay on the host side of the graph);
+ *   scratch: odt_<family>_loss_scratch_bytes(p, B) bytes, 8-byte aligned, owned by the call until it
+ *   completes on `stream`.  The size queries return -1 for a null p, B <= 0 or p->N <= 0. */
+
+/* RetinaNet softmax focal loss + smooth-L1 (anchor/GT matching included).
  * ref: RetinaNet.py:357-474 */
+long long odt_retina_loss_scratch_bytes(const odt_tail_params* p, int B);
 int odt_retina_loss_fwd(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
-                        float alpha, float gamma, float* partial_scratch, int* match_scratch,
-                        float* loss_out, void* stream);
-long long odt_retina_loss_scratch_floats(int B);
+                        float alpha, float gamma, void* scratch, float* loss_out, void* stream);
 /* SSD300 / SSD512 training-loss forward (matching, cross-entropy, smooth-L1, hard-negative mining by
  * NonMaxSuppressionV3 over the negative anchors): replaces `_compute_one_image_loss`
- * SSD300.py:345-453 (SSD512.py same body) on the candidate rows the inference tail reads.
- * gt [B,G,5] = (y, x, h, w, class) padded with -1 rows, G <= 128.  loss_out [B] fp32, one value per
- * image.  `scratch`: odt_ssd_loss_scratch_bytes(p, B) bytes, 8-byte aligned; after the call the ints at
- * byte offset odt_ssd_loss_info_offset(p, B) hold (#positives, #negatives, #mined negatives) per image. */
+ * SSD300.py:345-453 (SSD512.py same body).  info_out: i32 [B,3] (#positives, #negatives, #mined
+ * negatives) per image, or NULL. */
 long long odt_ssd_loss_scratch_bytes(const odt_tail_params* p, int B);
-long long odt_ssd_loss_info_offset(const odt_tail_params* p, int B);
 int odt_ssd_loss_fwd(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
-                     void* scratch, float* loss_out, void* stream);
+                     void* scratch, float* loss_out, int* info_out, void* stream);
 /* FCOS training-loss forward (level assignment by GT size, inside-box targets, IoU loss, centre-ness
  * BCE, sigmoid focal loss): replaces FCOS.py:153-187 + `_compute_one_image_loss` FCOS.py:266-348 on
- * the candidate rows [20 cls, ctr, l, r, t, b (pre-exp)].  gt as above; loss_out [B]; scratch:
- * odt_fcos_loss_scratch_bytes(B) bytes, 4-byte aligned. */
-long long odt_fcos_loss_scratch_bytes(int B);
+ * the candidate rows [20 cls, ctr, l, r, t, b (pre-exp)]. */
+long long odt_fcos_loss_scratch_bytes(const odt_tail_params* p, int B);
 int odt_fcos_loss_fwd(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
                       void* scratch, float* loss_out, void* stream);
 /* YOLOv3 training-loss forward (per-GT level / prior assignment by anchor IoU at the GT's cell,
@@ -293,7 +290,7 @@ int odt_fcos_loss_fwd(const float* head, const odt_tail_params* p, int B, const 
  * without a GT centre): replaces the loss section of `_build_graph` YOLOv3.py:115-318 on the candidate
  * rows [20 cls, y, x, h, w, obj].  The four scales are config['coord_scale' | 'noobj_scale' |
  * 'obj_scale' | 'class_scale'].  loss_out [B] is pos_loss + neg_loss per image (the graph then takes
- * 0.5 x the batch mean).  scratch: odt_yolo_loss_scratch_bytes(p, B) bytes, 4-byte aligned. */
+ * 0.5 x the batch mean). */
 long long odt_yolo_loss_scratch_bytes(const odt_tail_params* p, int B);
 int odt_yolo_loss_fwd(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
                       float coord_scale, float noobj_scale, float obj_scale, float class_scale,

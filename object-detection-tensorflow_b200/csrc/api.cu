@@ -51,7 +51,7 @@ bool wres_enabled() {
 }
 }  // namespace odt
 
-extern "C" int odt_abi_version(void) { return 4; }
+extern "C" int odt_abi_version(void) { return 5; }
 
 // CRC-32C (Castagnoli, reflected 0x82F63B78) of a host buffer, continuing from `crc`
 // (0 for a fresh sum): the checksum of TensorBundle index blocks and tensor payloads

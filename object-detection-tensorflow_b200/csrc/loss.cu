@@ -1,6 +1,6 @@
-// RetinaNet training-loss forward (BASELINE config 3 "focal-loss + decode + NMS"):
-// anchor/GT matching, softmax focal loss and smooth-L1 box loss, forward only.
-// Restates RetinaNet.py:357-474 (never copied):
+// Training-loss forwards of the four families (RetinaNet, SSD, FCOS, YOLOv3), forward only.
+// RetinaNet (BASELINE config 3 "focal-loss + decode + NMS"): anchor/GT matching, softmax focal loss and
+// smooth-L1 box loss.  Restates RetinaNet.py:357-474 (never copied):
 //   * GT rows (y,x,h,w,id) padded with -1; valid count = index of first -1 in col 0
 //   * IoU[G,A]; for every GT its arg-max anchor is a positive ("best", duplicates kept);
 //     the remaining anchors: max IoU > 0.5 -> positive with the arg-max GT,
@@ -42,6 +42,42 @@ __device__ __forceinline__ int gt_count(const float* gt, int G) {
   return arg;
 }
 
+// gt_count of the block's image, computed by thread 0 and handed to every thread
+__device__ __forceinline__ int block_gt_count(const float* gb, int G) {
+  __shared__ int s_cnt;
+  if (threadIdx.x == 0) s_cnt = gt_count(gb, G);
+  __syncthreads();
+  return s_cnt;
+}
+
+// GT row g, centre form (y, x, h, w) -> corners and area, in the op order iou_match expects
+struct GtBox {
+  float y1, x1, y2, x2, area;
+};
+__device__ __forceinline__ GtBox gt_box(const float* gb, int g) {
+  const float gy = gb[g * 5], gx = gb[g * 5 + 1], gh = gb[g * 5 + 2], gw = gb[g * 5 + 3];
+  const float hh = __fmul_rn(gh, 0.5f), hw = __fmul_rn(gw, 0.5f);
+  return {__fsub_rn(gy, hh), __fsub_rn(gx, hw), __fadd_rn(gy, hh), __fadd_rn(gx, hw), __fmul_rn(gh, gw)};
+}
+
+// Fixed-order block sum of Q values over the T threads of the block: thread t contributes v[q], the halving
+// tree leaves the sums in s[q][0].  The tree's order is what keeps every loss bit-identical from run to run
+// and from one batch size to another.  (threadIdx.x is read where it is used: holding it in a variable across the
+// tree costs fcos_loss_kernel three registers.)
+template <int Q, int T>
+__device__ __forceinline__ void block_sum(float (&s)[Q][T], const float (&v)[Q]) {
+#pragma unroll
+  for (int q = 0; q < Q; ++q) s[q][threadIdx.x] = v[q];
+  __syncthreads();
+  for (int o = T / 2; o; o >>= 1) {
+    if (threadIdx.x < o) {
+#pragma unroll
+      for (int q = 0; q < Q; ++q) s[q][threadIdx.x] += s[q][threadIdx.x + o];
+    }
+    __syncthreads();
+  }
+}
+
 // K1: per (gt, image) arg-max anchor (first maximum)
 __global__ void __launch_bounds__(kLossThreads)
     loss_best_anchor_kernel(const __grid_constant__ TailP tp, const float* __restrict__ gt, int G,
@@ -50,26 +86,19 @@ __global__ void __launch_bounds__(kLossThreads)
   const odt_tail_params& p = tp.p;
   const int g = blockIdx.x, b = blockIdx.y;
   const float* gb = gt + (long long)b * G * 5;
-  __shared__ int s_cnt;
   __shared__ float s_v[kLossThreads];
   __shared__ int s_i[kLossThreads];
-  if (threadIdx.x == 0) s_cnt = gt_count(gb, G);
-  __syncthreads();
-  if (g >= s_cnt) {
+  if (g >= block_gt_count(gb, G)) {
     if (threadIdx.x == 0) best[b * G + g] = -1;
     return;
   }
-  const float gy = gb[g * 5 + 0], gx = gb[g * 5 + 1], gh = gb[g * 5 + 2], gw = gb[g * 5 + 3];
-  const float hh = __fmul_rn(gh, 0.5f), hw = __fmul_rn(gw, 0.5f);
-  const float gy1 = __fsub_rn(gy, hh), gx1 = __fsub_rn(gx, hw);
-  const float gy2 = __fadd_rn(gy, hh), gx2 = __fadd_rn(gx, hw);
-  const float garea = __fmul_rn(gh, gw);
+  const GtBox box = gt_box(gb, g);
   float bv = -1.f;
   int bi = 0x7fffffff;
   for (int n = threadIdx.x; n < p.N; n += blockDim.x) {
     Cell c = locate(p, n);
     Anchor a = anchor_ssd(p, c);
-    float v = iou_match(a, gy1, gx1, gy2, gx2, garea);
+    float v = iou_match(a, box.y1, box.x1, box.y2, box.x2, box.area);
     if (v > bv) {
       bv = v;
       bi = n;
@@ -126,109 +155,6 @@ __device__ __forceinline__ float coord_loss(const float* r, const Anchor& a, flo
   return __fadd_rn(lyx, lhw);
 }
 
-// K2: per-anchor assignment + loss partial sums. partial[b][blk] = (conf, coord, npos)
-__global__ void __launch_bounds__(kLossThreads)
-    loss_anchor_kernel(const float* __restrict__ head, const __grid_constant__ TailP tp,
-                       const float* __restrict__ gt, int G, const int* __restrict__ best,
-                       float alpha, float gamma, float* __restrict__ partial) {
-  pdl_launch_dependents();
-  const odt_tail_params& p = tp.p;
-  const int b = blockIdx.y, blk = blockIdx.x;
-  const float* gb = gt + (long long)b * G * 5;
-  __shared__ float s_gt[kMaxGT][6];  // y1,x1,y2,x2,area,(unused)
-  __shared__ int s_best[kMaxGT];
-  __shared__ int s_cnt;
-  __shared__ float s_red[3][kLossThreads];
-  if (threadIdx.x == 0) s_cnt = gt_count(gb, G);
-  __syncthreads();
-  const int cnt = s_cnt;
-  for (int g = threadIdx.x; g < cnt; g += blockDim.x) {
-    float gy = gb[g * 5], gx = gb[g * 5 + 1], gh = gb[g * 5 + 2], gw = gb[g * 5 + 3];
-    float hh = __fmul_rn(gh, 0.5f), hw = __fmul_rn(gw, 0.5f);
-    s_gt[g][0] = __fsub_rn(gy, hh);
-    s_gt[g][1] = __fsub_rn(gx, hw);
-    s_gt[g][2] = __fadd_rn(gy, hh);
-    s_gt[g][3] = __fadd_rn(gx, hw);
-    s_gt[g][4] = __fmul_rn(gh, gw);
-    s_best[g] = best[b * G + g];
-  }
-  __syncthreads();
-  const float* hb = head + (long long)b * p.N * kRow;
-  float conf = 0.f, coord = 0.f, npos = 0.f;
-  const int per = (p.N + kLossBlocks - 1) / kLossBlocks;
-  const int n_begin = blk * per, n_end = min(p.N, n_begin + per);
-  for (int n = n_begin + threadIdx.x; n < n_end; n += blockDim.x) {
-    bool is_best = false;
-    for (int g = 0; g < cnt; ++g) is_best |= (s_best[g] == n);
-    if (is_best) continue;  // handled by the per-GT pass below (ref :397-411)
-    Cell c = locate(p, n);
-    Anchor a = anchor_ssd(p, c);
-    float bv = -1.f;
-    int bg = 0;
-    for (int g = 0; g < cnt; ++g) {
-      float v = iou_match(a, s_gt[g][0], s_gt[g][1], s_gt[g][2], s_gt[g][3], s_gt[g][4]);
-      if (v > bv) {
-        bv = v;
-        bg = g;
-      }
-    }
-    const bool pos = bv > 0.5f, neg = bv < 0.4f;
-    if (!pos && !neg) continue;
-    const float* r = hb + (long long)n * kRow;
-    float prob[21];
-    softmax21(r, prob);
-    if (pos) {
-      int label = (int)gb[bg * 5 + 4];
-      conf += focal(prob[label], alpha, gamma);
-      coord += coord_loss(r, a, gb[bg * 5], gb[bg * 5 + 1], gb[bg * 5 + 2], gb[bg * 5 + 3]);
-      npos += 1.f;
-    } else {
-      conf += focal(prob[20], alpha, gamma);
-    }
-  }
-  // the G "best anchor" positives (duplicates kept), once per image (block 0)
-  if (blk == 0) {
-    for (int g = threadIdx.x; g < cnt; g += blockDim.x) {
-      int n = s_best[g];
-      Cell c = locate(p, n);
-      Anchor a = anchor_ssd(p, c);
-      const float* r = hb + (long long)n * kRow;
-      float prob[21];
-      softmax21(r, prob);
-      int label = (int)gb[g * 5 + 4];
-      conf += focal(prob[label], alpha, gamma);
-      coord += coord_loss(r, a, gb[g * 5], gb[g * 5 + 1], gb[g * 5 + 2], gb[g * 5 + 3]);
-      npos += 1.f;
-    }
-  }
-  s_red[0][threadIdx.x] = conf;
-  s_red[1][threadIdx.x] = coord;
-  s_red[2][threadIdx.x] = npos;
-  __syncthreads();
-  for (int o = kLossThreads / 2; o; o >>= 1) {
-    if (threadIdx.x < o) {
-#pragma unroll
-      for (int q = 0; q < 3; ++q) s_red[q][threadIdx.x] += s_red[q][threadIdx.x + o];
-    }
-    __syncthreads();
-  }
-  if (threadIdx.x < 3) partial[((long long)b * kLossBlocks + blk) * 4 + threadIdx.x] = s_red[threadIdx.x][0];
-}
-
-__global__ void loss_final_kernel(const float* __restrict__ partial, int B, float* __restrict__ out) {
-  pdl_launch_dependents();
-  int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= B) return;
-  float conf = 0.f, coord = 0.f, npos = 0.f;
-  for (int i = 0; i < kLossBlocks; ++i) {
-    const float* q = partial + ((long long)b * kLossBlocks + i) * 4;
-    conf += q[0];
-    coord += q[1];
-    npos += q[2];
-  }
-  out[b] = conf / npos + coord / npos;
-}
-
 // ============================ SSD loss forward ==============================
 // Restates SSD300.py:345-453 / SSD512.py (never copied):
 //   * matching as above but with ONE threshold: other anchors with best IoU > 0.5 are
@@ -248,37 +174,55 @@ __device__ __forceinline__ float xent21(const float* r, int label) {
   return __fsub_rn(logf(s), __fsub_rn(r[label], m));
 }
 
-// K2': per-anchor assignment; positives -> partial sums, negatives -> (loss, row) keys
+// classification term of row r for class `label`: SSD cross-entropy, RetinaNet softmax focal loss
+template <bool kSsd>
+__device__ __forceinline__ float class_loss(const float* r, int label, float alpha, float gamma) {
+  if constexpr (kSsd) {
+    return xent21(r, label);
+  } else {
+    float prob[21];
+    softmax21(r, prob);
+    return focal(prob[label], alpha, gamma);
+  }
+}
+
+// K2: per-anchor assignment + loss partial sums, partial[b][blk] = (conf, coord, npos).  The families differ in
+// three places: RetinaNet ignores best IoUs in [0.4, 0.5] and scores with the focal term (alpha, gamma); SSD
+// scores with the cross-entropy and hands every negative to the mining kernel as a (loss, row) key in
+// neg_keys / neg_count.  A matched anchor's classification term is computed once, for its GT's class or for the
+// background (20).  The anchor loop is warp-uniform for the SSD ballot; each thread still visits
+// n_begin + tid, + blockDim.x, ... in that order.
+template <bool kSsd>
 __global__ void __launch_bounds__(kLossThreads)
-    ssd_loss_anchor_kernel(const float* __restrict__ head, const __grid_constant__ TailP tp,
-                           const float* __restrict__ gt, int G, const int* __restrict__ best,
-                           float* __restrict__ partial, unsigned long long* __restrict__ neg_keys,
-                           int* __restrict__ neg_count) {
+    loss_anchor_kernel(const float* __restrict__ head, const __grid_constant__ TailP tp,
+                       const float* __restrict__ gt, int G, const int* __restrict__ best, float alpha,
+                       float gamma, float* __restrict__ partial, unsigned long long* __restrict__ neg_keys,
+                       int* __restrict__ neg_count) {
   pdl_launch_dependents();
   const odt_tail_params& p = tp.p;
   const int b = blockIdx.y, blk = blockIdx.x;
   const float* gb = gt + (long long)b * G * 5;
-  __shared__ float s_gt[kMaxGT][6];
+  __shared__ float s_gt[kMaxGT][6];  // y1,x1,y2,x2,area,(unused)
   __shared__ int s_best[kMaxGT];
-  __shared__ int s_cnt;
   __shared__ float s_red[3][kLossThreads];
-  if (threadIdx.x == 0) s_cnt = gt_count(gb, G);
-  __syncthreads();
-  const int cnt = s_cnt;
+  const int cnt = block_gt_count(gb, G);
   for (int g = threadIdx.x; g < cnt; g += blockDim.x) {
-    float gy = gb[g * 5], gx = gb[g * 5 + 1], gh = gb[g * 5 + 2], gw = gb[g * 5 + 3];
-    float hh = __fmul_rn(gh, 0.5f), hw = __fmul_rn(gw, 0.5f);
-    s_gt[g][0] = __fsub_rn(gy, hh);
-    s_gt[g][1] = __fsub_rn(gx, hw);
-    s_gt[g][2] = __fadd_rn(gy, hh);
-    s_gt[g][3] = __fadd_rn(gx, hw);
-    s_gt[g][4] = __fmul_rn(gh, gw);
+    const GtBox box = gt_box(gb, g);
+    s_gt[g][0] = box.y1;
+    s_gt[g][1] = box.x1;
+    s_gt[g][2] = box.y2;
+    s_gt[g][3] = box.x2;
+    s_gt[g][4] = box.area;
     s_best[g] = best[b * G + g];
   }
   __syncthreads();
   const float* hb = head + (long long)b * p.N * kRow;
-  unsigned long long* nk = neg_keys + (long long)b * p.N;
   float conf = 0.f, coord = 0.f, npos = 0.f;
+  auto positive = [&](const float* r, const Anchor& a, int g, float cls) {  // row r, anchor a matched to GT g
+    conf += cls;
+    coord += coord_loss(r, a, gb[g * 5], gb[g * 5 + 1], gb[g * 5 + 2], gb[g * 5 + 3]);
+    npos += 1.f;
+  };
   const int per = (p.N + kLossBlocks - 1) / kLossBlocks;
   const int n_begin = blk * per, n_end = min(p.N, n_begin + per);
   for (int n0 = n_begin; n0 < n_end; n0 += blockDim.x) {
@@ -288,7 +232,7 @@ __global__ void __launch_bounds__(kLossThreads)
     if (n < n_end) {
       bool is_best = false;
       for (int g = 0; g < cnt; ++g) is_best |= (s_best[g] == n);
-      if (!is_best) {
+      if (!is_best) {  // the best anchors are handled by the per-GT pass below (ref :397-411)
         Cell c = locate(p, n);
         Anchor a = anchor_ssd(p, c);
         float bv = -1.f;
@@ -300,52 +244,70 @@ __global__ void __launch_bounds__(kLossThreads)
             bg = g;
           }
         }
-        const float* r = hb + (long long)n * kRow;
-        if (bv > 0.5f) {
-          conf += xent21(r, (int)gb[bg * 5 + 4]);
-          coord += coord_loss(r, a, gb[bg * 5], gb[bg * 5 + 1], gb[bg * 5 + 2], gb[bg * 5 + 3]);
-          npos += 1.f;
-        } else {
-          is_neg = true;
-          nloss = xent21(r, 20);
+        const bool pos = bv > 0.5f, neg = kSsd || bv < 0.4f;  // RetinaNet ignores best IoUs in [0.4, 0.5]
+        if (pos || neg) {
+          const float* r = hb + (long long)n * kRow;
+          const float cls = class_loss<kSsd>(r, pos ? (int)gb[bg * 5 + 4] : 20, alpha, gamma);
+          if (pos) {
+            positive(r, a, bg, cls);
+          } else if constexpr (kSsd) {
+            is_neg = true;
+            nloss = cls;
+          } else {
+            conf += cls;
+          }
         }
       }
     }
-    // warp-aggregated append of the negatives (order is irrelevant: keys are unique)
-    const unsigned mask = __ballot_sync(0xffffffffu, is_neg);
-    if (mask) {
-      const int lane = threadIdx.x & 31, leader = __ffs(mask) - 1;
-      int base = 0;
-      if (lane == leader) base = atomicAdd(&neg_count[b], __popc(mask));
-      base = __shfl_sync(0xffffffffu, base, leader);
-      if (is_neg)
-        nk[base + __popc(mask & ((1u << lane) - 1))] =
-            ((unsigned long long)__float_as_uint(nloss) << 32) | (0xFFFFFFFFu - (unsigned)n);
+    if constexpr (kSsd) {
+      // warp-aggregated append of the negatives (order is irrelevant: keys are unique)
+      unsigned long long* nk = neg_keys + (long long)b * p.N;
+      const unsigned mask = __ballot_sync(0xffffffffu, is_neg);
+      if (mask) {
+        const int lane = threadIdx.x & 31, leader = __ffs(mask) - 1;
+        int base = 0;
+        if (lane == leader) base = atomicAdd(&neg_count[b], __popc(mask));
+        base = __shfl_sync(0xffffffffu, base, leader);
+        if (is_neg)
+          nk[base + __popc(mask & ((1u << lane) - 1))] =
+              ((unsigned long long)__float_as_uint(nloss) << 32) | (0xFFFFFFFFu - (unsigned)n);
+      }
     }
   }
-  if (blk == 0) {  // the G "best anchor" positives (duplicates kept)
+  if (blk == 0) {  // the G "best anchor" positives (duplicates kept), once per image
     for (int g = threadIdx.x; g < cnt; g += blockDim.x) {
       int n = s_best[g];
       Cell c = locate(p, n);
-      Anchor a = anchor_ssd(p, c);
       const float* r = hb + (long long)n * kRow;
-      conf += xent21(r, (int)gb[g * 5 + 4]);
-      coord += coord_loss(r, a, gb[g * 5], gb[g * 5 + 1], gb[g * 5 + 2], gb[g * 5 + 3]);
-      npos += 1.f;
+      positive(r, anchor_ssd(p, c), g, class_loss<kSsd>(r, (int)gb[g * 5 + 4], alpha, gamma));
     }
   }
-  s_red[0][threadIdx.x] = conf;
-  s_red[1][threadIdx.x] = coord;
-  s_red[2][threadIdx.x] = npos;
-  __syncthreads();
-  for (int o = kLossThreads / 2; o; o >>= 1) {
-    if (threadIdx.x < o) {
-#pragma unroll
-      for (int q = 0; q < 3; ++q) s_red[q][threadIdx.x] += s_red[q][threadIdx.x + o];
-    }
-    __syncthreads();
-  }
+  block_sum(s_red, {conf, coord, npos});
   if (threadIdx.x < 3) partial[((long long)b * kLossBlocks + blk) * 4 + threadIdx.x] = s_red[threadIdx.x][0];
+}
+
+// (conf, coord, npos) of image b: its kLossBlocks partials summed in block order
+struct LossSums {
+  float conf, coord, npos;
+};
+__device__ __forceinline__ LossSums image_sums(const float* __restrict__ partial, int b) {
+  LossSums s = {0.f, 0.f, 0.f};
+  for (int i = 0; i < kLossBlocks; ++i) {
+    const float* q = partial + ((long long)b * kLossBlocks + i) * 4;
+    s.conf += q[0];
+    s.coord += q[1];
+    s.npos += q[2];
+  }
+  return s;
+}
+
+// K3 (RetinaNet)
+__global__ void loss_final_kernel(const float* __restrict__ partial, int B, float* __restrict__ out) {
+  pdl_launch_dependents();
+  int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const LossSums s = image_sums(partial, b);
+  out[b] = s.conf / s.npos + s.coord / s.npos;
 }
 
 // negative anchor box in the reference's op order: yx -+ hw/2 of the centre form (:419)
@@ -356,7 +318,7 @@ __device__ __forceinline__ float4 neg_anchor_box(const odt_tail_params& p, int n
   return make_float4(__fsub_rn(a.cy, hh), __fsub_rn(a.cx, hw), __fadd_rn(a.cy, hh), __fadd_rn(a.cx, hw));
 }
 
-// K3': one CTA per image: hard-negative mining (exact greedy NMS by repeated arg-max, as in
+// K3 (SSD): one CTA per image: hard-negative mining (exact greedy NMS by repeated arg-max, as in
 // tail.cu) + the final combination.  loss_out[b] = mean(selected neg) + conf/npos + coord/npos
 __global__ void __launch_bounds__(kLossThreads)
     ssd_loss_mine_kernel(const __grid_constant__ TailP tp, const float* __restrict__ partial,
@@ -367,14 +329,8 @@ __global__ void __launch_bounds__(kLossThreads)
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   __shared__ unsigned long long s_wkey[kLossThreads / 32];
   __shared__ int s_wpos[kLossThreads / 32];
-  float conf = 0.f, coord = 0.f, nposf = 0.f;
-  for (int i = 0; i < kLossBlocks; ++i) {
-    const float* q = partial + ((long long)b * kLossBlocks + i) * 4;
-    conf += q[0];
-    coord += q[1];
-    nposf += q[2];
-  }
-  const int npos = (int)nposf, cnt = neg_count[b];
+  const LossSums sums = image_sums(partial, b);
+  const int npos = (int)sums.npos, cnt = neg_count[b];
   const int chosen = cnt > 3 * npos ? 3 * npos : cnt;
   unsigned long long* keys = neg_keys + (long long)b * p.N;
   double neg_sum = 0.0;  // thread 0 only
@@ -427,7 +383,7 @@ __global__ void __launch_bounds__(kLossThreads)
     __syncthreads();
   }
   if (tid == 0) {
-    loss_out[b] = (float)(neg_sum / (double)nsel) + conf / nposf + coord / nposf;
+    loss_out[b] = (float)(neg_sum / (double)nsel) + sums.conf / sums.npos + sums.coord / sums.npos;
     if (info_out) {
       info_out[b * 3 + 0] = npos;
       info_out[b * 3 + 1] = cnt;
@@ -462,11 +418,8 @@ __global__ void __launch_bounds__(kLossThreads)
   __shared__ float s_box[kMaxGT][kFcosLevels][4];  // y1,x1,y2,x2 in stride units of each level
   __shared__ int s_cls[kMaxGT];
   __shared__ int s_lv[kMaxGT];                      // level membership bits
-  __shared__ int s_cnt;
-  __shared__ float s_red[kLossThreads];
-  if (threadIdx.x == 0) s_cnt = gt_count(gb, G);
-  __syncthreads();
-  const int cnt = s_cnt;
+  __shared__ float s_red[1][kLossThreads];
+  const int cnt = block_gt_count(gb, G);
   for (int g = threadIdx.x; g < cnt; g += blockDim.x) {
     const float gy = gb[g * 5], gx = gb[g * 5 + 1], gh = gb[g * 5 + 2], gw = gb[g * 5 + 3];
     const float size = __fsqrt_rn(__fmul_rn(gh, gw));
@@ -564,17 +517,11 @@ __global__ void __launch_bounds__(kLossThreads)
       }
     }
   }
-  // fixed-order block reduction of the 5 x 4 sums
+  // the 5 x 4 sums one at a time
   for (int l = 0; l < kFcosLevels; ++l) {
     for (int q = 0; q < 4; ++q) {
-      s_red[threadIdx.x] = acc[l][q];
-      __syncthreads();
-      for (int o = kLossThreads / 2; o; o >>= 1) {
-        if (threadIdx.x < o) s_red[threadIdx.x] += s_red[threadIdx.x + o];
-        __syncthreads();
-      }
-      if (threadIdx.x == 0) partial[(((long long)b * kLossBlocks + blk) * kFcosLevels + l) * 4 + q] = s_red[0];
-      __syncthreads();
+      block_sum(s_red, {acc[l][q]});
+      if (threadIdx.x == 0) partial[(((long long)b * kLossBlocks + blk) * kFcosLevels + l) * 4 + q] = s_red[0][0];
     }
   }
 }
@@ -612,6 +559,24 @@ __device__ __forceinline__ float iou_unclamped(float gy1, float gx1, float gy2, 
 }
 constexpr int kYoloLevels = 3;
 
+// GT row g normalised for level k (divided by 32 / 16 / 8): centre, size and corners
+struct YoloGt {
+  float y, x, h, w, y1, x1, y2, x2;
+};
+__device__ __forceinline__ YoloGt yolo_gt(const float* gb, int g, int k) {
+  const float norm = k == 0 ? 32.f : (k == 1 ? 16.f : 8.f);
+  YoloGt n;
+  n.y = __fdiv_rn(gb[g * 5], norm);
+  n.x = __fdiv_rn(gb[g * 5 + 1], norm);
+  n.h = __fdiv_rn(gb[g * 5 + 2], norm);
+  n.w = __fdiv_rn(gb[g * 5 + 3], norm);
+  n.y1 = __fsub_rn(n.y, __fdiv_rn(n.h, 2.f));
+  n.x1 = __fsub_rn(n.x, __fdiv_rn(n.w, 2.f));
+  n.y2 = __fadd_rn(n.y, __fdiv_rn(n.h, 2.f));
+  n.x2 = __fadd_rn(n.x, __fdiv_rn(n.w, 2.f));
+  return n;
+}
+
 // K1: one block per image, one thread per GT: level / prior assignment, positive terms, cell occupancy
 __global__ void __launch_bounds__(kMaxGT)
     yolo_loss_pos_kernel(const float* __restrict__ head, const __grid_constant__ TailP tp,
@@ -621,36 +586,26 @@ __global__ void __launch_bounds__(kMaxGT)
   const odt_tail_params& p = tp.p;
   const int b = blockIdx.x, g = threadIdx.x;
   const float* gb = gt + (long long)b * G * 5;
-  __shared__ int s_cnt;
   __shared__ float s_red[3][kMaxGT];
-  if (threadIdx.x == 0) s_cnt = gt_count(gb, G);
-  __syncthreads();
-  const int cnt = s_cnt;
-  const float norm[kYoloLevels] = {32.f, 16.f, 8.f};
+  const int cnt = block_gt_count(gb, G);
   const long long cells = p.N / 3;
   float coord = 0.f, cls = 0.f, obj = 0.f;
   if (g < cnt) {
     float mx[kYoloLevels];
     int arg[kYoloLevels], cy[kYoloLevels], cx[kYoloLevels];
-    float ny[kYoloLevels], nx[kYoloLevels], nh[kYoloLevels], nw[kYoloLevels];
 #pragma unroll
     for (int k = 0; k < kYoloLevels; ++k) {
       const odt_level& L = p.level[k];
-      ny[k] = __fdiv_rn(gb[g * 5], norm[k]);
-      nx[k] = __fdiv_rn(gb[g * 5 + 1], norm[k]);
-      nh[k] = __fdiv_rn(gb[g * 5 + 2], norm[k]);
-      nw[k] = __fdiv_rn(gb[g * 5 + 3], norm[k]);
-      cy[k] = min(max((int)floorf(ny[k]), 0), L.H - 1);
-      cx[k] = min(max((int)floorf(nx[k]), 0), L.W - 1);
+      const YoloGt n = yolo_gt(gb, g, k);
+      cy[k] = min(max((int)floorf(n.y), 0), L.H - 1);
+      cx[k] = min(max((int)floorf(n.x), 0), L.W - 1);
       occ[(long long)b * cells + L.offset / 3 + cy[k] * L.W + cx[k]] = 1;  // every GT marks its cell on every level
-      const float gy1 = __fsub_rn(ny[k], __fdiv_rn(nh[k], 2.f)), gx1 = __fsub_rn(nx[k], __fdiv_rn(nw[k], 2.f));
-      const float gy2 = __fadd_rn(ny[k], __fdiv_rn(nh[k], 2.f)), gx2 = __fadd_rn(nx[k], __fdiv_rn(nw[k], 2.f));
       const float ay = (float)cy[k] + 0.5f, ax = (float)cx[k] + 0.5f;
       float bv = 0.f;
       int bi = 0;
       for (int a = 0; a < 3; ++a) {
         const float hh = __fdiv_rn(L.prior_h[a], 2.f), hw = __fdiv_rn(L.prior_w[a], 2.f);
-        const float v = iou_unclamped(gy1, gx1, gy2, gx2, __fsub_rn(ay, hh), __fsub_rn(ax, hw), __fadd_rn(ay, hh),
+        const float v = iou_unclamped(n.y1, n.x1, n.y2, n.x2, __fsub_rn(ay, hh), __fsub_rn(ax, hw), __fadd_rn(ay, hh),
                                       __fadd_rn(ax, hw), __fmul_rn(L.prior_h[a], L.prior_w[a]));
         if (a == 0 || v > bv) {
           bv = v;
@@ -664,9 +619,10 @@ __global__ void __launch_bounds__(kMaxGT)
     if (mx[0] > mx[1] && mx[0] > mx[2]) k = 0;
     else if (mx[1] > mx[0] && mx[1] > mx[2]) k = 1;
     const odt_level& L = p.level[k];
+    const YoloGt n = yolo_gt(gb, g, k);
     const float* r = head + ((long long)b * p.N + L.offset + (long long)(cy[k] * L.W + cx[k]) * 3 + arg[k]) * kRow;
-    const float ty = __fsub_rn(ny[k], floorf(ny[k])), tx = __fsub_rn(nx[k], floorf(nx[k]));
-    const float th = logf(__fdiv_rn(nh[k], L.prior_h[arg[k]])), tw = logf(__fdiv_rn(nw[k], L.prior_w[arg[k]]));
+    const float ty = __fsub_rn(n.y, floorf(n.y)), tx = __fsub_rn(n.x, floorf(n.x));
+    const float th = logf(__fdiv_rn(n.h, L.prior_h[arg[k]])), tw = logf(__fdiv_rn(n.w, L.prior_w[arg[k]]));
     coord = sig_xent(ty, r[20]) + sig_xent(tx, r[21]);
     const float dh = __fsub_rn(r[22], th), dw = __fsub_rn(r[23], tw);
     coord += 0.5f * (dh * dh + dw * dw);
@@ -674,17 +630,7 @@ __global__ void __launch_bounds__(kMaxGT)
     for (int c = 0; c < 20; ++c) cls += sig_xent(c == label ? 1.f : 0.f, r[c]);
     obj = sig_xent(1.f, r[24]);
   }
-  s_red[0][threadIdx.x] = coord;
-  s_red[1][threadIdx.x] = cls;
-  s_red[2][threadIdx.x] = obj;
-  __syncthreads();
-  for (int o = kMaxGT / 2; o; o >>= 1) {
-    if (threadIdx.x < o) {
-#pragma unroll
-      for (int q = 0; q < 3; ++q) s_red[q][threadIdx.x] += s_red[q][threadIdx.x + o];
-    }
-    __syncthreads();
-  }
+  block_sum(s_red, {coord, cls, obj});
   if (threadIdx.x < 3) pos_out[b * 4 + threadIdx.x] = s_red[threadIdx.x][0];
   if (threadIdx.x == 3) pos_out[b * 4 + 3] = (float)cnt;
 }
@@ -699,21 +645,16 @@ __global__ void __launch_bounds__(kLossThreads)
   const int b = blockIdx.y, blk = blockIdx.x;
   const float* gb = gt + (long long)b * G * 5;
   __shared__ float s_g[kMaxGT][kYoloLevels][4];
-  __shared__ int s_cnt;
-  __shared__ float s_red[kLossThreads];
-  if (threadIdx.x == 0) s_cnt = gt_count(gb, G);
-  __syncthreads();
-  const int cnt = s_cnt;
-  const float norm[kYoloLevels] = {32.f, 16.f, 8.f};
+  __shared__ float s_red[1][kLossThreads];
+  const int cnt = block_gt_count(gb, G);
   for (int g = threadIdx.x; g < cnt; g += blockDim.x) {
 #pragma unroll
     for (int k = 0; k < kYoloLevels; ++k) {
-      const float ny = __fdiv_rn(gb[g * 5], norm[k]), nx = __fdiv_rn(gb[g * 5 + 1], norm[k]);
-      const float nh = __fdiv_rn(gb[g * 5 + 2], norm[k]), nw = __fdiv_rn(gb[g * 5 + 3], norm[k]);
-      s_g[g][k][0] = __fsub_rn(ny, __fdiv_rn(nh, 2.f));
-      s_g[g][k][1] = __fsub_rn(nx, __fdiv_rn(nw, 2.f));
-      s_g[g][k][2] = __fadd_rn(ny, __fdiv_rn(nh, 2.f));
-      s_g[g][k][3] = __fadd_rn(nx, __fdiv_rn(nw, 2.f));
+      const YoloGt n = yolo_gt(gb, g, k);
+      s_g[g][k][0] = n.y1;
+      s_g[g][k][1] = n.x1;
+      s_g[g][k][2] = n.y2;
+      s_g[g][k][3] = n.x2;
     }
   }
   __syncthreads();
@@ -739,13 +680,8 @@ __global__ void __launch_bounds__(kLossThreads)
                                        bx1, by2, bx2, aarea));
     if (best <= 0.5f) acc += sig_xent(0.f, hb[(long long)n * kRow + 24]);
   }
-  s_red[threadIdx.x] = acc;
-  __syncthreads();
-  for (int o = kLossThreads / 2; o; o >>= 1) {
-    if (threadIdx.x < o) s_red[threadIdx.x] += s_red[threadIdx.x + o];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) partial[(long long)b * kLossBlocks + blk] = s_red[0];
+  block_sum(s_red, {acc});
+  if (threadIdx.x == 0) partial[(long long)b * kLossBlocks + blk] = s_red[0][0];
 }
 
 __global__ void yolo_loss_final_kernel(const float* __restrict__ pos, const float* __restrict__ partial, int B,
@@ -759,90 +695,129 @@ __global__ void yolo_loss_final_kernel(const float* __restrict__ pos, const floa
   out[b] = (cs * pos[b * 4 + 0] + ks * pos[b * 4 + 1] + os * pos[b * 4 + 2]) / ng + ns * (float)noobj / ng;
 }
 
+// ============================ scratch layouts ===============================
+// Every loss call gets one caller-allocated scratch buffer, 8-byte aligned, carved into arrays that each start
+// on an 8-byte boundary.  A family's layout function is the only place its arrays are placed: the size query
+// carves from address 0 and returns the total, the launcher carves the caller's buffer.  (The layouts take()
+// inside braced lists, which C++ evaluates left to right.)
+struct Carve {
+  uintptr_t base;
+  long long bytes;
+  template <class T>
+  T* take(long long n) {
+    T* at = reinterpret_cast<T*>(base + bytes);
+    bytes += (n * (long long)sizeof(T) + 7) & ~7ll;
+    return at;
+  }
+};
+
+struct RetinaScratch {
+  float* partial;  // (conf, coord, npos, -) per (image, anchor block)
+  int* best;       // arg-max anchor per (image, GT)
+  long long bytes;
+};
+static RetinaScratch retina_scratch(const odt_tail_params&, int B, void* base) {
+  Carve c{(uintptr_t)base, 0};
+  return {c.take<float>((long long)B * kLossBlocks * 4), c.take<int>((long long)B * kMaxGT), c.bytes};
+}
+
+struct SsdScratch {
+  float* partial;                // as RetinaScratch
+  int* best;
+  int* neg_count;                // negatives per image
+  unsigned long long* neg_keys;  // (background loss, row) per negative, [B][N]
+  long long bytes;
+};
+static SsdScratch ssd_scratch(const odt_tail_params& p, int B, void* base) {
+  Carve c{(uintptr_t)base, 0};
+  return {c.take<float>((long long)B * kLossBlocks * 4), c.take<int>((long long)B * kMaxGT), c.take<int>(B),
+          c.take<unsigned long long>((long long)B * p.N), c.bytes};
+}
+
+struct FcosScratch {
+  float* partial;  // (iou, focal, centre, #positive class cells) per (image, anchor block, level)
+  int* level_cnt;  // GT per (image, level)
+  long long bytes;
+};
+static FcosScratch fcos_scratch(const odt_tail_params&, int B, void* base) {
+  Carve c{(uintptr_t)base, 0};
+  return {c.take<float>((long long)B * kLossBlocks * kFcosLevels * 4), c.take<int>((long long)B * kFcosLevels),
+          c.bytes};
+}
+
+struct YoloScratch {
+  float* pos;          // (coord, class, obj, #GT) per image
+  float* partial;      // no-object sum per (image, anchor block)
+  unsigned char* occ;  // 1 for a cell that holds a GT, [B][N / 3]
+  long long bytes;
+};
+static YoloScratch yolo_scratch(const odt_tail_params& p, int B, void* base) {
+  Carve c{(uintptr_t)base, 0};
+  return {c.take<float>((long long)B * 4), c.take<float>((long long)B * kLossBlocks),
+          c.take<unsigned char>((long long)B * (p.N / 3)), c.bytes};
+}
+
+template <class Layout>
+static long long scratch_bytes(const odt_tail_params* p, int B, Layout layout) {
+  return p && B > 0 && p->N > 0 ? layout(*p, B, nullptr).bytes : -1;
+}
+
 }  // namespace odt
 
 using namespace odt;
 
-extern "C" long long odt_retina_loss_scratch_floats(int B) {
-  return B > 0 ? (long long)B * kLossBlocks * 4 : -1;
+extern "C" long long odt_retina_loss_scratch_bytes(const odt_tail_params* p, int B) {
+  return scratch_bytes(p, B, retina_scratch);
 }
-
-extern "C" int odt_retina_loss_fwd(const float* head, const odt_tail_params* p, int B,
-                                   const float* gt, int G, float alpha, float gamma,
-                                   float* partial_scratch, int* match_scratch, float* loss_out,
-                                   void* stream) {
-  ODT_CHECK_ARG(head && p && gt && partial_scratch && match_scratch && loss_out, "null pointer");
-  ODT_CHECK_ARG(p->kind == ODT_DECODE_SSD, "softmax-family head expected");
-  ODT_CHECK_ARG(B > 0 && G > 0 && G <= kMaxGT, "B/G (G <= 128)");
-  cudaStream_t st = (cudaStream_t)stream;
-  TailP tp;
-  tp.p = *p;
-  loss_best_anchor_kernel<<<dim3(G, B), kLossThreads, 0, st>>>(tp, gt, G, match_scratch);
-  ODT_LAUNCH_OK();
-  loss_anchor_kernel<<<dim3(kLossBlocks, B), kLossThreads, 0, st>>>(head, tp, gt, G, match_scratch,
-                                                                  alpha, gamma, partial_scratch);
-  ODT_LAUNCH_OK();
-  loss_final_kernel<<<(B + 63) / 64, 64, 0, st>>>(partial_scratch, B, loss_out);
-  ODT_LAUNCH_OK();
-  return ODT_OK;
-}
-
-// ---- SSD ----
-static long long ssd_loss_layout(const odt_tail_params* p, int B, long long* o_match, long long* o_count,
-                                 long long* o_info, long long* o_keys) {
-  long long off = (long long)B * kLossBlocks * 4 * 4;             // partial sums (floats)
-  *o_match = off;  off += (long long)B * kMaxGT * 4;              // best anchor per GT (ints)
-  *o_count = off;  off += (((long long)B + 1) & ~1ll) * 4;        // negatives per image
-  *o_info = off;   off += (((long long)B * 3 + 1) & ~1ll) * 4;    // (#pos, #neg, #selected) per image
-  off = (off + 7) & ~7ll;
-  *o_keys = off;   off += (long long)B * p->N * 8;                // negative keys (u64)
-  return off;
-}
-
 extern "C" long long odt_ssd_loss_scratch_bytes(const odt_tail_params* p, int B) {
-  if (!p || B <= 0 || p->N <= 0) return -1;
-  long long a, b2, c, d;
-  return ssd_loss_layout(p, B, &a, &b2, &c, &d);
+  return scratch_bytes(p, B, ssd_scratch);
+}
+extern "C" long long odt_fcos_loss_scratch_bytes(const odt_tail_params* p, int B) {
+  return scratch_bytes(p, B, fcos_scratch);
+}
+extern "C" long long odt_yolo_loss_scratch_bytes(const odt_tail_params* p, int B) {
+  return scratch_bytes(p, B, yolo_scratch);
 }
 
-extern "C" long long odt_ssd_loss_info_offset(const odt_tail_params* p, int B) {
-  if (!p || B <= 0 || p->N <= 0) return -1;
-  long long a, b2, c, d;
-  ssd_loss_layout(p, B, &a, &b2, &c, &d);
-  return c;
-}
-
-extern "C" int odt_ssd_loss_fwd(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
-                                void* scratch, float* loss_out, void* stream) {
+extern "C" int odt_retina_loss_fwd(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
+                                   float alpha, float gamma, void* scratch, float* loss_out, void* stream) {
   ODT_CHECK_ARG(head && p && gt && scratch && loss_out, "null pointer");
   ODT_CHECK_ARG(p->kind == ODT_DECODE_SSD, "softmax-family head expected");
   ODT_CHECK_ARG(B > 0 && G > 0 && G <= kMaxGT, "B/G (G <= 128)");
   ODT_CHECK_ARG(((uintptr_t)scratch & 7) == 0, "scratch must be 8-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
-  long long o_match, o_count, o_info, o_keys;
-  ssd_loss_layout(p, B, &o_match, &o_count, &o_info, &o_keys);
-  char* sb = static_cast<char*>(scratch);
-  float* partial = reinterpret_cast<float*>(sb);
-  int* match = reinterpret_cast<int*>(sb + o_match);
-  int* count = reinterpret_cast<int*>(sb + o_count);
-  int* info = reinterpret_cast<int*>(sb + o_info);
-  unsigned long long* keys = reinterpret_cast<unsigned long long*>(sb + o_keys);
-  ODT_CUDA_OK(cudaMemsetAsync(count, 0, sizeof(int) * (size_t)B, st));
+  const RetinaScratch s = retina_scratch(*p, B, scratch);
   TailP tp;
   tp.p = *p;
-  loss_best_anchor_kernel<<<dim3(G, B), kLossThreads, 0, st>>>(tp, gt, G, match);
+  loss_best_anchor_kernel<<<dim3(G, B), kLossThreads, 0, st>>>(tp, gt, G, s.best);
   ODT_LAUNCH_OK();
-  ssd_loss_anchor_kernel<<<dim3(kLossBlocks, B), kLossThreads, 0, st>>>(head, tp, gt, G, match, partial, keys,
-                                                                      count);
+  loss_anchor_kernel<false><<<dim3(kLossBlocks, B), kLossThreads, 0, st>>>(head, tp, gt, G, s.best, alpha, gamma,
+                                                                          s.partial, nullptr, nullptr);
   ODT_LAUNCH_OK();
-  ssd_loss_mine_kernel<<<B, kLossThreads, 0, st>>>(tp, partial, keys, count, loss_out, info);
+  loss_final_kernel<<<(B + 63) / 64, 64, 0, st>>>(s.partial, B, loss_out);
   ODT_LAUNCH_OK();
   return ODT_OK;
 }
 
-// ---- FCOS ----
-extern "C" long long odt_fcos_loss_scratch_bytes(int B) {
-  return B > 0 ? (long long)B * kLossBlocks * kFcosLevels * 4 * 4 + (long long)B * kFcosLevels * 4 : -1;
+extern "C" int odt_ssd_loss_fwd(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
+                                void* scratch, float* loss_out, int* info_out, void* stream) {
+  ODT_CHECK_ARG(head && p && gt && scratch && loss_out, "null pointer");
+  ODT_CHECK_ARG(p->kind == ODT_DECODE_SSD, "softmax-family head expected");
+  ODT_CHECK_ARG(B > 0 && G > 0 && G <= kMaxGT, "B/G (G <= 128)");
+  ODT_CHECK_ARG(((uintptr_t)scratch & 7) == 0, "scratch must be 8-byte aligned");
+  cudaStream_t st = (cudaStream_t)stream;
+  const SsdScratch s = ssd_scratch(*p, B, scratch);
+  ODT_CUDA_OK(cudaMemsetAsync(s.neg_count, 0, sizeof(int) * (size_t)B, st));
+  TailP tp;
+  tp.p = *p;
+  loss_best_anchor_kernel<<<dim3(G, B), kLossThreads, 0, st>>>(tp, gt, G, s.best);
+  ODT_LAUNCH_OK();
+  loss_anchor_kernel<true><<<dim3(kLossBlocks, B), kLossThreads, 0, st>>>(head, tp, gt, G, s.best, 0.f, 0.f,
+                                                                         s.partial, s.neg_keys, s.neg_count);
+  ODT_LAUNCH_OK();
+  ssd_loss_mine_kernel<<<B, kLossThreads, 0, st>>>(tp, s.partial, s.neg_keys, s.neg_count, loss_out, info_out);
+  ODT_LAUNCH_OK();
+  return ODT_OK;
 }
 
 extern "C" int odt_fcos_loss_fwd(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
@@ -851,22 +826,16 @@ extern "C" int odt_fcos_loss_fwd(const float* head, const odt_tail_params* p, in
   ODT_CHECK_ARG(p->kind == ODT_DECODE_FCOS && p->num_levels == kFcosLevels && p->num_fg == 20,
                 "FCOS head with 5 levels and 20 classes expected");
   ODT_CHECK_ARG(B > 0 && G > 0 && G <= kMaxGT, "B/G (G <= 128)");
+  ODT_CHECK_ARG(((uintptr_t)scratch & 7) == 0, "scratch must be 8-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
-  float* partial = static_cast<float*>(scratch);
-  int* level_cnt = reinterpret_cast<int*>(partial + (long long)B * kLossBlocks * kFcosLevels * 4);
+  const FcosScratch s = fcos_scratch(*p, B, scratch);
   TailP tp;
   tp.p = *p;
-  fcos_loss_kernel<<<dim3(kLossBlocks, B), kLossThreads, 0, st>>>(head, tp, gt, G, partial, level_cnt);
+  fcos_loss_kernel<<<dim3(kLossBlocks, B), kLossThreads, 0, st>>>(head, tp, gt, G, s.partial, s.level_cnt);
   ODT_LAUNCH_OK();
-  fcos_loss_final_kernel<<<(B + 63) / 64, 64, 0, st>>>(partial, level_cnt, B, loss_out);
+  fcos_loss_final_kernel<<<(B + 63) / 64, 64, 0, st>>>(s.partial, s.level_cnt, B, loss_out);
   ODT_LAUNCH_OK();
   return ODT_OK;
-}
-
-// ---- YOLOv3 ----
-extern "C" long long odt_yolo_loss_scratch_bytes(const odt_tail_params* p, int B) {
-  if (!p || B <= 0 || p->N <= 0) return -1;
-  return (long long)B * 4 * 4 + (long long)B * kLossBlocks * 4 + (((long long)B * (p->N / 3) + 3) & ~3ll);
 }
 
 extern "C" int odt_yolo_loss_fwd(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
@@ -877,18 +846,17 @@ extern "C" int odt_yolo_loss_fwd(const float* head, const odt_tail_params* p, in
                 "YOLOv3 head with 3 levels and 20 classes expected");
   for (int i = 0; i < kYoloLevels; ++i) ODT_CHECK_ARG(p->level[i].A == 3, "3 priors per level expected");
   ODT_CHECK_ARG(B > 0 && G > 0 && G <= kMaxGT, "B/G (G <= 128)");
+  ODT_CHECK_ARG(((uintptr_t)scratch & 7) == 0, "scratch must be 8-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
-  float* pos = static_cast<float*>(scratch);
-  float* partial = pos + (long long)B * 4;
-  unsigned char* occ = reinterpret_cast<unsigned char*>(partial + (long long)B * kLossBlocks);
-  ODT_CUDA_OK(cudaMemsetAsync(occ, 0, (size_t)B * (p->N / 3), st));
+  const YoloScratch s = yolo_scratch(*p, B, scratch);
+  ODT_CUDA_OK(cudaMemsetAsync(s.occ, 0, (size_t)B * (p->N / 3), st));
   TailP tp;
   tp.p = *p;
-  yolo_loss_pos_kernel<<<B, kMaxGT, 0, st>>>(head, tp, gt, G, occ, pos);
+  yolo_loss_pos_kernel<<<B, kMaxGT, 0, st>>>(head, tp, gt, G, s.occ, s.pos);
   ODT_LAUNCH_OK();
-  yolo_loss_noobj_kernel<<<dim3(kLossBlocks, B), kLossThreads, 0, st>>>(head, tp, gt, G, occ, partial);
+  yolo_loss_noobj_kernel<<<dim3(kLossBlocks, B), kLossThreads, 0, st>>>(head, tp, gt, G, s.occ, s.partial);
   ODT_LAUNCH_OK();
-  yolo_loss_final_kernel<<<(B + 63) / 64, 64, 0, st>>>(pos, partial, B, coord_scale, noobj_scale, obj_scale,
+  yolo_loss_final_kernel<<<(B + 63) / 64, 64, 0, st>>>(s.pos, s.partial, B, coord_scale, noobj_scale, obj_scale,
                                                        class_scale, loss_out);
   ODT_LAUNCH_OK();
   return ODT_OK;

@@ -1,5 +1,5 @@
-// Device helpers shared by the inference tail (tail.cu) and the RetinaNet loss
-// forward (loss.cu): level lookup, analytic anchors / priors, box decode.
+// Device helpers shared by the inference tail (tail.cu) and the training-loss
+// forwards (loss.cu): level lookup, analytic anchors / priors, box decode.
 #pragma once
 #include "common.cuh"
 

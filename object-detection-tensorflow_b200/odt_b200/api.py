@@ -341,6 +341,22 @@ class _Detector:
         return self.detect_stream(batches_local, precision, sharded=True, consumer=consumer)
 
     # ---- training / checkpoints (API surface; SURVEY 8f) --------------------
+    loss_kind = None  # the family's training loss: 'ssd' | 'retina' | 'yolo' | 'fcos' (engine.Tail.loss)
+
+    def _loss_scalars(self):
+        """The family's loss scalars from config, as keywords of engine.Tail.loss."""
+        return {}
+
+    def loss_forward(self, images, ground_truth, precision=None, return_info=False):
+        """Forward of the per-image training loss on the head rows the inference tail reads (what it computes:
+        the class's `loss_kind`).  ground_truth: [B,G,5] (y,x,h,w,id) padded with -1.  Returns float32 [B]; for
+        the SSD models with return_info=True also int32 [B,3] = (#positives, #negatives, #mined negatives)."""
+        images = _as_host_tensor(images)
+        net = self.engine(images.shape[0], precision)
+        net.image_buf.copy_(images)
+        net.run()
+        return net.tail.loss(net, self.loss_kind, ground_truth, return_info, **self._loss_scalars())
+
     def trainer(self):
         """The training state (variables as tensors, Momentum slots, BN moving statistics), created on first use."""
         if getattr(self, "_trainer", None) is None:
@@ -429,6 +445,8 @@ class _Detector:
 
 class SSD300(_Detector):
     name, input_size = "SSD300", 300
+    # matching, cross-entropy, smooth-L1, hard-negative mining by NMS over the negative anchors: ref SSD300.py:345-453
+    loss_kind = "ssd"
 
     def __init__(self, config, data_provider):
         self._common_init(config, data_provider)
@@ -440,33 +458,6 @@ class SSD300(_Detector):
     def _build(self, batch, precision, allow_tc=True):
         return nets.build_ssd(self.input_size, batch, self.config, precision, self.device, allow_tc)
 
-    def loss_forward(self, images, ground_truth, precision=None, return_info=False):
-        """Forward of the per-image training loss (matching, cross-entropy, smooth-L1, hard-negative
-        mining by NMS over the negative anchors) on the head rows the inference tail reads.
-        ground_truth: [B,G,5] (y,x,h,w,id) padded with -1.  ref SSD300.py:345-453."""
-        import ctypes as C
-        from . import lib as L
-        images = np.ascontiguousarray(images, dtype=np.float32)
-        gt = np.ascontiguousarray(ground_truth, dtype=np.float32)
-        net = self.engine(images.shape[0], precision)
-        B, G = gt.shape[0], gt.shape[1]
-        net.image_buf.copy_(torch.from_numpy(images))
-        net.run()
-        dev = net.device
-        gtd = torch.from_numpy(gt).to(dev)
-        nbytes = net.lib.odt_ssd_loss_scratch_bytes(C.byref(net.tail.p), B)
-        scratch = torch.zeros((nbytes + 7) // 8, dtype=torch.int64, device=dev)
-        out = torch.zeros(B, dtype=torch.float32, device=dev)
-        L.check(net.lib.odt_ssd_loss_fwd(net.head_buf.data_ptr(), C.byref(net.tail.p), B, gtd.data_ptr(), G,
-                                         scratch.data_ptr(), out.data_ptr(),
-                                         torch.cuda.current_stream().cuda_stream), "ssd_loss")
-        loss = out.cpu().numpy()
-        if not return_info:
-            return loss
-        off = net.lib.odt_ssd_loss_info_offset(C.byref(net.tail.p), B)
-        info = scratch.view(torch.int32)[off // 4: off // 4 + 3 * B].cpu().numpy().reshape(B, 3)
-        return loss, info
-
 
 class SSD512(SSD300):
     name, input_size = "SSD512", 512
@@ -474,6 +465,7 @@ class SSD512(SSD300):
 
 class RetinaNet(_Detector):
     name = "RetinaNet"
+    loss_kind = "retina"  # matching + softmax focal + smooth-L1: ref RetinaNet.py:357-474
 
     def __init__(self, config, data_provider):
         assert len(config["data_shape"]) == 3
@@ -491,34 +483,16 @@ class RetinaNet(_Detector):
     def _build(self, batch, precision, allow_tc=True):
         return nets.build_retinanet(batch, self.config, precision, self.device, allow_tc)
 
-    def loss_forward(self, images, ground_truth, precision=None):
-        """Forward of the training loss (matching + softmax focal + smooth-L1),
-        per image, on the same head rows the inference tail reads.
-        ground_truth: [B,G,5] (y,x,h,w,id) padded with -1.  ref RetinaNet.py:357-474."""
-        import ctypes as C
-        images = np.ascontiguousarray(images, dtype=np.float32)
-        gt = np.ascontiguousarray(ground_truth, dtype=np.float32)
-        net = self.engine(images.shape[0], precision)
-        B, G = gt.shape[0], gt.shape[1]
-        net.image_buf.copy_(torch.from_numpy(images))
-        net.run()
-        dev = net.device
-        gtd = torch.from_numpy(gt).to(dev)
-        nf = net.lib.odt_retina_loss_scratch_floats(B)
-        partial = torch.zeros(nf, dtype=torch.float32, device=dev)
-        match = torch.zeros(B * G, dtype=torch.int32, device=dev)
-        out = torch.zeros(B, dtype=torch.float32, device=dev)
-        from . import lib as L
-        L.check(net.lib.odt_retina_loss_fwd(net.head_buf.data_ptr(), C.byref(net.tail.p), B,
-                                            gtd.data_ptr(), G, float(self.alpha), float(self.gamma),
-                                            partial.data_ptr(), match.data_ptr(), out.data_ptr(),
-                                            torch.cuda.current_stream().cuda_stream), "retina_loss")
-        return out.cpu().numpy()
+    def _loss_scalars(self):
+        return {"alpha": self.alpha, "gamma": self.gamma}
 
 
 class YOLOv3(_Detector):
     name = "YOLOv3"
     backbone_scope = "backone"  # sic: the reference's scope name (YOLOv3.py:377)
+    # level / prior assignment, sigmoid-CE centre, class and objectness terms, squared log-size term, no-object
+    # term: ref YOLOv3.py:115-318
+    loss_kind = "yolo"
 
     def __init__(self, config, data_provider):
         assert len(config["data_shape"]) == 3
@@ -534,33 +508,16 @@ class YOLOv3(_Detector):
     def _build(self, batch, precision, allow_tc=True):
         return nets.build_yolov3(batch, self.config, precision, self.device, allow_tc)
 
-    def loss_forward(self, images, ground_truth, precision=None):
-        """Forward of the per-image training loss (level / prior assignment, sigmoid-CE centre, class and
-        objectness terms, squared log-size term, no-object term) on the head rows the inference tail
-        reads.  ground_truth: [B,G,5] (y,x,h,w,id) padded with -1.  ref YOLOv3.py:115-318."""
-        import ctypes as C
-        from . import lib as L
-        images = np.ascontiguousarray(images, dtype=np.float32)
-        gt = np.ascontiguousarray(ground_truth, dtype=np.float32)
-        net = self.engine(images.shape[0], precision)
-        B, G = gt.shape[0], gt.shape[1]
-        net.image_buf.copy_(torch.from_numpy(images))
-        net.run()
-        dev = net.device
-        gtd = torch.from_numpy(gt).to(dev)
-        nbytes = net.lib.odt_yolo_loss_scratch_bytes(C.byref(net.tail.p), B)
-        scratch = torch.zeros((nbytes + 3) // 4, dtype=torch.int32, device=dev)
-        out = torch.zeros(B, dtype=torch.float32, device=dev)
-        L.check(net.lib.odt_yolo_loss_fwd(net.head_buf.data_ptr(), C.byref(net.tail.p), B, gtd.data_ptr(), G,
-                                          float(self.coord_sacle), float(self.noobj_scale), float(self.obj_scale),
-                                          float(self.class_scale), scratch.data_ptr(), out.data_ptr(),
-                                          torch.cuda.current_stream().cuda_stream), "yolo_loss")
-        return out.cpu().numpy()
+    def _loss_scalars(self):
+        return {"coord_scale": self.coord_sacle, "noobj_scale": self.noobj_scale, "obj_scale": self.obj_scale,
+                "class_scale": self.class_scale}
 
 
 class FCOS(_Detector):
     name = "FCOS"
     backbone_scope = "backone"  # sic (FCOS.py:391)
+    # level assignment, IoU loss, centre-ness BCE, sigmoid focal loss: ref FCOS.py:153-187,266-348
+    loss_kind = "fcos"
 
     def __init__(self, config, data_provider):
         self._common_init(config, data_provider)
@@ -570,24 +527,3 @@ class FCOS(_Detector):
     def _build(self, batch, precision, allow_tc=True):
         return nets.build_fcos(batch, self.config, precision, self.device, allow_tc,
                                share_heads=self.config.get("share_heads", True))
-
-    def loss_forward(self, images, ground_truth, precision=None):
-        """Forward of the per-image training loss (level assignment, IoU loss, centre-ness BCE, sigmoid
-        focal loss) on the head rows the inference tail reads.  ground_truth: [B,G,5] (y,x,h,w,id) padded
-        with -1.  ref FCOS.py:153-187,266-348."""
-        import ctypes as C
-        from . import lib as L
-        images = np.ascontiguousarray(images, dtype=np.float32)
-        gt = np.ascontiguousarray(ground_truth, dtype=np.float32)
-        net = self.engine(images.shape[0], precision)
-        B, G = gt.shape[0], gt.shape[1]
-        net.image_buf.copy_(torch.from_numpy(images))
-        net.run()
-        dev = net.device
-        gtd = torch.from_numpy(gt).to(dev)
-        scratch = torch.zeros((net.lib.odt_fcos_loss_scratch_bytes(B) + 3) // 4, dtype=torch.int32, device=dev)
-        out = torch.zeros(B, dtype=torch.float32, device=dev)
-        L.check(net.lib.odt_fcos_loss_fwd(net.head_buf.data_ptr(), C.byref(net.tail.p), B, gtd.data_ptr(), G,
-                                          scratch.data_ptr(), out.data_ptr(),
-                                          torch.cuda.current_stream().cuda_stream), "fcos_loss")
-        return out.cpu().numpy()

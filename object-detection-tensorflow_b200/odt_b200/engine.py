@@ -953,6 +953,36 @@ class Tail:
         self.launch_decode(net, stream)
         self.launch_nms(net, stream)
 
+    # training-loss kind -> the family's scalars of odt_<kind>_loss_fwd, in argument order, with their defaults
+    LOSS_SCALARS = {"retina": (("alpha", 0.25), ("gamma", 2.0)), "ssd": (), "fcos": (),
+                    "yolo": (("coord_scale", 1.0), ("noobj_scale", 1.0), ("obj_scale", 5.0), ("class_scale", 1.0))}
+
+    def loss(self, net, kind, ground_truth, return_info=False, **kw):
+        """Training-loss forward kernels on the rows this tail reads: kind in 'retina' | 'ssd' | 'fcos' | 'yolo',
+        the family's scalars (LOSS_SCALARS) as keywords.  ground_truth [B,G,5] (y,x,h,w,id) padded with -1.
+        Returns float32 [B]; for 'ssd' with return_info=True also int32 [B,3] = (#positives, #negatives,
+        #mined negatives) per image."""
+        if kind not in self.LOSS_SCALARS:
+            raise ValueError(kind)
+        if return_info and kind != "ssd":
+            raise ValueError("return_info: only the SSD loss reports (#pos, #neg, #mined)")
+        gt = torch.as_tensor(np.ascontiguousarray(ground_truth, dtype=np.float32)).to(net.device)
+        B, G = gt.shape[0], gt.shape[1]
+        assert B == net.batch
+        p = C.byref(self.p)
+        nbytes = getattr(net.lib, "odt_%s_loss_scratch_bytes" % kind)(p, B)
+        scratch = torch.zeros((nbytes + 7) // 8, dtype=torch.int64, device=net.device)
+        out = torch.zeros(B, dtype=torch.float32, device=net.device)
+        info = torch.zeros((B, 3), dtype=torch.int32, device=net.device) if return_info else None
+        args = [float(kw.get(k, d)) for k, d in self.LOSS_SCALARS[kind]] + [scratch.data_ptr(), out.data_ptr()]
+        if kind == "ssd":
+            args.append(None if info is None else info.data_ptr())
+        L.check(getattr(net.lib, "odt_%s_loss_fwd" % kind)(self.head_buf.data_ptr(), p, B, gt.data_ptr(), G, *args,
+                                                          torch.cuda.current_stream().cuda_stream), kind + "_loss")
+        if return_info:
+            return out.cpu().numpy(), info.cpu().numpy()
+        return out.cpu().numpy()
+
     def num_launches(self):
         return 2  # decode + NMS kernels (plus 3 memset nodes)
 
@@ -1028,47 +1058,8 @@ class RowsHarness:
         return [anc[b, :cnt[b]].copy() for b in range(self.batch)]
 
     def loss(self, kind, ground_truth, return_info=False, **kw):
-        """Training-loss forward kernels on the same rows: kind in 'retina' | 'ssd' | 'fcos' | 'yolo'.
-        ground_truth [B,G,5] (y,x,h,w,id) padded with -1.  Returns float32 [B]; for 'ssd' with
-        return_info=True also int32 [B,3] = (#positives, #negatives, #mined negatives) per image."""
-        gt = torch.as_tensor(np.ascontiguousarray(ground_truth, dtype=np.float32)).to(self.device)
-        B, G = gt.shape[0], gt.shape[1]
-        assert B == self.batch
-        if return_info and kind != "ssd":
-            raise ValueError("return_info: only the SSD loss reports (#pos, #neg, #mined)")
-        st = torch.cuda.current_stream().cuda_stream
-        out = torch.zeros(B, dtype=torch.float32, device=self.device)
-        p = C.byref(self.tail.p)
-        if kind == "retina":
-            partial = torch.zeros(self.lib.odt_retina_loss_scratch_floats(B), dtype=torch.float32, device=self.device)
-            match = torch.zeros(B * G, dtype=torch.int32, device=self.device)
-            L.check(self.lib.odt_retina_loss_fwd(self.head_buf.data_ptr(), p, B, gt.data_ptr(), G,
-                                                 float(kw.get("alpha", 0.25)), float(kw.get("gamma", 2.0)),
-                                                 partial.data_ptr(), match.data_ptr(), out.data_ptr(), st), "retina_loss")
-        elif kind == "ssd":
-            scratch = torch.zeros((self.lib.odt_ssd_loss_scratch_bytes(p, B) + 7) // 8, dtype=torch.int64,
-                                  device=self.device)
-            L.check(self.lib.odt_ssd_loss_fwd(self.head_buf.data_ptr(), p, B, gt.data_ptr(), G, scratch.data_ptr(),
-                                              out.data_ptr(), st), "ssd_loss")
-            if return_info:
-                off = self.lib.odt_ssd_loss_info_offset(p, B)
-                info = scratch.view(torch.int32)[off // 4: off // 4 + 3 * B].cpu().numpy().reshape(B, 3)
-                return out.cpu().numpy(), info
-        elif kind == "fcos":
-            scratch = torch.zeros((self.lib.odt_fcos_loss_scratch_bytes(B) + 3) // 4, dtype=torch.int32,
-                                  device=self.device)
-            L.check(self.lib.odt_fcos_loss_fwd(self.head_buf.data_ptr(), p, B, gt.data_ptr(), G, scratch.data_ptr(),
-                                               out.data_ptr(), st), "fcos_loss")
-        elif kind == "yolo":
-            scratch = torch.zeros((self.lib.odt_yolo_loss_scratch_bytes(p, B) + 3) // 4, dtype=torch.int32,
-                                  device=self.device)
-            L.check(self.lib.odt_yolo_loss_fwd(self.head_buf.data_ptr(), p, B, gt.data_ptr(), G,
-                                               float(kw.get("coord_scale", 1.0)), float(kw.get("noobj_scale", 1.0)),
-                                               float(kw.get("obj_scale", 5.0)), float(kw.get("class_scale", 1.0)),
-                                               scratch.data_ptr(), out.data_ptr(), st), "yolo_loss")
-        else:
-            raise ValueError(kind)
-        return out.cpu().numpy()
+        """Training-loss forward kernels on the same rows (Tail.loss)."""
+        return self.tail.loss(self, kind, ground_truth, return_info, **kw)
 
 
 # ------------------------------------------------------------------ weights --

@@ -15,7 +15,7 @@ DECODE_SSD, DECODE_YOLO3, DECODE_FCOS = 0, 1, 2
 MAX_LEVELS, MAX_PRIORS = 8, 9
 ERR_OVERFLOW = -4
 ERR_UNSUPPORTED = -3
-ABI_VERSION = 4  # odt_abi_version(): bumped whenever a signature in include/odt_b200.h changes
+ABI_VERSION = 5  # odt_abi_version(): bumped whenever a signature in include/odt_b200.h changes
 
 
 class ConvParams(C.Structure):
@@ -84,14 +84,13 @@ SYMBOLS = {
     "odt_decode_candidates": (_I, [_P, C.POINTER(TailParams), _I, _P, _P, _P]),
     "odt_nms_per_class": (_I, [_P, C.POINTER(TailParams), _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _L, _L, _P]),
     "odt_nms_scratch_bytes": (_L, [C.POINTER(TailParams), _I]),
-    "odt_retina_loss_fwd": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _F, _F, _P, _P, _P, _P]),
-    "odt_retina_loss_scratch_floats": (_L, [_I]),
+    "odt_retina_loss_scratch_bytes": (_L, [C.POINTER(TailParams), _I]),
+    "odt_retina_loss_fwd": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _F, _F, _P, _P, _P]),
     "odt_ssd_loss_scratch_bytes": (_L, [C.POINTER(TailParams), _I]),
-    "odt_ssd_loss_info_offset": (_L, [C.POINTER(TailParams), _I]),
-    "odt_ssd_loss_fwd": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _P, _P, _P]),
+    "odt_ssd_loss_fwd": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _P, _P, _P, _P]),
     "odt_yolo_loss_scratch_bytes": (_L, [C.POINTER(TailParams), _I]),
     "odt_yolo_loss_fwd": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _F, _F, _F, _F, _P, _P, _P]),
-    "odt_fcos_loss_scratch_bytes": (_L, [_I]),
+    "odt_fcos_loss_scratch_bytes": (_L, [C.POINTER(TailParams), _I]),
     "odt_fcos_loss_fwd": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _P, _P, _P]),
     "odt_ctx_unique_id": (_I, [_P]),
     "odt_ctx_create": (_I, [C.POINTER(_P), _I, _I, _P]),

@@ -461,28 +461,29 @@ def test_loss_entry_points_reject_bad_arguments_without_gpu(built):
         return rc == -1 and b"invalid argument" in L.odt_last_error()
 
     ssd, fcos, yolo = params(lib.DECODE_SSD, 1), params(lib.DECODE_FCOS, 5), params(lib.DECODE_YOLO3, 3)
-    retina = lambda p, B, G: L.odt_retina_loss_fwd(fake, ctypes.byref(p), B, fake, G, 0.25, 2.0, fake, fake,
-                                                   fake, None)
+    retina = lambda p, B, G, scratch=fake: L.odt_retina_loss_fwd(fake, ctypes.byref(p), B, fake, G, 0.25, 2.0,
+                                                                 scratch, fake, None)
     ssd_fwd = lambda p, B, G, scratch=fake: L.odt_ssd_loss_fwd(fake, ctypes.byref(p), B, fake, G, scratch, fake,
-                                                               None)
-    fcos_fwd = lambda p, B, G: L.odt_fcos_loss_fwd(fake, ctypes.byref(p), B, fake, G, fake, fake, None)
-    yolo_fwd = lambda p, B, G: L.odt_yolo_loss_fwd(fake, ctypes.byref(p), B, fake, G, 1.0, 1.0, 5.0, 1.0, fake,
-                                                   fake, None)
+                                                               None, None)
+    fcos_fwd = lambda p, B, G, scratch=fake: L.odt_fcos_loss_fwd(fake, ctypes.byref(p), B, fake, G, scratch, fake,
+                                                                 None)
+    yolo_fwd = lambda p, B, G, scratch=fake: L.odt_yolo_loss_fwd(fake, ctypes.byref(p), B, fake, G, 1.0, 1.0, 5.0,
+                                                                 1.0, scratch, fake, None)
     for fwd, p in ((retina, ssd), (ssd_fwd, ssd), (fcos_fwd, fcos), (yolo_fwd, yolo)):
         for B, G in ((1, 0), (1, 129), (0, 4), (-1, 4)):
             assert rejected(fwd(p, B, G)), (fwd, B, G)
         wrong = yolo if p is not yolo else ssd
         assert rejected(fwd(wrong, 1, 4)), "wrong head kind"
+        assert rejected(fwd(p, 1, 4, scratch=ctypes.c_void_p(68))), "unaligned scratch"
     assert rejected(fcos_fwd(params(lib.DECODE_FCOS, 3), 1, 4)), "FCOS level count"
     assert rejected(yolo_fwd(params(lib.DECODE_YOLO3, 2), 1, 4)), "YOLO level count"
     assert rejected(yolo_fwd(params(lib.DECODE_YOLO3, 3, A=2), 1, 4)), "YOLO priors per level"
-    assert rejected(ssd_fwd(ssd, 1, 4, scratch=ctypes.c_void_p(68))), "unaligned SSD scratch"
-    for B in (0, -3):
-        assert L.odt_retina_loss_scratch_floats(B) == -1
-        assert L.odt_ssd_loss_scratch_bytes(ctypes.byref(ssd), B) == -1
-        assert L.odt_ssd_loss_info_offset(ctypes.byref(ssd), B) == -1
-        assert L.odt_fcos_loss_scratch_bytes(B) == -1
-        assert L.odt_yolo_loss_scratch_bytes(ctypes.byref(yolo), B) == -1
+    for family, p in (("retina", ssd), ("ssd", ssd), ("fcos", fcos), ("yolo", yolo)):
+        size = getattr(L, "odt_%s_loss_scratch_bytes" % family)
+        for B in (0, -3):
+            assert size(ctypes.byref(p), B) == -1, (family, B)
+        assert size(None, 2) == -1, family
+        assert size(ctypes.byref(p), 2) > 0, family
 
 
 # ------------------------------------------------------------------- GPU ------

@@ -24,7 +24,7 @@ def test_library_exports_every_declared_symbol(built):
         assert hasattr(so, name), "symbol %s declared in include/odt_b200.h is not exported" % name
     assert declared == set(lib.SYMBOLS), declared ^ set(lib.SYMBOLS)
     L = lib.load()
-    assert L.odt_abi_version() == 4
+    assert L.odt_abi_version() == 5
 
 
 def test_same_pad_abi_matches_host_and_oracle(built):
