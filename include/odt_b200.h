@@ -249,8 +249,9 @@ int odt_decode_candidates(const float* head, const odt_tail_params* p, int B,
  * fixed-size record [B, D*6+2] that one all-gather / one device->host copy ships.  work: i32 [round_up(B,2) + 2] zero-initialised, 8-byte aligned scratch
  * (per-image completion counters reset by the kernel, then the 64-bit bump pointer
  * of the box pool).  box_pool: optional f32 [box_pool_entries][4]
- * scratch where lists longer than the 4096-entry shared-memory window cache their
- * decoded boxes (NULL / exhausted -> boxes are re-decoded every round).
+ * scratch where lists longer than the 1024-entry shared-memory window cache their
+ * decoded boxes when they take the full-list path (the prefilter subset ran dry, or more
+ * than 1024 scores tie at the top); NULL / exhausted -> boxes are re-decoded every round.
  * ref: SSD300.py:173-190; RetinaNet.py:240-256; YOLOv3.py:352-368; FCOS.py:249-264 */
 int odt_nms_per_class(const float* head, const odt_tail_params* p, int B,
                       unsigned long long* cand_keys, const int* cand_count, float* dets,

@@ -84,8 +84,10 @@ def test_tail_empty_and_single(built):
     assert list(res[2]) == [3] and list(h.keep_indices()[0]) == [700]
 
 
-def test_tail_spill_path_more_than_smem_candidates(built):
-    """> 4096 candidates per class: in-place global-memory sort path."""
+def test_tail_prefilter_subset_on_lists_longer_than_smem(built):
+    """6 912 random-score candidates per class (longer than the 1 024-entry shared-memory window): every list
+    runs on its radix-select prefilter subset in shared memory, which yields max_boxes boxes, so no list takes
+    the full-list path: the box-pool bump counter (int64 behind the per-image counters in `work`) stays 0."""
     from golden import make_golden as mg
     from odt_b200.engine import RowsHarness
     name = "tail_yolo"
@@ -96,6 +98,8 @@ def test_tail_spill_path_more_than_smem_candidates(built):
         assert rows.shape[1] == 6912
         h = RowsHarness(_tail_for(name, case), case["levels"], rows)
         res, keep = h.run(), h.keep_indices()
+        assert np.all(h.tail.cand_count.cpu().numpy() == 6912) and h.tail.box_pool is not None
+        assert int(h.tail.work.cpu().numpy()[2:4].view(np.int64)[0]) == 0, "a list took the full-list path"
         for b in range(2):
             _check(res[b], keep[b], mg.run_case("_spill", rows, image=b))
     finally:
