@@ -139,6 +139,9 @@ typedef struct {
  * RetinaNet.py:579,599,609, YOLOv3.py:495, FCOS.py:449,469,479; the fused
  * epilogue is bias_add/BN/ReLU SSD300.py:520-521,534-537 */
 int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_conv_params* p, void* stream);
+/* the N tile (32 .. 128, or 256) odt_conv2d_f16_tc picks for an im2col-mode layer of M = B*OH*OW output
+ * pixels, Cout_pad channels and kblocks = R*S*in_ld/64 K blocks (host only; honours ODT_TC_WIDE) */
+int odt_conv_tc_pick_bn(int cout_pad, long long M, int kblocks);
 /* generic direct convolution on CUDA cores: any Cin/Cout/filter; `dtype` is
  * the activation dtype (ODT_F32: reference-precision path, ODT_F16: stems and
  * shapes the tensor-core kernel does not take).  Same call sites as above. */

@@ -45,6 +45,11 @@ int pw_mode() {
   const char* e = getenv("ODT_TC_PW");
   return (e && e[0] >= '0' && e[0] <= '2') ? e[0] - '0' : 1;
 }
+int wide_mode() {
+  // conv_tc's 128 x 256 tile: 0 = off, 1 = where pick_bn's cost model takes it (default), 2 = wherever Cout_pad % 256 == 0
+  const char* e = getenv("ODT_TC_WIDE");  // read every call: lets one process compare both tiles
+  return (e && e[0] >= '0' && e[0] <= '2') ? e[0] - '0' : 1;
+}
 bool wres_enabled() {
   const char* e = getenv("ODT_TC_WRES");
   return !(e && e[0] == '0');

@@ -89,6 +89,7 @@ cudaError_t launch_pdl(void (*kern)(KArgs...), unsigned grid, int block, int sme
 
 bool flat_enabled();  // ODT_TC_FLAT=0 disables the halo-flat 3x3 path (A/B measurements)
 bool kskip_enabled();  // ODT_TC_KSKIP=1: do not issue the all-zero 16-deep K steps of thin layers (Cin padded to 64)
+int wide_mode();     // ODT_TC_WIDE: conv_tc's 128 x 256 im2col tile, 0 off / 1 cost model (default) / 2 always
 int thin_mode();       // ODT_TC_THIN: 1 = very thin layers (Cin, Cout <= 32, few multiply-adds per pixel) go through the
                        // CUDA-core kernel of conv_thin.cu, 2 = wherever the layer qualifies, 0 / unset = never
 int tapn_mode();       // ODT_TC_TAPN: 1 = narrow 3x3 halo layers go through conv_tapn.cu (taps folded into N) where its

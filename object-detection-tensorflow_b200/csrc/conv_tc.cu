@@ -20,6 +20,11 @@
 //   their mainloops strictly alternate, so one warpgroup's epilogue runs while the other's MMAs
 //   keep the tensor pipe busy.  A pipeline stage goes back to the producer as soon as the MMAs
 //   that read it have retired (one wgmma group kept in flight).
+//   Wide im2col layers (Cout_pad % 256 == 0, where pick_bn's cost model says so) run 128 x 256
+//   tiles instead: both warpgroups on every tile, one m64n256k16 per K step on their own 64-row
+//   half, each ring stage consumed by both.  A quarter fewer operand bytes per multiply-add reach
+//   shared memory, which lifts the feed-bound mainloop to near the dense wgmma rate; the epilogue
+//   is then exposed once per tile, shared by all 256 consumer threads.
 // * Epilogue: the accumulators pass, one 32-column slice at a time, through a per-warpgroup fp32
 //   buffer in shared memory so that every epilogue lane owns one pixel row: folded bias/BN
 //   scale+shift, activation, residual, up to two extra pre-activated outputs, fused max-pool,
@@ -51,12 +56,20 @@ constexpr int TC_EPI_PAR = 7 * TC_MAX_BN;  // floats per parameter block: epi_pa
 constexpr int TC_SLICE_PITCH = 36;
 constexpr int TC_SLICE_FLOATS = TC_BM * TC_SLICE_PITCH;
 constexpr int TC_EPI_SMEM = 2 * (TC_EPI_PAR + TC_SLICE_FLOATS) * 4;  // per consumer warpgroup: parameters + slice
+// Wide tile (BN = 256, im2col mode): both consumer warpgroups work on one 128 x 256 tile, warpgroup g on rows
+// 64g .. 64g+63 (one m64n256 accumulator set each).  Epilogue: one parameter block of 256 columns shared by the two
+// warpgroups, then per warpgroup a [64 rows x 32 columns] slice in which two lanes share a pixel row (16 columns each).
+constexpr int TC_WIDE_BN = 256;
+constexpr int TC_WIDE_SLICE_FLOATS = (TC_BM / 2) * TC_SLICE_PITCH;
+constexpr int TC_WIDE_EPI_SMEM = (7 * TC_WIDE_BN + 2 * TC_WIDE_SLICE_FLOATS) * 4;
 constexpr int TC_MAX_STAGES = 8;
 constexpr int TC_A_BYTES = TC_BM * TC_BK * 2;  // 16 KiB
 constexpr int TC_SMEM_LIMIT = 232448;          // 227 KiB
 // named barriers: 1 + g = the 128 threads of consumer warpgroup g; 3 + g = "warpgroup g may start its mainloop"
+// (ping-pong); 5 = all 256 consumer threads (the wide tile's shared parameter block)
 constexpr int TC_BAR_EPI = 1;
 constexpr int TC_BAR_ORDER = 3;
+constexpr int TC_BAR_WIDE = 5;
 
 struct TcGeom {
   long long M;  // B*OH*OW
@@ -112,12 +125,31 @@ __device__ __forceinline__ void tl_stamp(int role, int event, int tile) {
 #else
 #define tl_stamp(role, event, tile) ((void)0)
 #endif
+// Bound probes of the timeline build (wrong results by design, never in the product library):
+//   -DODT_TC_PROBE_FEED: the consumers wait for each stage and hand it back without issuing MMAs (the feed's rate);
+//   -DODT_TC_PROBE_MMA:  the producer loads nothing and the consumers do not wait (the MMAs' rate on stale operands).
+#if defined(ODT_TC_PROBE_FEED) || defined(ODT_TC_PROBE_MMA)
+#ifndef ODT_TC_TIMELINE
+#error "the bound probes belong to the -DODT_TC_TIMELINE build"
+#endif
+#endif
+#ifdef ODT_TC_PROBE_FEED
+constexpr bool TC_ISSUE_MMA = false;
+#else
+constexpr bool TC_ISSUE_MMA = true;
+#endif
+#ifdef ODT_TC_PROBE_MMA
+constexpr bool TC_FEED = false;
+#else
+constexpr bool TC_FEED = true;
+#endif
 
 // --------------------------------------------------------------- kernel ----
 template <int BN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
     conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                    const __grid_constant__ TcGeom g, const __grid_constant__ Epi e) {
+  constexpr bool WIDE = BN > TC_MAX_BN;  // the cooperative 128 x 256 tile (im2col mode only)
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // carve (base rounded up to 1024 for the 128B swizzle atoms)
   const uint32_t raw = smem_u32(smem_raw);
@@ -143,7 +175,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
     for (int s = 0; s < stages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 4);  // one arrival per warp of the consuming warpgroup
+      mbar_init(empty_bar(s), WIDE ? 8 : 4);  // one arrival per warp of the consuming warpgroup(s)
     }
     mbar_init(wfull_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -227,8 +259,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
       for (int r = 0; r < g.R; ++r) {
         for (int s = 0; s < g.S; ++s) {
           for (int cc = 0; cc < g.cchunks; ++cc) {
-            mbar_wait(empty_bar(stage), phase ^ 1u);
-            if (elect_one()) {
+            if (TC_FEED) mbar_wait(empty_bar(stage), phase ^ 1u);
+            if (TC_FEED && elect_one()) {
               mbar_expect_tx(full_bar(stage), a_bytes + b_bytes);
               tma_load_im2col(a_base + (uint32_t)stage * a_bytes, &tmA, full_bar(stage),
                               cc * TC_BK, cw, ch, img, (uint16_t)(s * g.dil),
@@ -248,26 +280,33 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   } else {
     wg_reg_alloc<TC_CONSUMER_REGS>();
     // ===================== consumer warpgroups ===============================
-    // Warpgroup `group` owns the tiles i = group, group + 2, ... of the CTA's list, all 128 rows
-    // (acc[h] = rows 64*h .. +63).  Its mainloop starts once the other warpgroup has issued every
-    // MMA of the previous tile, so the k-blocks reach the ring's stages in the producer's order.
-    // Epilogue: warp `quarter` of the group owns pixel rows 32*quarter .. +31 (one per lane).
+    // BN <= 128 (ping-pong): warpgroup `group` owns the tiles i = group, group + 2, ... of the CTA's
+    // list, all 128 rows (acc[h] = rows 64*h .. +63).  Its mainloop starts once the other warpgroup
+    // has issued every MMA of the previous tile, so the k-blocks reach the ring's stages in the
+    // producer's order.  Epilogue: warp `quarter` of the group owns pixel rows 32*quarter .. +31
+    // (one per lane), 32 columns per slice.
+    // BN = 256 (wide): both warpgroups take every tile and consume every stage together, warpgroup
+    // `group` on rows 64*group .. +63 (acc[0]).  Epilogue: warps quarter&1 own rows 32*(quarter&1)
+    // .. +31 of the group's half, quarter>>1 picks the 16-column half of each 32-column slice.
+    constexpr int EW = WIDE ? 16 : 32;               // columns one epilogue lane handles per slice
+    constexpr int P = WIDE ? TC_WIDE_BN : TC_MAX_BN;  // parameter block stride
     const int quarter = warp & 3;
     const int group = (warp - 4) >> 2;
     const int et = threadIdx.x - 128 * (1 + group);  // index among the warpgroup's 128 threads
     const int epi_bar = TC_BAR_EPI + group;
-    float* par = epi_smem + group * (TC_EPI_PAR + TC_SLICE_FLOATS);
-    float* slice = par + TC_EPI_PAR;
-    constexpr int P = TC_MAX_BN;  // parameter block stride
+    float* par = WIDE ? epi_smem : epi_smem + group * (TC_EPI_PAR + TC_SLICE_FLOATS);
+    float* slice = WIDE ? epi_smem + 7 * P + group * TC_WIDE_SLICE_FLOATS : par + TC_EPI_PAR;
+    const int erow = WIDE ? 32 * (quarter & 1) + lane : 32 * quarter + lane;  // this lane's row of the slice
+    const int ecol = WIDE ? 16 * (quarter >> 1) : 0;                          // and its first column
     int staged_n_tile = -1;
     int stage = 0;
     uint32_t phase = 0;
     int cc_mma = 0;  // channel chunk of the current k-block (the k-block order ends with the chunk index)
-    float acc[2][BN / 2];
+    float acc[WIDE ? 1 : 2][BN / 2];
     if (g.bres) mbar_wait(wfull_bar, 0);
     int i = 0;  // position of `tile` in the CTA's list
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++i) {
-      if ((i & 1) != group) {  // the other warpgroup's tile: its k-blocks pass through the ring
+      if (!WIDE && (i & 1) != group) {  // the other warpgroup's tile: its k-blocks pass through the ring
         const int adv = stage + kblocks;
         stage = adv % stages;
         phase ^= (uint32_t)(adv / stages) & 1u;
@@ -275,33 +314,40 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
       }
       const int n_tile = tile % g.num_n_tiles;
       const int m_tile = tile / g.num_n_tiles;
-      if (i > 0) named_bar_sync(TC_BAR_ORDER + group, 256);
+      if (!WIDE && i > 0) named_bar_sync(TC_BAR_ORDER + group, 256);
       if (quarter == 0) tl_stamp(1 + group, 0, tile);  // mainloop start
       int prev = -1;
       for (int kb = 0; kb < kblocks; ++kb) {
-        mbar_wait(full_bar(stage), phase);
+        if (TC_FEED) mbar_wait(full_bar(stage), phase);
         const uint32_t a_stage = a_base + (uint32_t)stage * a_bytes;
-        const uint64_t adesc0 = make_desc_sw128(a_stage), adesc1 = make_desc_sw128(a_stage + 64u * 128u);
-        // resident bank: tile ((r*3 + s)*cchunks + cc) with kb = r*cchunks + cc
-        const uint64_t bdesc = make_desc_sw128(
-            g.bres ? b_base + (uint32_t)((kb / g.cchunks) * 3 * g.cchunks + kb % g.cchunks) * (uint32_t)BN * 128u
-                   : b_base + (uint32_t)stage * b_bytes);
         // 16-deep K steps of this chunk that hold real channels (see TcGeom::klast)
         // (broadcast from lane 0 so that ptxas sees a warp-uniform count)
         const int ksteps = __shfl_sync(0xffffffffu, (cc_mma == g.cchunks - 1) ? g.klast : TC_BK / 16, 0);
         if (++cc_mma == g.cchunks) cc_mma = 0;
-        wg_fence();
-        if (g.flat) {
-          // three horizontal taps from the same slab: operand rows s .. s+63 of the half, i.e. the
-          // descriptor start shifted by s*128 B inside the 1024 B swizzle pattern
-          const uint64_t bstep = (uint64_t)(((uint32_t)(g.bres ? g.cchunks : 1) * (uint32_t)BN * 128u) >> 4);
-          const uint64_t astep = (uint64_t)(g.flat == 2 ? 8 * g.RP : 8);  // rows per tap shift x 128 B >> 4
+        if (TC_ISSUE_MMA) {
+          wg_fence();
+          if constexpr (WIDE) {
+            wg_mma_chunk<BN>(acc[0], make_desc_sw128(a_stage + (uint32_t)group * 64u * 128u),
+                             make_desc_sw128(b_base + (uint32_t)stage * b_bytes), ksteps, kb == 0);
+          } else {
+            const uint64_t adesc0 = make_desc_sw128(a_stage), adesc1 = make_desc_sw128(a_stage + 64u * 128u);
+            // resident bank: tile ((r*3 + s)*cchunks + cc) with kb = r*cchunks + cc
+            const uint64_t bdesc = make_desc_sw128(
+                g.bres ? b_base + (uint32_t)((kb / g.cchunks) * 3 * g.cchunks + kb % g.cchunks) * (uint32_t)BN * 128u
+                       : b_base + (uint32_t)stage * b_bytes);
+            if (g.flat) {
+              // three horizontal taps from the same slab: operand rows s .. s+63 of the half, i.e. the
+              // descriptor start shifted by s*128 B inside the 1024 B swizzle pattern
+              const uint64_t bstep = (uint64_t)(((uint32_t)(g.bres ? g.cchunks : 1) * (uint32_t)BN * 128u) >> 4);
+              const uint64_t astep = (uint64_t)(g.flat == 2 ? 8 * g.RP : 8);  // rows per tap shift x 128 B >> 4
 #pragma unroll
-          for (int s3 = 0; s3 < 3; ++s3)
-            wg_mma_chunk2<BN>(acc[0], acc[1], adesc0 + astep * s3, adesc1 + astep * s3, bdesc + bstep * s3, ksteps,
-                              (kb | s3) == 0);
-        } else {
-          wg_mma_chunk2<BN>(acc[0], acc[1], adesc0, adesc1, bdesc, ksteps, kb == 0);
+              for (int s3 = 0; s3 < 3; ++s3)
+                wg_mma_chunk2<BN>(acc[0], acc[1], adesc0 + astep * s3, adesc1 + astep * s3, bdesc + bstep * s3,
+                                  ksteps, (kb | s3) == 0);
+            } else {
+              wg_mma_chunk2<BN>(acc[0], acc[1], adesc0, adesc1, bdesc, ksteps, kb == 0);
+            }
+          }
         }
         wg_commit();
         wg_wait<1>();  // the previous k-block's MMAs have retired: its stage goes back to the producer
@@ -313,12 +359,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         }
       }
       // every MMA of this tile is issued: the other warpgroup's mainloop may start
-      if (tile + (int)gridDim.x < num_tiles) named_bar_arrive(TC_BAR_ORDER + (group ^ 1), 256);
+      if (!WIDE && tile + (int)gridDim.x < num_tiles) named_bar_arrive(TC_BAR_ORDER + (group ^ 1), 256);
       wg_wait<0>();
       if (lane == 0) mbar_arrive(empty_bar(prev));
       if (quarter == 0) tl_stamp(1 + group, 1, tile);  // accumulators complete
 
-      const long long m = (long long)m_tile * TC_BM + quarter * 32 + lane;
+      const long long m = (long long)m_tile * TC_BM + (WIDE ? 64 * group : 0) + erow;
       bool row_ok;
       int img, pix;
       long long pool_row = 0;  // element offset of this lane's pooled pixel (flat == 2)
@@ -353,6 +399,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
       // consecutive tiles of single-N-tile layers reuse them
       const bool new_par = n_tile != staged_n_tile;
       staged_n_tile = n_tile;
+      if (WIDE && new_par) {
+        // the shared block: both warpgroups have finished reading the previous one, then stage column t
+        const int t = threadIdx.x - 128;
+        named_bar_sync(TC_BAR_WIDE, 256);
+#pragma unroll
+        for (int row = 0; row < 6; ++row) par[row * P + t] = epi_param(e, row, n0 + t);
+        reinterpret_cast<int*>(par)[6 * P + t] = n0 + t < e.Cout ? regroup(e, n0 + t) : 0;
+        named_bar_sync(TC_BAR_WIDE, 256);
+      }
       long long o0_row = (long long)img * e.out0_img_stride;
       if (g.out_halo) {
         const int oy = pix / g.OW, ox = pix - oy * g.OW;
@@ -362,36 +417,41 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
       }
       const long long o1_row = aux_row(e.out1_img_stride, e.out1_pix_stride, e.out1_halo, g.OW, img, pix);
       const long long o2_row = aux_row(e.out2_img_stride, e.out2_pix_stride, e.out2_halo, g.OW, img, pix);
-      const float* my_acc = slice + (quarter * 32 + lane) * TC_SLICE_PITCH;
+      const float* my_acc = slice + erow * TC_SLICE_PITCH + ecol;
       for (int j = 0; j < BN / 32; ++j) {
-        const int nb = n0 + j * 32;
-        if (nb >= e.Cout) break;  // fully padded chunk (uniform)
+        if (n0 + j * 32 >= e.Cout) break;  // fully padded chunk (uniform)
+        const int nb = n0 + j * 32 + ecol;  // this lane's first column
         // every lane of the warpgroup has finished reading the previous slice and, on a new tile, the parameters
         named_bar_sync(epi_bar, 128);
-        if (j == 0 && new_par) {
+        if (!WIDE && j == 0 && new_par) {
           const int n = et < BN ? n0 + et : e.Cout;  // columns past the tile: identity
 #pragma unroll
           for (int row = 0; row < 6; ++row) par[row * P + et] = epi_param(e, row, n);
           reinterpret_cast<int*>(par)[6 * P + et] = n < e.Cout ? regroup(e, n) : 0;
         }
-        wg_acc_slice_to_smem<BN>(acc[0], j, slice, TC_SLICE_PITCH, 0);
-        wg_acc_slice_to_smem<BN>(acc[1], j, slice, TC_SLICE_PITCH, 64);
+        if constexpr (WIDE) {
+          wg_acc_slice_to_smem<BN>(acc[0], j, slice, TC_SLICE_PITCH, 0);
+        } else {
+          wg_acc_slice_to_smem<BN>(acc[0], j, slice, TC_SLICE_PITCH, 0);
+          wg_acc_slice_to_smem<BN>(acc[1], j, slice, TC_SLICE_PITCH, 64);
+        }
         named_bar_sync(epi_bar, 128);
         float v[32];
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
+        for (int i = 0; i < EW / 4; ++i) {
           const float4 t = *reinterpret_cast<const float4*>(my_acc + 4 * i);
           v[4 * i + 0] = t.x;
           v[4 * i + 1] = t.y;
           v[4 * i + 2] = t.z;
           v[4 * i + 3] = t.w;
         }
-        if (g.flat == 2) {
+        const float* ps = par + j * 32 + ecol;  // this lane's parameter columns
+        if (!WIDE && g.flat == 2) {
           // fused 2x2/2 max pooling: bias/BN + activation, round to fp16, then the maximum over
           // the window's four lanes (vertical neighbour = lane^1, horizontal = lane^RP); each
           // of the four lanes stores one 8-channel quarter of the pooled pixel
           uint4 packed[4];
-          epi_act_f16<4>(v, par + j * 32, P, e.act, packed);
+          epi_act_f16<4>(v, ps, P, e.act, packed);
           uint32_t* pw = reinterpret_cast<uint32_t*>(packed);
 #pragma unroll
           for (int i = 0; i < 16; ++i) {
@@ -405,26 +465,25 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
           const uint4 sel = pool_q == 0 ? packed[0] : pool_q == 1 ? packed[1] : pool_q == 2 ? packed[2] : packed[3];
           if (row_ok && nb + 8 * pool_q < g.fast_cols)
             *reinterpret_cast<uint4*>(reinterpret_cast<__half*>(e.out0) + pool_row + nb + 8 * pool_q) = sel;
-        } else if (g.fast_store && nb + 32 <= g.fast_cols) {
+        } else if (g.fast_store && nb + EW <= g.fast_cols) {
           if (row_ok) {
             const long long o0 = o0_row + nb;
             const uint4* rp = reinterpret_cast<const uint4*>(reinterpret_cast<const __half*>(e.residual) + o0);
-            epi_store_f16<4>(e, v, par + j * 32, P, [&](int q) { return __ldg(rp + q); }, o0, o1_row + nb,
-                             o2_row + nb);
+            epi_store_f16<EW / 8>(e, v, ps, P, [&](int q) { return __ldg(rp + q); }, o0, o1_row + nb, o2_row + nb);
           }
         } else if (row_ok || g.head_mode) {
           // generic path: fp32 head outputs scattered into the candidate rows,
           // channel regrouping, ragged Cout; parameters come from shared memory
-          const float* ps = par + j * 32;
-          const int* pofs = reinterpret_cast<const int*>(par) + 6 * P + j * 32;
-          const int nvalid = min(32, e.Cout - nb);
+          const int* pofs = reinterpret_cast<const int*>(par) + 6 * P + j * 32 + ecol;
+          const int nvalid = min(EW, e.Cout - nb);
           if (g.head_mode) {
             // head convolutions: fp32 scatter into the candidate rows.  The staged accumulator
             // slice is read column-wise, so the warp writes one row per instruction with the
             // lanes on consecutive channels (4-5 sectors per request instead of 32).
-            const float* acol = slice + (quarter * 32) * TC_SLICE_PITCH + lane;
-            const float sc = ps[lane], sh = ps[P + lane];
-            const int my_ofs = pofs[lane];
+            const int cl = lane < EW ? lane : 0;  // this lane's column (lanes past EW store nothing)
+            const float* acol = slice + (erow - lane) * TC_SLICE_PITCH + ecol + cl;
+            const float sc = ps[cl], sh = ps[P + cl];
+            const int my_ofs = pofs[cl];
             const long long my_row = row_ok ? o0_row : -1;
             float* obase = reinterpret_cast<float*>(e.out0);
 #pragma unroll 4
@@ -435,7 +494,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
             }
           } else {
 #pragma unroll
-            for (int i = 0; i < 32; ++i) {
+            for (int i = 0; i < EW; ++i) {
               if (i >= nvalid) break;
               const int n = nb + i;
               float x = apply_act(fmaf(v[i], ps[i], ps[P + i]), e.act);
@@ -573,6 +632,15 @@ using namespace odt;
 // The constants are estimates from the instruction counts, not measured on the H100.
 // Small-M layers (FPN P5-P7 towers, SSD extras) come out with narrow tiles spread over many
 // SMs, large ones with 128-wide tiles.
+//
+// The 128 x 256 tile (Cout_pad % 256 == 0) is then weighed against the chosen narrow tile in
+// clocks measured with scripts/tc_timeline.py (CTA 0, conv4_2 38x38 512->512 and conv7 19x19
+// 1024->1024 1x1 at B = 64; H100 SXM, 400 W power limit):
+//   narrow = rounds * max(mma, epi) + epi,   wide = rounds * (mma + epi)   (its epilogue is exposed),
+//   mma    = kblocks * clk per K block: 1015 for 128 x 128 x 64 (operand-feed bound: the dense
+//            rate would be 512; scaled by BN/128 below 128), 1085 for 128 x 256 x 64 (dense: 1024),
+//   epi    = 16500 clk for a 128 x 128 tile on 128 threads, 15000 for 128 x 256 on 256 threads.
+constexpr long long TC_KB_CLK_128 = 1015, TC_KB_CLK_256 = 1085, TC_EPI_CLK = 16500, TC_EPI_CLK_256 = 15000;
 static int pick_bn(int cout_pad, int m_tiles, int kblocks) {
   long long best = -1;
   int best_bn = 32;
@@ -587,7 +655,19 @@ static int pick_bn(int cout_pad, int m_tiles, int kblocks) {
       best_bn = bn;
     }
   }
-  return best_bn;
+  const int wide = wide_mode();
+  if (wide == 0 || cout_pad % TC_WIDE_BN != 0) return best_bn;
+  if (wide == 2) return TC_WIDE_BN;
+  auto rounds = [&](int bn) { return ((long long)m_tiles * (cout_pad / bn) + kNumSMs - 1) / kNumSMs; };
+  const long long mma_n = (long long)kblocks * TC_KB_CLK_128 * best_bn / 128, epi_n = TC_EPI_CLK * best_bn / 128;
+  const long long narrow = rounds(best_bn) * (mma_n > epi_n ? mma_n : epi_n) + epi_n;
+  const long long wide_cost = rounds(TC_WIDE_BN) * ((long long)kblocks * TC_KB_CLK_256 + TC_EPI_CLK_256);
+  return wide_cost < narrow ? TC_WIDE_BN : best_bn;
+}
+
+// The N tile conv_tc picks for an im2col-mode layer (see pick_bn); lets tests and scripts read the plan.
+extern "C" int odt_conv_tc_pick_bn(int cout_pad, long long M, int kblocks) {
+  return pick_bn(cout_pad, (int)((M + TC_BM - 1) / TC_BM), kblocks);
 }
 
 extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_conv_params* p,
@@ -695,7 +775,8 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
   stage_bytes = g.a_bytes + g.b_bytes;
   g.head_mode = (p->out0 && p->out0_dtype == ODT_F32 && !p->residual && !p->out1 && !p->out2) ? 1 : 0;
   // barriers + 1024-byte alignment slack, per consumer warpgroup: epilogue parameters + accumulator slice
-  const int fixed_bytes = 2048 + TC_EPI_SMEM;
+  // (the wide tile: one shared parameter block + two 64-row slices)
+  const int fixed_bytes = 2048 + (g.BN > TC_MAX_BN ? TC_WIDE_EPI_SMEM : TC_EPI_SMEM);
   // small filter banks of the flat modes stay resident in shared memory if at least three
   // activation stages still fit beside them
   const long long wres = 9ll * g.cchunks * g.BN * 128;
@@ -758,14 +839,16 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
   const int smem = stages * stage_bytes + (g.bres ? (int)wres : 0) + fixed_bytes;
   void (*kern)(CUtensorMap, CUtensorMap, TcGeom, Epi) =
       g.BN == 32 ? conv_tc_kernel<32> : g.BN == 64 ? conv_tc_kernel<64> : g.BN == 96 ? conv_tc_kernel<96>
-                                                                                    : conv_tc_kernel<128>;
-  ODT_CHECK_ARG(g.BN % 32 == 0 && g.BN <= TC_MAX_BN, "N tile");
+                                      : g.BN == 128 ? conv_tc_kernel<128> : conv_tc_kernel<TC_WIDE_BN>;
+  ODT_CHECK_ARG(g.BN % 32 == 0 && (g.BN <= TC_MAX_BN || (g.BN == TC_WIDE_BN && !g.flat)), "N tile");
   static bool smem_set = false;
   if (!smem_set) {
     ODT_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
     ODT_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
     ODT_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<96>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
     ODT_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
+    ODT_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<TC_WIDE_BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     TC_SMEM_LIMIT));
     smem_set = true;
   }
   const int num_tiles = g.num_m_tiles * g.num_n_tiles;
