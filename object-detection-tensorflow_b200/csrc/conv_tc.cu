@@ -25,10 +25,13 @@
 //   half, each ring stage consumed by both.  A quarter fewer operand bytes per multiply-add reach
 //   shared memory, which lifts the feed-bound mainloop to near the dense wgmma rate; the epilogue
 //   is then exposed once per tile, shared by all 256 consumer threads.
-// * Epilogue: the accumulators pass, one 32-column slice at a time, through a per-warpgroup fp32
-//   buffer in shared memory so that every epilogue lane owns one pixel row: folded bias/BN
-//   scale+shift, activation, residual, up to two extra pre-activated outputs, fused max-pool,
-//   fp32 head scatter; 128-bit global stores.
+// * Epilogue, fp16 out0 alone (tmO): folded bias/BN scale+shift and activation on the accumulator
+//   registers, rounded to fp16 there (the fused 2x2/2 max-pool: two lane shuffles), 32-column
+//   chunks written with stmatrix into a double-buffered, 64-byte-swizzled staging buffer per
+//   warpgroup and stored by TMA (one elected thread; the tensor map clips ragged rows / columns).
+//   Every other output (residual, up to two extra pre-activated outputs, channel regrouping, fp32
+//   head scatter, strides the maps do not cover): the accumulators pass, one 32-column slice at a
+//   time, through a per-warpgroup fp32 buffer so that every epilogue lane owns one pixel row.
 // * Persistent: one CTA per SM, static round-robin tile schedule.  Warp 0 = TMA producer (runs
 //   ahead across tiles; warps 1..3 only pad the producer warpgroup, which hands most of its
 //   registers to the consumers with setmaxnreg), warps 4..11 = the two consumer warpgroups.
@@ -56,6 +59,8 @@ constexpr int TC_EPI_PAR = 7 * TC_MAX_BN;  // floats per parameter block: epi_pa
 constexpr int TC_SLICE_PITCH = 36;
 constexpr int TC_SLICE_FLOATS = TC_BM * TC_SLICE_PITCH;
 constexpr int TC_EPI_SMEM = 2 * (TC_EPI_PAR + TC_SLICE_FLOATS) * 4;  // per consumer warpgroup: parameters + slice
+// the fp16 output path stages two 32-column chunks (64-byte rows, 64-byte swizzle) per warpgroup in its slice buffer
+constexpr int TC_OUT_COLS = 32;
 // Wide tile (BN = 256, im2col mode): both consumer warpgroups work on one 128 x 256 tile, warpgroup g on rows
 // 64g .. 64g+63 (one m64n256 accumulator set each).  Epilogue: one parameter block of 256 columns shared by the two
 // warpgroups, then per warpgroup a [64 rows x 32 columns] slice in which two lanes share a pixel row (16 columns each).
@@ -79,6 +84,7 @@ struct TcGeom {
   int cchunks;     // in_ld / 64
   int num_m_tiles, num_n_tiles, BN;
   int stages;
+  int tma_out;     // 1: fp16 out0 alone, through the fragment epilogue and the output tensor map
   int fast_store;  // 1: fp16 out0, no regroup, 16-byte aligned rows
   int fast_cols;   // columns that may be written by whole 32-column chunks (min channel stride)
   int a_bytes, b_bytes;  // shared memory per pipeline stage
@@ -95,7 +101,7 @@ struct TcGeom {
   // columns (RP*XB = 128); the slab of one filter row is a [XB+2 columns][RP rows][64 ch]
   // box, column-major over the tile so that tap s is the slab shifted by s*RP rows and the
   // four pixels of a pooling window sit in four lanes of one warp
-  int RP, lgRP, XB, xblocks, yblocks;
+  int RP, XB, xblocks, yblocks;
   int a_tx;        // bytes one activation slab load delivers
   // flat modes with a small filter bank: all 9*cchunks weight tiles [BN x 64] stay resident
   // in shared memory (loaded once per CTA); the pipeline stages then carry activations only
@@ -145,10 +151,11 @@ constexpr bool TC_FEED = true;
 #endif
 
 // --------------------------------------------------------------- kernel ----
-template <int BN>
+template <int BN, bool TMA_OUT>
 __global__ void __launch_bounds__(TC_THREADS, 1)
     conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                   const __grid_constant__ TcGeom g, const __grid_constant__ Epi e) {
+                   const __grid_constant__ CUtensorMap tmO, const __grid_constant__ TcGeom g,
+                   const __grid_constant__ Epi e) {
   constexpr bool WIDE = BN > TC_MAX_BN;  // the cooperative 128 x 256 tile (im2col mode only)
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // carve (base rounded up to 1024 for the 128B swizzle atoms)
@@ -164,15 +171,18 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (TC_MAX_STAGES + s); };
   const uint32_t wfull_bar = bar_base + 8u * (2 * TC_MAX_STAGES);  // resident weights landed
-  // per consumer warpgroup: the epilogue parameters of its current N tile
-  // [scale|shift|scale2|shift2|scale3|shift3|offset][TC_MAX_BN], then its accumulator slice
-  float* epi_smem = reinterpret_cast<float*>(smem_raw + (bar_base + 256u - raw));
+  // epilogue region, 1024 bytes past the barriers (the swizzled staging buffers need the alignment): the two
+  // consumer warpgroups' accumulator slices, then the parameter blocks [scale|shift|scale2|shift2|scale3|shift3|offset]
+  // (one per warpgroup of TC_MAX_BN columns; the wide tile: one of 256 columns)
+  const uint32_t epi_base = bar_base + 1024u;
+  float* epi_smem = reinterpret_cast<float*>(smem_raw + (epi_base - raw));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
+    if (TMA_OUT) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmO) : "memory");
     for (int s = 0; s < stages; ++s) {
       mbar_init(full_bar(s), 1);
       mbar_init(empty_bar(s), WIDE ? 8 : 4);  // one arrival per warp of the consuming warpgroup(s)
@@ -294,8 +304,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     const int group = (warp - 4) >> 2;
     const int et = threadIdx.x - 128 * (1 + group);  // index among the warpgroup's 128 threads
     const int epi_bar = TC_BAR_EPI + group;
-    float* par = WIDE ? epi_smem : epi_smem + group * (TC_EPI_PAR + TC_SLICE_FLOATS);
-    float* slice = WIDE ? epi_smem + 7 * P + group * TC_WIDE_SLICE_FLOATS : par + TC_EPI_PAR;
+    constexpr int SLICE_FLOATS = WIDE ? TC_WIDE_SLICE_FLOATS : TC_SLICE_FLOATS;
+    float* slice = epi_smem + group * SLICE_FLOATS;
+    float* par = epi_smem + 2 * SLICE_FLOATS + (WIDE ? 0 : group * TC_EPI_PAR);
+    // fp16 output staging: two chunk buffers of 128 (wide tile: 64, pooled tile: 32) rows x 64 bytes at the start
+    // of the slice buffer (1024-byte aligned); `sbuf` = the one the next chunk goes to (alternates across chunks and
+    // tiles)
+    int sbuf = 0;
     const int erow = WIDE ? 32 * (quarter & 1) + lane : 32 * quarter + lane;  // this lane's row of the slice
     const int ecol = WIDE ? 16 * (quarter >> 1) : 0;                          // and its first column
     int staged_n_tile = -1;
@@ -364,36 +379,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
       if (lane == 0) mbar_arrive(empty_bar(prev));
       if (quarter == 0) tl_stamp(1 + group, 1, tile);  // accumulators complete
 
-      const long long m = (long long)m_tile * TC_BM + (WIDE ? 64 * group : 0) + erow;
-      bool row_ok;
-      int img, pix;
-      long long pool_row = 0;  // element offset of this lane's pooled pixel (flat == 2)
-      int pool_q = 0;          // which 8-channel quarter of a 32-column chunk this lane stores
-      if (g.flat == 2) {
-        const int per_img = g.yblocks * g.xblocks;
-        img = m_tile / per_img;
-        const int rem = m_tile - img * per_img;
-        const int yq = rem / g.xblocks, xq = rem - yq * g.xblocks;
-        const int ml = quarter * 32 + lane;
-        const int x = g.XB * xq + (ml >> g.lgRP), y = g.RP * yq + (ml & (g.RP - 1));
-        row_ok = x < g.W && y < g.H;  // even sizes: a window is valid or invalid as a whole
-        pix = 0;
-        const int oh = g.out_halo;
-        pool_row = (long long)img * e.out0_img_stride +
-                   (long long)(((y >> 1) + oh) * ((g.W >> 1) + 2 * oh) + (x >> 1) + oh) * e.out0_pix_stride;
-        pool_q = (ml & 1) | (((ml >> g.lgRP) & 1) << 1);
-      } else if (g.flat) {
-        // padded-linear position -> (image, padded y, padded x); halo positions are not stored
-        img = m < g.Q ? (int)(m / g.PHW) : 0;
-        const int rem = (int)(m - (long long)img * g.PHW);
-        const int yp = rem / g.PW, xp = rem - yp * g.PW;
-        row_ok = m < g.Q && yp >= 1 && yp <= g.H && xp >= 1 && xp <= g.W;
-        pix = row_ok ? (yp - 1) * g.W + (xp - 1) : 0;
-      } else {
-        row_ok = m < g.M;
-        img = row_ok ? (int)(m / g.ohw) : 0;
-        pix = row_ok ? (int)(m - (long long)img * g.ohw) : 0;
-      }
       const int n0 = n_tile * BN;
       // the per-channel parameters of this N tile are staged once (broadcast reads later);
       // consecutive tiles of single-N-tile layers reuse them
@@ -408,119 +393,221 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         reinterpret_cast<int*>(par)[6 * P + t] = n0 + t < e.Cout ? regroup(e, n0 + t) : 0;
         named_bar_sync(TC_BAR_WIDE, 256);
       }
-      long long o0_row = (long long)img * e.out0_img_stride;
-      if (g.out_halo) {
-        const int oy = pix / g.OW, ox = pix - oy * g.OW;
-        o0_row += (long long)((oy + 1) * (g.OW + 2) + ox + 1) * e.out0_pix_stride;
-      } else {
-        o0_row += (long long)pix * e.out0_pix_stride;
-      }
-      const long long o1_row = aux_row(e.out1_img_stride, e.out1_pix_stride, e.out1_halo, g.OW, img, pix);
-      const long long o2_row = aux_row(e.out2_img_stride, e.out2_pix_stride, e.out2_halo, g.OW, img, pix);
-      const float* my_acc = slice + erow * TC_SLICE_PITCH + ecol;
-      for (int j = 0; j < BN / 32; ++j) {
-        if (n0 + j * 32 >= e.Cout) break;  // fully padded chunk (uniform)
-        const int nb = n0 + j * 32 + ecol;  // this lane's first column
-        // every lane of the warpgroup has finished reading the previous slice and, on a new tile, the parameters
-        named_bar_sync(epi_bar, 128);
-        if (!WIDE && j == 0 && new_par) {
+      if constexpr (TMA_OUT) {
+        // ---- fp16 out0 alone: epilogue on the accumulator fragments, TMA stores of staged 32-column chunks ----
+        // This thread's fragment rows: 64*h + 16*quarter + lane/4 + 8*k of the warpgroup's rows (acc[h], k = register
+        // pair), its columns 8*i + 2*(lane%4) + {0,1} of each 32-column chunk.
+        constexpr int HALVES = WIDE ? 1 : 2;
+        const int m0 = m_tile * TC_BM + (WIDE ? 64 * group : 0);  // TMA coordinates are 32-bit
+        const int lr = lane >> 2;
+        if (!WIDE && new_par) {
+          // this warpgroup's reads of the previous block ended before the barrier of its last chunk
           const int n = et < BN ? n0 + et : e.Cout;  // columns past the tile: identity
-#pragma unroll
-          for (int row = 0; row < 6; ++row) par[row * P + et] = epi_param(e, row, n);
-          reinterpret_cast<int*>(par)[6 * P + et] = n < e.Cout ? regroup(e, n) : 0;
+          par[et] = epi_param(e, 0, n);
+          par[P + et] = epi_param(e, 1, n);
+          named_bar_sync(epi_bar, 128);
         }
-        if constexpr (WIDE) {
-          wg_acc_slice_to_smem<BN>(acc[0], j, slice, TC_SLICE_PITCH, 0);
-        } else {
-          wg_acc_slice_to_smem<BN>(acc[0], j, slice, TC_SLICE_PITCH, 0);
-          wg_acc_slice_to_smem<BN>(acc[1], j, slice, TC_SLICE_PITCH, 64);
-        }
-        named_bar_sync(epi_bar, 128);
-        float v[32];
+        // halo-flat: the rows of border positions are stored as zeros (bit 2*h + k set: interior)
+        uint32_t keep = 0xFu;
+        if (g.flat == 1) {
+          keep = 0u;
 #pragma unroll
-        for (int i = 0; i < EW / 4; ++i) {
-          const float4 t = *reinterpret_cast<const float4*>(my_acc + 4 * i);
-          v[4 * i + 0] = t.x;
-          v[4 * i + 1] = t.y;
-          v[4 * i + 2] = t.z;
-          v[4 * i + 3] = t.w;
-        }
-        const float* ps = par + j * 32 + ecol;  // this lane's parameter columns
-        if (!WIDE && g.flat == 2) {
-          // fused 2x2/2 max pooling: bias/BN + activation, round to fp16, then the maximum over
-          // the window's four lanes (vertical neighbour = lane^1, horizontal = lane^RP); each
-          // of the four lanes stores one 8-channel quarter of the pooled pixel
-          uint4 packed[4];
-          epi_act_f16<4>(v, ps, P, e.act, packed);
-          uint32_t* pw = reinterpret_cast<uint32_t*>(packed);
+          for (int h = 0; h < HALVES; ++h)
 #pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            uint32_t o = __shfl_xor_sync(0xffffffffu, pw[i], 1);
-            __half2 a = __hmax2(*reinterpret_cast<__half2*>(&pw[i]), *reinterpret_cast<__half2*>(&o));
-            pw[i] = *reinterpret_cast<uint32_t*>(&a);
-            o = __shfl_xor_sync(0xffffffffu, pw[i], g.RP);
-            a = __hmax2(a, *reinterpret_cast<__half2*>(&o));
-            pw[i] = *reinterpret_cast<uint32_t*>(&a);
-          }
-          const uint4 sel = pool_q == 0 ? packed[0] : pool_q == 1 ? packed[1] : pool_q == 2 ? packed[2] : packed[3];
-          if (row_ok && nb + 8 * pool_q < g.fast_cols)
-            *reinterpret_cast<uint4*>(reinterpret_cast<__half*>(e.out0) + pool_row + nb + 8 * pool_q) = sel;
-        } else if (g.fast_store && nb + EW <= g.fast_cols) {
-          if (row_ok) {
-            const long long o0 = o0_row + nb;
-            const uint4* rp = reinterpret_cast<const uint4*>(reinterpret_cast<const __half*>(e.residual) + o0);
-            epi_store_f16<EW / 8>(e, v, ps, P, [&](int q) { return __ldg(rp + q); }, o0, o1_row + nb, o2_row + nb);
-          }
-        } else if (row_ok || g.head_mode) {
-          // generic path: fp32 head outputs scattered into the candidate rows,
-          // channel regrouping, ragged Cout; parameters come from shared memory
-          const int* pofs = reinterpret_cast<const int*>(par) + 6 * P + j * 32 + ecol;
-          const int nvalid = min(EW, e.Cout - nb);
-          if (g.head_mode) {
-            // head convolutions: fp32 scatter into the candidate rows.  The staged accumulator
-            // slice is read column-wise, so the warp writes one row per instruction with the
-            // lanes on consecutive channels (4-5 sectors per request instead of 32).
-            const int cl = lane < EW ? lane : 0;  // this lane's column (lanes past EW store nothing)
-            const float* acol = slice + (erow - lane) * TC_SLICE_PITCH + ecol + cl;
-            const float sc = ps[cl], sh = ps[P + cl];
-            const int my_ofs = pofs[cl];
-            const long long my_row = row_ok ? o0_row : -1;
-            float* obase = reinterpret_cast<float*>(e.out0);
-#pragma unroll 4
-            for (int rr = 0; rr < 32; ++rr) {
-              const long long orow_r = __shfl_sync(0xffffffffu, my_row, rr);
-              const float val = apply_act(fmaf(acol[rr * TC_SLICE_PITCH], sc, sh), e.act);
-              if (orow_r >= 0 && lane < nvalid) obase[orow_r + my_ofs] = val;
+            for (int k = 0; k < 2; ++k) {
+              // Q < 2^31 - 4096 in this mode: 32-bit arithmetic
+              const unsigned m = (unsigned)(m0 + 64 * h + 16 * quarter + lr + 8 * k);
+              const unsigned rem = m % (unsigned)g.PHW;
+              const int yp = (int)(rem / (unsigned)g.PW), xp = (int)(rem % (unsigned)g.PW);
+              if (yp >= 1 && yp <= g.H && xp >= 1 && xp <= g.W) keep |= 1u << (2 * h + k);
             }
-          } else {
+        }
+        // row-block pooled tile: tile row ml = RP*x + y, its window partners ml^1 and ml^RP sit in lanes ^4 and
+        // ^(4*RP); lanes with lr & (1|RP) == 0 keep the window's maximum.  Pooled pixel (x/2, y/2) is row
+        // (y/2)*(XB/2) + x/2 of the staged chunk (the {32, XB/2, RP/2, 1} box).
 #pragma unroll
-            for (int i = 0; i < EW; ++i) {
-              if (i >= nvalid) break;
-              const int n = nb + i;
-              float x = apply_act(fmaf(v[i], ps[i], ps[P + i]), e.act);
-              const long long o0 = o0_row + pofs[i];
-              if (e.residual) x += __half2float(reinterpret_cast<const __half*>(e.residual)[o0]);
-              if (e.out0) {
-                if (e.out0_dtype == ODT_F32) {
-                  reinterpret_cast<float*>(e.out0)[o0] = x;
-                } else {
-                  const __half hv = __float2half_rn(x);
-                  reinterpret_cast<__half*>(e.out0)[o0] = hv;
-                  x = __half2float(hv);
+        for (int j = 0; j < BN / TC_OUT_COLS; ++j) {
+          if (n0 + j * TC_OUT_COLS >= e.Cout) break;  // fully padded chunk (uniform)
+          const uint32_t buf = smem_u32(slice) + (uint32_t)(sbuf * (g.flat == 2 ? 32 : (WIDE ? 64 : 128)) * 64);
+#pragma unroll
+          for (int h = 0; h < HALVES; ++h) {
+            uint32_t hv[8];  // [2*i + k]: the half2 of column pair i on row k
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              const float* f = acc[h] + 4 * (4 * j + i);
+              const float* pc = par + 32 * j + 8 * i + 2 * (lane & 3);
+              const float2 sc = *reinterpret_cast<const float2*>(pc);
+              const float2 sh = *reinterpret_cast<const float2*>(pc + P);
+#pragma unroll
+              for (int k = 0; k < 2; ++k) {
+                __half2 v = epi_act_f16x2(f[2 * k], f[2 * k + 1], sc, sh, e.act);
+                hv[2 * i + k] = ((keep >> (2 * h + k)) & 1u) ? *reinterpret_cast<uint32_t*>(&v) : 0u;
+              }
+            }
+            if (!WIDE && g.flat == 2) {
+              // the window maximum of the rounded values (the fp16 maximum the stand-alone pool takes)
+#pragma unroll
+              for (int q = 0; q < 8; ++q) {
+                uint32_t o = __shfl_xor_sync(0xffffffffu, hv[q], 4);
+                __half2 a = __hmax2(*reinterpret_cast<__half2*>(&hv[q]), *reinterpret_cast<__half2*>(&o));
+                uint32_t au = *reinterpret_cast<uint32_t*>(&a);
+                o = __shfl_xor_sync(0xffffffffu, au, 4 * g.RP);
+                a = __hmax2(a, *reinterpret_cast<__half2*>(&o));
+                hv[q] = *reinterpret_cast<uint32_t*>(&a);
+              }
+              if ((lr & (1 | g.RP)) == 0) {
+#pragma unroll
+                for (int k = 0; k < 2; ++k) {
+                  const int ml = 64 * h + 16 * quarter + 8 * k + lr;
+                  const int prow = g.RP == 2 ? ml >> 2 : ((ml >> 1) & 1) * 16 + (ml >> 3);
+#pragma unroll
+                  for (int i = 0; i < 4; ++i)
+                    st_shared_u32(buf + (uint32_t)(prow * 64 + ((i ^ ((prow >> 1) & 3)) << 4) + 4 * (lane & 3)),
+                                  hv[2 * i + k]);
                 }
               }
-              if (e.out1)
-                reinterpret_cast<__half*>(e.out1)[o1_row + n] =
-                    __float2half_rn(apply_act(fmaf(x, ps[2 * P + i], ps[3 * P + i]), e.act2));
-              if (e.out2)
-                reinterpret_cast<__half*>(e.out2)[o2_row + n] =
-                    __float2half_rn(apply_act(fmaf(x, ps[4 * P + i], ps[5 * P + i]), e.act3));
+            } else {
+              // 64-byte swizzle: 16-byte piece c of row r at r*64 + ((c ^ (r/2 % 4)) * 16)
+              const int mi = lane >> 3;
+              const int row = 64 * h + 16 * quarter + (lane & 7) + 8 * (mi & 1);
+#pragma unroll
+              for (int s2 = 0; s2 < 2; ++s2) {
+                const int c = 2 * s2 + (mi >> 1);
+                stmatrix_x4(buf + (uint32_t)(row * 64 + ((c ^ ((row >> 1) & 3)) << 4)), hv[4 * s2], hv[4 * s2 + 1],
+                            hv[4 * s2 + 2], hv[4 * s2 + 3]);
+              }
+            }
+          }
+          fence_proxy_async_smem();
+          if (et == 0) bulk_wait_read<0>();  // the previous chunk's store has read the buffer the next chunk takes
+          named_bar_sync(epi_bar, 128);
+          if (et == 0) {
+            if (!WIDE && g.flat == 2) {
+              const int per_img = g.yblocks * g.xblocks;
+              const int im = m_tile / per_img, rem = m_tile - im * per_img;
+              const int yq = rem / g.xblocks, xq = rem - yq * g.xblocks;
+              tma_store_4d(&tmO, buf, j * TC_OUT_COLS, (g.XB >> 1) * xq, (g.RP >> 1) * yq, im);
+            } else {
+              tma_store_2d(&tmO, buf, n0 + j * TC_OUT_COLS, m0);
+            }
+            bulk_commit();
+          }
+          sbuf ^= 1;
+        }
+      } else {
+        // ---- staged path: every output through the per-warpgroup fp32 slice, one pixel row per lane ----
+        const long long m = (long long)m_tile * TC_BM + (WIDE ? 64 * group : 0) + erow;
+        bool row_ok;
+        int img, pix;
+        if (g.flat) {
+          // padded-linear position -> (image, padded y, padded x); halo positions are not stored
+          img = m < g.Q ? (int)(m / g.PHW) : 0;
+          const int rem = (int)(m - (long long)img * g.PHW);
+          const int yp = rem / g.PW, xp = rem - yp * g.PW;
+          row_ok = m < g.Q && yp >= 1 && yp <= g.H && xp >= 1 && xp <= g.W;
+          pix = row_ok ? (yp - 1) * g.W + (xp - 1) : 0;
+        } else {
+          row_ok = m < g.M;
+          img = row_ok ? (int)(m / g.ohw) : 0;
+          pix = row_ok ? (int)(m - (long long)img * g.ohw) : 0;
+        }
+        long long o0_row = (long long)img * e.out0_img_stride;
+        if (g.out_halo) {
+          const int oy = pix / g.OW, ox = pix - oy * g.OW;
+          o0_row += (long long)((oy + 1) * (g.OW + 2) + ox + 1) * e.out0_pix_stride;
+        } else {
+          o0_row += (long long)pix * e.out0_pix_stride;
+        }
+        const long long o1_row = aux_row(e.out1_img_stride, e.out1_pix_stride, e.out1_halo, g.OW, img, pix);
+        const long long o2_row = aux_row(e.out2_img_stride, e.out2_pix_stride, e.out2_halo, g.OW, img, pix);
+        const float* my_acc = slice + erow * TC_SLICE_PITCH + ecol;
+        for (int j = 0; j < BN / 32; ++j) {
+          if (n0 + j * 32 >= e.Cout) break;  // fully padded chunk (uniform)
+          const int nb = n0 + j * 32 + ecol;  // this lane's first column
+          // every lane of the warpgroup has finished reading the previous slice and, on a new tile, the parameters
+          named_bar_sync(epi_bar, 128);
+          if (!WIDE && j == 0 && new_par) {
+            const int n = et < BN ? n0 + et : e.Cout;  // columns past the tile: identity
+#pragma unroll
+            for (int row = 0; row < 6; ++row) par[row * P + et] = epi_param(e, row, n);
+            reinterpret_cast<int*>(par)[6 * P + et] = n < e.Cout ? regroup(e, n) : 0;
+          }
+          if constexpr (WIDE) {
+            wg_acc_slice_to_smem<BN>(acc[0], j, slice, TC_SLICE_PITCH, 0);
+          } else {
+            wg_acc_slice_to_smem<BN>(acc[0], j, slice, TC_SLICE_PITCH, 0);
+            wg_acc_slice_to_smem<BN>(acc[1], j, slice, TC_SLICE_PITCH, 64);
+          }
+          named_bar_sync(epi_bar, 128);
+          float v[32];
+#pragma unroll
+          for (int i = 0; i < EW / 4; ++i) {
+            const float4 t = *reinterpret_cast<const float4*>(my_acc + 4 * i);
+            v[4 * i + 0] = t.x;
+            v[4 * i + 1] = t.y;
+            v[4 * i + 2] = t.z;
+            v[4 * i + 3] = t.w;
+          }
+          const float* ps = par + j * 32 + ecol;  // this lane's parameter columns
+          if (g.fast_store && nb + EW <= g.fast_cols) {
+            if (row_ok) {
+              const long long o0 = o0_row + nb;
+              const uint4* rp = reinterpret_cast<const uint4*>(reinterpret_cast<const __half*>(e.residual) + o0);
+              epi_store_f16<EW / 8>(e, v, ps, P, [&](int q) { return __ldg(rp + q); }, o0, o1_row + nb, o2_row + nb);
+            }
+          } else if (row_ok || g.head_mode) {
+            // generic path: fp32 head outputs scattered into the candidate rows,
+            // channel regrouping, ragged Cout; parameters come from shared memory
+            const int* pofs = reinterpret_cast<const int*>(par) + 6 * P + j * 32 + ecol;
+            const int nvalid = min(EW, e.Cout - nb);
+            if (g.head_mode) {
+              // head convolutions: fp32 scatter into the candidate rows.  The staged accumulator
+              // slice is read column-wise, so the warp writes one row per instruction with the
+              // lanes on consecutive channels (4-5 sectors per request instead of 32).
+              const int cl = lane < EW ? lane : 0;  // this lane's column (lanes past EW store nothing)
+              const float* acol = slice + (erow - lane) * TC_SLICE_PITCH + ecol + cl;
+              const float sc = ps[cl], sh = ps[P + cl];
+              const int my_ofs = pofs[cl];
+              const long long my_row = row_ok ? o0_row : -1;
+              float* obase = reinterpret_cast<float*>(e.out0);
+#pragma unroll 4
+              for (int rr = 0; rr < 32; ++rr) {
+                const long long orow_r = __shfl_sync(0xffffffffu, my_row, rr);
+                const float val = apply_act(fmaf(acol[rr * TC_SLICE_PITCH], sc, sh), e.act);
+                if (orow_r >= 0 && lane < nvalid) obase[orow_r + my_ofs] = val;
+              }
+            } else {
+#pragma unroll
+              for (int i = 0; i < EW; ++i) {
+                if (i >= nvalid) break;
+                const int n = nb + i;
+                float x = apply_act(fmaf(v[i], ps[i], ps[P + i]), e.act);
+                const long long o0 = o0_row + pofs[i];
+                if (e.residual) x += __half2float(reinterpret_cast<const __half*>(e.residual)[o0]);
+                if (e.out0) {
+                  if (e.out0_dtype == ODT_F32) {
+                    reinterpret_cast<float*>(e.out0)[o0] = x;
+                  } else {
+                    const __half hv = __float2half_rn(x);
+                    reinterpret_cast<__half*>(e.out0)[o0] = hv;
+                    x = __half2float(hv);
+                  }
+                }
+                if (e.out1)
+                  reinterpret_cast<__half*>(e.out1)[o1_row + n] =
+                      __float2half_rn(apply_act(fmaf(x, ps[2 * P + i], ps[3 * P + i]), e.act2));
+                if (e.out2)
+                  reinterpret_cast<__half*>(e.out2)[o2_row + n] =
+                      __float2half_rn(apply_act(fmaf(x, ps[4 * P + i], ps[5 * P + i]), e.act3));
+              }
             }
           }
         }
       }
       if (quarter == 0) tl_stamp(1 + group, 2, tile);  // epilogue done
     }
+    // the shared-memory sources of the last output stores stay valid until the stores are done
+    if (TMA_OUT && et == 0) bulk_wait<0>();
   }
 }
 
@@ -559,12 +646,12 @@ static int resolve_driver() {
 }
 
 int tc_encode_tiled(CUtensorMap* map, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides,
-                    const cuuint32_t* box, bool l2_promote_256) {
+                    const cuuint32_t* box, bool l2_promote_256, CUtensorMapSwizzle swizzle) {
   int rc = resolve_driver();
   if (rc) return rc;
   cuuint32_t estr[5] = {1, 1, 1, 1, 1};
   CUresult cr = g_encode_tiled(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(base), dims,
-                               strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                               strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
                                l2_promote_256 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B : CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (cr != CUDA_SUCCESS) {
@@ -629,7 +716,8 @@ using namespace odt;
 //             warpgroup's mainloop, so a round costs the longer of the two and only the CTA's
 //             last epilogue is exposed,
 //   rounds  = tiles per CTA of the slowest SM.
-// The constants are estimates from the instruction counts, not measured on the H100.
+// The constants are estimates from the instruction counts, not measured on the H100 (nor refitted to the
+// fp16 output path of the fragment epilogue).
 // Small-M layers (FPN P5-P7 towers, SSD extras) come out with narrow tiles spread over many
 // SMs, large ones with 128-wide tiles.
 //
@@ -747,7 +835,6 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
   if (g.flat == 2) {
     long long tiles_per_img;
     g.RP = tc_rowblock_rp(p->OH, p->OW, &tiles_per_img);
-    g.lgRP = g.RP == 4 ? 2 : 1;
     g.XB = TC_BM / g.RP;
     g.yblocks = (p->OH + g.RP - 1) / g.RP;
     g.xblocks = (p->OW + g.XB - 1) / g.XB;
@@ -776,6 +863,7 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
   g.head_mode = (p->out0 && p->out0_dtype == ODT_F32 && !p->residual && !p->out1 && !p->out2) ? 1 : 0;
   // barriers + 1024-byte alignment slack, per consumer warpgroup: epilogue parameters + accumulator slice
   // (the wide tile: one shared parameter block + two 64-row slices)
+  // (the staging buffers of the fp16 output path reuse the slices)
   const int fixed_bytes = 2048 + (g.BN > TC_MAX_BN ? TC_WIDE_EPI_SMEM : TC_EPI_SMEM);
   // small filter banks of the flat modes stay resident in shared memory if at least three
   // activation stages still fit beside them
@@ -798,6 +886,16 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
                  (!p->out2 || (((uintptr_t)p->out2 & 15) == 0 && p->out2_pix_stride % 8 == 0 &&
                                p->out2_img_stride % 8 == 0));
   g.fast_cols = p->out0 ? p->out0_pix_stride : (1 << 30);
+  // fp16 out0 alone, in a layout one output tensor map covers: the fragment epilogue with TMA stores.  Rows of the
+  // im2col / halo-flat tile are consecutive output rows of the map, so the halo-flat output must keep its halo and
+  // the im2col output must not have one; images must be stored back to back.
+  const long long pix = p->out0_pix_stride;
+  g.tma_out = p->out0 && p->out0_dtype == ODT_F16 && !p->residual && !p->out1 && !p->out2 && p->out0_group == 0 &&
+              f16_rows_aligned(p->out0, p->out0_img_stride, p->out0_pix_stride, p->Cout_pad) &&
+              (g.flat == 2 ||
+               (g.flat == 1 && p->out0_halo == 1 && p->out0_img_stride == (long long)g.PHW * pix) ||
+               (g.flat == 0 && p->out0_halo == 0 && p->out0_img_stride == (long long)g.ohw * pix));
+  ODT_CHECK_ARG(g.flat != 2 || g.tma_out, "fused pooling: out0 layout");
   if (p->out1 && p->out1_pix_stride < g.fast_cols) g.fast_cols = p->out1_pix_stride;
   if (p->out2 && p->out2_pix_stride < g.fast_cols) g.fast_cols = p->out2_pix_stride;
 
@@ -835,24 +933,51 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
     rc = tc_encode_tiled(&tmB, weights, 2, dims, strides, box, true);
     if (rc) return rc;
   }
+  // out0 of the fp16 output path: 32-column boxes (64-byte swizzle, like the staging buffers), columns up to Cout_pad
+  CUtensorMap tmO;
+  memset(&tmO, 0, sizeof(tmO));
+  if (g.tma_out) {
+    const cuuint64_t cp = (cuuint64_t)p->Cout_pad, ps = (cuuint64_t)pix * 2;
+    if (g.flat == 2) {
+      // [B][H/2][W/2] interior of the pooled tensor (a halo shifts the origin by one row and one column), box = the
+      // tile's 32 pooled pixels; ragged column / row blocks are clipped at W/2 / H/2
+      const int oh = p->out0_halo;
+      const cuuint64_t PW2 = (cuuint64_t)(p->W / 2 + 2 * oh);
+      const __half* o = reinterpret_cast<const __half*>(p->out0) + (long long)(oh * PW2 + oh) * pix;
+      cuuint64_t dims[4] = {cp, (cuuint64_t)(p->W / 2), (cuuint64_t)(p->H / 2), (cuuint64_t)p->B};
+      cuuint64_t strides[3] = {ps, PW2 * ps, (cuuint64_t)p->out0_img_stride * 2};
+      cuuint32_t box[4] = {TC_OUT_COLS, (cuuint32_t)(g.XB / 2), (cuuint32_t)(g.RP / 2), 1};
+      rc = tc_encode_tiled(&tmO, o, 4, dims, strides, box, false, CU_TENSOR_MAP_SWIZZLE_64B);
+    } else {
+      // [rows][Cout_pad]: the output positions (im2col) or padded-linear positions (halo-flat); rows past the end
+      // are clipped.  The wide tile stores each warpgroup's 64-row half.
+      cuuint64_t dims[2] = {cp, (cuuint64_t)(g.flat ? g.Q : g.M)};
+      cuuint64_t strides[1] = {ps};
+      cuuint32_t box[2] = {TC_OUT_COLS, (cuuint32_t)(g.BN > TC_MAX_BN ? TC_BM / 2 : TC_BM)};
+      rc = tc_encode_tiled(&tmO, p->out0, 2, dims, strides, box, false, CU_TENSOR_MAP_SWIZZLE_64B);
+    }
+    if (rc) return rc;
+  }
 
   const int smem = stages * stage_bytes + (g.bres ? (int)wres : 0) + fixed_bytes;
-  void (*kern)(CUtensorMap, CUtensorMap, TcGeom, Epi) =
-      g.BN == 32 ? conv_tc_kernel<32> : g.BN == 64 ? conv_tc_kernel<64> : g.BN == 96 ? conv_tc_kernel<96>
-                                      : g.BN == 128 ? conv_tc_kernel<128> : conv_tc_kernel<TC_WIDE_BN>;
   ODT_CHECK_ARG(g.BN % 32 == 0 && (g.BN <= TC_MAX_BN || (g.BN == TC_WIDE_BN && !g.flat)), "N tile");
+  // the two epilogues are separate instantiations: each gets the register allocation of its own path
+  typedef void (*Kern)(CUtensorMap, CUtensorMap, CUtensorMap, TcGeom, Epi);
+  static const Kern kerns[2][5] = {
+      {conv_tc_kernel<32, false>, conv_tc_kernel<64, false>, conv_tc_kernel<96, false>, conv_tc_kernel<128, false>,
+       conv_tc_kernel<TC_WIDE_BN, false>},
+      {conv_tc_kernel<32, true>, conv_tc_kernel<64, true>, conv_tc_kernel<96, true>, conv_tc_kernel<128, true>,
+       conv_tc_kernel<TC_WIDE_BN, true>}};
   static bool smem_set = false;
   if (!smem_set) {
-    ODT_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
-    ODT_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
-    ODT_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<96>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
-    ODT_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
-    ODT_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<TC_WIDE_BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     TC_SMEM_LIMIT));
+    for (int t = 0; t < 2; ++t)
+      for (int b = 0; b < 5; ++b)
+        ODT_CUDA_OK(cudaFuncSetAttribute(kerns[t][b], cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
     smem_set = true;
   }
+  const Kern kern = kerns[g.tma_out][g.BN > TC_MAX_BN ? 4 : g.BN / 32 - 1];
   const int num_tiles = g.num_m_tiles * g.num_n_tiles;
-  ODT_CUDA_OK(launch_pdl(kern, num_tiles < kNumSMs ? num_tiles : kNumSMs, TC_THREADS, smem, st, tmA, tmB, g,
+  ODT_CUDA_OK(launch_pdl(kern, num_tiles < kNumSMs ? num_tiles : kNumSMs, TC_THREADS, smem, st, tmA, tmB, tmO, g,
                          make_epi(*p)));
   ODT_LAUNCH_OK();
   return ODT_OK;

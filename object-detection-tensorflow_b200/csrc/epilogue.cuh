@@ -149,6 +149,12 @@ __host__ __device__ __forceinline__ void epi_act_f16(float* v, const float* par,
   epi_round_f16<NV>(v, out);
 }
 
+// the fragment form of epi_act_f16: one pair of adjacent columns of an accumulator row (a wgmma fragment register
+// pair), act(v * sc + sh) rounded to one half2 -- the same operations, element by element, as epi_act_f16
+__host__ __device__ __forceinline__ __half2 epi_act_f16x2(float a, float b, float2 sc, float2 sh, int act) {
+  return __floats2half2_rn(apply_act(fmaf(a, sc.x, sh.x), act), apply_act(fmaf(b, sc.y, sh.y), act));
+}
+
 // a consumer's pre-activation act(x * par[0] + par[1]) of the rounded fp16 values x
 template <int NV>
 __host__ __device__ __forceinline__ void epi_pre_f16(const uint4* x, const float* par, int ps, int act, uint4* out) {

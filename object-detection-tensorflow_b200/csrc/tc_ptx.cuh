@@ -70,6 +70,41 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
       : "r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+// ---- TMA stores (shared -> global), tracked per issuing thread in bulk async-groups ----
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               :
+               : "l"(map), "r"(src), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+               :
+               : "l"(map), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's committed store groups still read their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// at most N of this thread's committed store groups are still incomplete
+template <int N>
+__device__ __forceinline__ void bulk_wait() {
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
+// four 8 x 8 fp16 matrices to shared memory: lane l gives the address of row l%8 of matrix l/8, register k holds
+// this lane's pair (row l/4, columns 2*(l%4) + {0,1}) of matrix k -- the wgmma accumulator fragment's layout
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3)
+               : "memory");
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+
 // ---- warpgroup MMA (wgmma): D[64 x N] (+)= A[64 x 16] * B[16 x N], fp32 accumulators in registers ----
 // Both operands come from shared memory through matrix descriptors, K-major with the 128-byte swizzle.
 // Fragment of thread t of the warpgroup (warp w = t/32, lane l): register 4*i + {0,1} holds row 16w + l/4,
@@ -290,10 +325,12 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
-// host (conv_tc.cu): the tensor maps of the tensor-core kernels, fp16 with the 128-byte swizzle and zero fill;
-// 0 or an ODT_ERR_* code with the message set.  L2 promotion: 256 B for weights, 128 B for activations.
+// host (conv_tc.cu): the tensor maps of the tensor-core kernels, fp16 with the 128-byte swizzle (the output maps of
+// 32-column boxes: 64-byte) and zero fill; 0 or an ODT_ERR_* code with the message set.  L2 promotion: 256 B for
+// weights, 128 B for activations.
 int tc_encode_tiled(CUtensorMap* map, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides,
-                    const cuuint32_t* box, bool l2_promote_256);
+                    const cuuint32_t* box, bool l2_promote_256,
+                    CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B);
 // rank-4 NHWC activations, `channels` x `pixels` boxes, traversal stride `stride` along W and H
 int tc_encode_im2col(CUtensorMap* map, const void* base, const cuuint64_t* dims, const cuuint64_t* strides,
                      const int* lower, const int* upper, cuuint32_t channels, cuuint32_t pixels, int stride);
