@@ -300,6 +300,19 @@ int odt_yolo_loss_fwd(const float* head, const odt_tail_params* p, int B, const 
                       float coord_scale, float noobj_scale, float obj_scale, float class_scale,
                       void* scratch, float* loss_out, void* stream);
 
+/* ------------------------------------------------- classification tail --- */
+/* Global mean pool + arg-max (+ sparse softmax cross-entropy) of RetinaNet's ImageNet-pretraining mode.
+ *   feat: activation `dtype` [B][H+2*halo][W+2*halo][ld], real channels [0, C) (C <= 4096, ld >= C); the halo
+ *         border and channels >= C are never summed.
+ *   logits: f32 [B,C] = (float)(sum over H x W, in fp64) / (H*W), rounded division;
+ *   pred: i64 [B] = the first maximum of each row (tf.argmax);
+ *   labels: i64 [B] and loss: f32 [B], both or neither: loss = log(sum_c exp(x_c - max)) - (x_label - max),
+ *         NaN for a label outside [0, C) (the host rejects those before the call).
+ * One CTA per image, fixed-order reductions: repeated calls give bit-identical results.
+ * ref: RetinaNet.py:123-127 (reduce_mean over [1, 2], sparse_softmax_cross_entropy, argmax) */
+int odt_pool_classify(const void* feat, int dtype, int B, int H, int W, int C, int ld, int halo, float* logits,
+                      long long* pred, const long long* labels, float* loss, void* stream);
+
 /* ------------------------------------------------------- multi-GPU ------- */
 /* One process per GPU; images shard batch-parallel, weights are replicated, and the only data-path collective is
  * ONE all-gather of the packed detection records (the `dets` buffer of odt_nms_per_class with the record stride).

@@ -8,9 +8,9 @@ drivers run unchanged (SURVEY.md section 8b):
 Inference (`test_one_image`) runs entirely on the hand-written GPU kernels; there is no CPU
 fallback.  `train_one_epoch` runs the training step of odt_b200/train.py (PyTorch autograd over the
 engine's layer list + the reference's losses + Momentum: the first stage of SURVEY 8f row 2; RetinaNet's
-ImageNet-pretraining mode is not built).  Extensions: `test_one_image` accepts [B,H,W,3] (returns a list per
-image for B > 1), `detect_batch` / `detect_stream` / `detect_*_sharded` expose the batched, pipelined and
-multi-GPU paths.
+ImageNet-pretraining mode: the same step with the pooled-logit cross-entropy).  Extensions: `test_one_image`
+accepts [B,H,W,3] (returns a list per image for B > 1), `detect_batch` / `detect_stream` / `detect_*_sharded`
+expose the batched, pipelined and multi-GPU paths.
 """
 import os
 import sys
@@ -19,7 +19,7 @@ import numpy as np
 import torch
 
 from . import nets, tf_checkpoint
-from .engine import init_weights
+from .engine import Net, check_class_labels, init_weights
 
 # VGG-16 classification checkpoint scope -> (kernel variable, bias variable) as the reference
 # names them, typos included (SSD300.py:195-301: 'kenrel_conv2_1', 'bias_conv_3_1')
@@ -470,21 +470,140 @@ class RetinaNet(_Detector):
     def __init__(self, config, data_provider):
         assert len(config["data_shape"]) == 3
         self._common_init(config, data_provider)
-        if config["is_pretraining"]:
-            raise NotImplementedError("RetinaNet ImageNet-pretraining mode is classification, "
-                                      "outside the detection hot path (SURVEY.md section 2 #3)")
+        self.is_pretraining = bool(config["is_pretraining"])
         self.is_bottleneck = config["is_bottleneck"]
         self.block_list = config["residual_block_list"]
         self.data_shape = config["data_shape"]
-        nets.check_num_classes(config)
+        # ImageNet-pretraining mode (RetinaNet.py:61-69,120-135) classifies into 4 * filters[-1] classes; the
+        # configured num_classes is unused there
+        if not self.is_pretraining:
+            nets.check_num_classes(config)
         self.num_classes = config["num_classes"] + 1
         self.gamma, self.alpha = config["gamma"], config["alpha"]
 
     def _build(self, batch, precision, allow_tc=True):
+        if self.is_pretraining:
+            return nets.build_retinanet_backbone(batch, self.config, precision, self.device, allow_tc)
         return nets.build_retinanet(batch, self.config, precision, self.device, allow_tc)
 
     def _loss_scalars(self):
         return {"alpha": self.alpha, "gamma": self.gamma}
+
+    # ---- ImageNet-pretraining mode (ref RetinaNet.py:476-519) -------------------------------------------------------
+    @property
+    def num_logits(self):
+        """Width of the pretraining-mode logits: 4 * filters[-1] with filters = 7 * 2^i (RetinaNet.py:27)."""
+        return 4 * 7 * 2 ** (len(self.block_list) - 1)
+
+    def test_one_image(self, images):
+        """Detection: [scores, bbox, class_id] (ref RetinaNet.py:505-507).  Pretraining mode: int64 [B] = the first
+        maximum of the pooled logits (ref :501-503); [B,H,W,3] batches run as one engine batch."""
+        if not self.is_pretraining:
+            return _Detector.test_one_image(self, images)
+        if self.data_format == "channels_first":
+            images = np.transpose(np.asarray(images), (0, 2, 3, 1))
+        net = self._classify(images)
+        return net.tail.results()
+
+    def _classify(self, images, precision=None):
+        images = _as_host_tensor(images)
+        assert images.dim() == 4 and images.shape[3] == 3, "expected [B,H,W,3]"
+        net = self.engine(images.shape[0], precision)
+        assert tuple(images.shape[1:3]) == (net.in_h, net.in_w), (images.shape, net.in_h, net.in_w)
+        net.image_buf.copy_(images, non_blocking=True)
+        net.run()
+        return net
+
+    def loss_forward(self, images, ground_truth, precision=None, return_info=False):
+        """Detection: the focal + smooth-L1 loss per image (see _Detector.loss_forward).  Pretraining mode:
+        `ground_truth` is the label vector [B] and the result is the per-image sparse softmax cross-entropy of the
+        pooled logits, float32 [B], on the GPU kernel (labels outside [0, C) raise ValueError before any launch)."""
+        if not self.is_pretraining:
+            return _Detector.loss_forward(self, images, ground_truth, precision, return_info)
+        labels = check_class_labels(ground_truth, _as_host_tensor(images).shape[0], self.num_logits)
+        net = self._classify(images, precision)
+        return net.tail.loss(net, labels)
+
+    def train_one_epoch(self, lr):
+        """Detection: the mean loss (see _Detector.train_one_epoch).  Pretraining mode (ref RetinaNet.py:476-486):
+        (mean loss, mean accuracy) over `num_train // batch_size` steps on (images, labels) batches."""
+        if not self.is_pretraining:
+            return _Detector.train_one_epoch(self, lr)
+        assert self.mode == "train", "construct the model with mode='train'"
+        tr = self.trainer()
+        self.train_initializer()
+        num_iters = self.num_train // self.batch_size
+        losses, accs = [], []
+        for i in range(num_iters):
+            images, labels = self.train_iterator.get_next()
+            if self.data_format == "channels_first":
+                images = np.transpose(np.asarray(images), (0, 2, 3, 1))
+            loss, acc = tr.step(images, labels, lr)
+            losses.append(loss)
+            accs.append(acc)
+        self._weights = tr.export()
+        self._engines = {}
+        self.global_step = tr.global_step
+        if not losses:
+            return float("nan"), float("nan")
+        return float(np.mean(losses)), float(np.mean(accs))
+
+    def save_weight(self, mode, path):
+        """Detection: every variable + global_step.  Pretraining mode (ref RetinaNet.py:509-519,548-551):
+        `Saver(trainable feature_extractor variables).save(path, global_step)` -> `<path>-<step>` holding those
+        variables only (no BN moving statistics, no global_step)."""
+        if not self.is_pretraining:
+            return _Detector.save_weight(self, mode, path)
+        assert mode in ["latest", "best"]
+        d = os.path.dirname(path)
+        if d and not os.path.exists(d):
+            os.makedirs(d)
+            print(d, "does not exist, create it done")
+        out = "%s-%d" % (path, self.global_step)
+        w = self.get_weights()
+        tf_checkpoint.write_checkpoint(out, {k: w[k] for k in self.pretraining_variables()})
+        print("save", mode, "model in", out, "successfully")
+        return out
+
+    def load_weight(self, path):
+        """Pretraining mode: `saver.restore` with the pretraining saver -- every trainable variable must be in the
+        checkpoint; the BN moving statistics keep their values."""
+        if not self.is_pretraining:
+            return _Detector.load_weight(self, path)
+        w = dict(self.get_weights())
+        if path.endswith(".npz"):
+            self._load_npz_into(w, path)
+        else:
+            self._load_bundle_into(w, path, require=self.pretraining_variables())
+        self.set_weights(w)
+        print("load weight", path, "successfully")
+
+    def load_pretraining_weight(self, path):
+        """`pretraining_weight_saver.restore` (RetinaNet.py:537-539,553-555): the trainable 'feature_extractor'
+        variables.  The ResNet's must all be in the checkpoint -- they are what pretraining-mode `save_weight` writes;
+        the pyramid convolutions, which the reference's saver also lists but no pretraining checkpoint holds, are
+        restored when present."""
+        if self.is_pretraining:  # the reference builds no pretraining_weight_saver in this mode (:61-69)
+            raise AttributeError("RetinaNet in the ImageNet-pretraining mode has no load_pretraining_weight; "
+                                 "use load_weight")
+        if path.endswith(".npz"):
+            return _Detector.load_pretraining_weight(self, path)
+        Net.spec_only = True
+        try:
+            backbone, _ = nets.build_retinanet_backbone(1, self.config, "fp32", self.device, False)
+        finally:
+            Net.spec_only = False
+        resnet = [k for k, (_, kind) in backbone.vars.items() if kind not in ("bn_mean", "bn_var")]
+        w = dict(self.get_weights())
+        self._load_bundle_into(w, path, require=resnet)
+        r = tf_checkpoint.open_checkpoint(path)
+        for k in set(self.pretraining_variables()) - set(resnet):
+            if r.has_tensor(k):
+                t = r.get_tensor(k)
+                assert tuple(t.shape) == tuple(w[k].shape), (k, t.shape, w[k].shape)
+                w[k] = t.astype(np.float32)
+        self.set_weights(w)
+        print("load pretraining weight", path, "successfully")
 
 
 class YOLOv3(_Detector):

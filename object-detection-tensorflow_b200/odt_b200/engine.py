@@ -992,6 +992,58 @@ class Tail:
         return unpack_records(self.rec.cpu().numpy(), self.p.cap)
 
 
+def check_class_labels(labels, batch, num_classes):
+    """Sparse class labels [B] (or the reference's [B, 1] placeholder shape) -> int64 ndarray [B].  A label outside
+    [0, num_classes) is a ValueError, as TF's sparse_softmax_cross_entropy CPU kernel rejects it."""
+    lab = np.asarray(labels)
+    if lab.ndim == 2 and lab.shape[1] == 1:
+        lab = lab[:, 0]
+    if lab.shape != (batch,):
+        raise ValueError("labels: expected shape [%d], got %s" % (batch, np.asarray(labels).shape))
+    if lab.dtype.kind not in "iu" and not (lab.dtype.kind == "f" and np.all(lab == np.floor(lab))):
+        raise ValueError("labels must be integer class ids")
+    lab = lab.astype(np.int64)
+    bad = (lab < 0) | (lab >= num_classes)
+    if bad.any():
+        raise ValueError("label %d of image %d is outside [0, %d)" % (lab[bad][0], int(np.nonzero(bad)[0][0]),
+                                                                     num_classes))
+    return lab
+
+
+class ClassifyTail:
+    """Classification tail of RetinaNet's pretraining mode (ref RetinaNet.py:123-127) on the last feature tensor
+    `feat`: fp32 logits [B, C] = mean over H x W, `pred` int64 [B] = their first maximum, and on request the
+    per-image sparse softmax cross-entropy -- one odt_pool_classify launch.  Same interface as Tail."""
+
+    def __init__(self, feat):
+        self.feat = feat
+
+    def prepare(self, net):
+        self.logits = torch.zeros((net.batch, self.feat.C), dtype=torch.float32, device=net.device)
+        self.pred = torch.zeros((net.batch,), dtype=torch.int64, device=net.device)
+
+    def launch(self, net, stream, labels=None, loss=None):
+        f = self.feat
+        L.check(net.lib.odt_pool_classify(f.ptr(), net.dt, f.B, f.H, f.W, f.C, f.ld, f.halo, self.logits.data_ptr(),
+                                          self.pred.data_ptr(), labels.data_ptr() if labels is not None else None,
+                                          loss.data_ptr() if loss is not None else None, stream), "pool_classify")
+
+    def loss(self, net, labels):
+        """Per-image sparse softmax cross-entropy [B] (float32 ndarray) of the features the last forward left in
+        `feat`; also refreshes `logits` / `pred`.  Labels are checked on the host before the launch."""
+        lab = torch.from_numpy(check_class_labels(labels, net.batch, self.feat.C)).to(net.device)
+        out = torch.zeros((net.batch,), dtype=torch.float32, device=net.device)
+        self.launch(net, torch.cuda.current_stream().cuda_stream, lab, out)
+        return out.cpu().numpy()
+
+    def num_launches(self):
+        return 1
+
+    def results(self):
+        """pred int64 [B] (ref RetinaNet.py:127,501-503)."""
+        return self.pred.cpu().numpy()
+
+
 class Detections:
     """Sequence view over packed detection records [M, D*6+2] (host memory): item b is the reference's
     per-image result `[scores f32[K], bbox f32[K,4] (y1,x1,y2,x2), class_id i32[K]]` (SSD300.py:190).

@@ -7,7 +7,7 @@ order so variables get the same TF1 names as in the reference checkpoints
 import numpy as np
 
 from . import lib as L
-from .engine import Net, Tail
+from .engine import ClassifyTail, Net, Tail
 
 F32 = np.float32
 
@@ -155,18 +155,34 @@ def _pyramid(net, feat, top, norm):
     return _bac(net, total, 256, 3, 1, norm), total
 
 
+def _retinanet_resnet(net, cfg):
+    """RetinaNet's `_feature_extractor` (RetinaNet.py:258-285) under the 'feature_extractor' scope of `net`."""
+    blocks = cfg["residual_block_list"]
+    assert cfg["is_bottleneck"], "only the bottleneck variant is on the hot path"
+    filters = [7 * (2 ** i) for i in range(len(blocks))]  # RetinaNet.py:27 quirk
+    return _resnet(net, filters, blocks, cfg["init_conv_filters"], "bn")
+
+
+def build_retinanet_backbone(batch, cfg, precision="fp16", device="cuda", allow_tc=True):
+    """ImageNet-pretraining graph (ref RetinaNet.py:120-127): the same ResNet as build_retinanet -- created first in
+    both graphs, so the variable names match -- and a classification tail on its last bottleneck output (the raw
+    conv + shortcut sum, 4 * 7 * 2^(stages-1) channels: 224 logits for four stages)."""
+    H, W, _ = cfg["data_shape"]
+    net = Net(batch, H, W, precision, device, allow_tc)
+    with net.scope("feature_extractor"):
+        _, _, features = _retinanet_resnet(net, cfg)
+    return net, ClassifyTail(features)
+
+
 def build_retinanet(batch, cfg, precision="fp16", device="cuda", allow_tc=True):
     """ref RetinaNet.py:137-155,258-301."""
     check_num_classes(cfg)
     H, W, _ = cfg["data_shape"]
     nc = cfg["num_classes"] + 1
-    blocks = cfg["residual_block_list"]
-    assert cfg["is_bottleneck"], "only the bottleneck variant is on the hot path"
-    filters = [7 * (2 ** i) for i in range(len(blocks))]  # RetinaNet.py:27 quirk
     net = Net(batch, H, W, precision, device, allow_tc)
     A = 9
     with net.scope("feature_extractor"):
-        f1, f2, f3 = _resnet(net, filters, blocks, cfg["init_conv_filters"], "bn")
+        f1, f2, f3 = _retinanet_resnet(net, cfg)
         p5, _ = _pyramid(net, f3, None, "bn")
         p4, td = _pyramid(net, f2, p5, "bn")
         p3, _ = _pyramid(net, f1, td, "bn")

@@ -177,7 +177,6 @@ def encode_voc_example(jpeg_bytes, shape, ground_truth):
 
 def decode_voc_example(data):
     """-> (image uint8 [H,W,3] RGB, ground_truth float32 [n,5] = (ymin, ymax, xmin, xmax, id))."""
-    import cv2
     ex = parse_example(data)
     for k in ("image", "shape", "ground_truth"):
         if k not in ex or len(ex[k]) == 0:
@@ -187,15 +186,45 @@ def decode_voc_example(data):
             raise RecordError("feature %r is not a bytes list" % k)
     if len(ex["shape"][0]) != 12 or len(ex["ground_truth"][0]) % 20:
         raise RecordError("'shape' must hold 3 int32 and 'ground_truth' rows of 5 float32")
-    shape = np.frombuffer(ex["shape"][0], "<i4")
     gt = np.frombuffer(ex["ground_truth"][0], "<f4").reshape(-1, 5).astype(np.float32)
+    return _decode_image(ex), gt
+
+
+# -------------------------------------------------------- ImageNet schema ---
+def encode_imagenet_example(jpeg_bytes, shape, label):
+    """utils/tfrecord_imagenet_utils.py:83-93: 'image' = JPEG bytes, 'shape' = int32[3] (h, w, c) as bytes,
+    'label' = int64 class id."""
+    return encode_example({"image": jpeg_bytes, "shape": np.asarray(shape, "<i4").tobytes(),
+                           "label": np.asarray([label], np.int64)})
+
+
+def decode_imagenet_example(data):
+    """-> (image uint8 [H,W,3] RGB, label int64) (parse_function, utils/tfrecord_imagenet_utils.py:100-115)."""
+    ex = parse_example(data)
+    for k in ("image", "shape", "label"):
+        if k not in ex or len(ex[k]) == 0:
+            raise RecordError("record lacks the %r feature" % k)
+    for k in ("image", "shape"):
+        if not isinstance(ex[k], list):
+            raise RecordError("feature %r is not a bytes list" % k)
+    if isinstance(ex["label"], list) or ex["label"].dtype != np.int64 or len(ex["label"]) != 1:
+        raise RecordError("'label' must be one int64")
+    if len(ex["shape"][0]) != 12:
+        raise RecordError("'shape' must hold 3 int32")
+    return _decode_image(ex), np.int64(ex["label"][0])
+
+
+def _decode_image(ex):
+    """The 'image' JPEG of a parsed record, RGB, checked against its 'shape' feature."""
+    import cv2
+    shape = np.frombuffer(ex["shape"][0], "<i4")
     img = cv2.imdecode(np.frombuffer(ex["image"][0], np.uint8), cv2.IMREAD_COLOR)
     if img is None:
         raise RecordError("image bytes are not decodable")
     img = cv2.cvtColor(img, cv2.COLOR_BGR2RGB)
     if tuple(img.shape) != tuple(int(x) for x in shape):
         raise RecordError("decoded image %s does not match the stored shape %s" % (img.shape, shape.tolist()))
-    return img, gt
+    return img
 
 
 def _resize_bilinear_aligned(img, oh, ow):
@@ -371,7 +400,11 @@ def preprocess(img, gt, config, rng=None):
     `zoom_size` / `output_shape`, centre or random crop, top-down / left-right flips, colour jitter, rotation, box
     clamping and the centre-inside filter, conversion to (y_c, x_c, h, w, id), `pad_truth_to`.  Randomness comes
     from the seeded numpy generator `rng` (TF's generator is not reproducible outside TF); without one the
-    random steps are skipped."""
+    random steps are skipped.  gt=None (`image_augmentor(ground_truth=None)`, the ImageNet path) returns the
+    image alone."""
+    no_boxes = gt is None
+    if no_boxes:
+        gt = np.zeros((0, 5), np.float32)
     oh, ow = config["output_shape"]
     rot = config.get("rotate")
     if rot is not None:                       # argument checks of :50-59
@@ -454,6 +487,8 @@ def preprocess(img, gt, config, rng=None):
         box = full
     if config.get("data_format") == "channels_first":
         out = np.transpose(out, (2, 0, 1))
+    if no_boxes:
+        return np.ascontiguousarray(out, np.float32)
     return np.ascontiguousarray(out, np.float32), box
 
 
@@ -500,3 +535,19 @@ class BatchIterator:
         if self._it is None:
             self.initialize()
         return next(self._it)
+
+
+class ImageNetBatchIterator(BatchIterator):
+    """`iterator.get_next()` of utils/tfrecord_imagenet_utils.py:118-123: endless batches (images float32 [B,...],
+    labels int64 [B]) of ImageNet records, each image through `preprocess` without boxes."""
+
+    def _examples(self):
+        while True:
+            n = 0
+            for path in self.files:
+                for rec in read_records(path):
+                    n += 1
+                    img, label = decode_imagenet_example(rec)
+                    yield preprocess(img, None, self.config, self.rng), label
+            if n == 0:
+                raise RecordError("no records in %r" % (self.files,))

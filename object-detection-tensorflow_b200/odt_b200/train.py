@@ -252,10 +252,13 @@ class GraphTrainer:
         from . import engine as E
         self.model, self.cfg, self.E = model, model.config, E
         self.kind = {"SSD300": "ssd", "SSD512": "ssd", "RetinaNet": "retina", "YOLOv3": "yolo", "FCOS": "fcos"}[model.name]
+        if getattr(model, "is_pretraining", False):
+            self.kind = "classify"                # RetinaNet's ImageNet-pretraining mode
         self.weight_decay = float(model.weight_decay)
         self.device = torch.device(device if device is not None else ("cuda" if torch.cuda.is_available() else "cpu"))
         self.dtype = dtype
         self.net = model._build_spec()            # unfused op list, no CUDA
+        self.features = self.net.ops[-1].y        # the last tensor of the list (forward_features)
         w = model.get_weights()
         self.params, self.buffers, self.slots = {}, {}, {}
         for name, arr in w.items():
@@ -287,6 +290,17 @@ class GraphTrainer:
 
     def forward_rows(self, images, training=True, stats=None):
         """images [B,H,W,3] -> candidate rows [B,N,25] in the layout of DESIGN.md section 2."""
+        _, rows = self._replay(images, training, stats)
+        return rows.view(rows.shape[0], rows.shape[1] // 25, 25)
+
+    def forward_features(self, images, training=True, stats=None):
+        """images [B,H,W,3] -> the last tensor of the layer list, NCHW (pretraining mode: the last bottleneck's
+        conv + shortcut sum that the classification tail pools)."""
+        val, _ = self._replay(images, training, stats)
+        return val[id(self.features)]
+
+    def _replay(self, images, training, stats):
+        """The layer list with torch ops -> ({id(Act): NCHW value}, head rows [B, N*25])."""
         E, P = self.E, self.params
         stats = [] if stats is None else stats
         x0 = torch.as_tensor(images, device=self.device, dtype=self.dtype)
@@ -335,7 +349,7 @@ class GraphTrainer:
                 val[id(op.y)] = torch.cat([a, _resize_nearest_legacy(b, a.shape[2], a.shape[3])], dim=1)
             else:
                 raise TypeError(type(op))
-        return rows.view(B, N, 25)
+        return val, rows
 
     # ------------------------------------------------------------------ losses --
     def _softmax_anchors(self):
@@ -519,10 +533,27 @@ class GraphTrainer:
         l2 = sum((p * p).sum() for p in self.params.values()) * 0.5
         return data + self.weight_decay * l2, data
 
+    def classify_loss(self, features, labels):
+        """Pretraining mode (RetinaNet.py:123-133): mean-pooled logits, sparse softmax cross-entropy (MEAN over the
+        batch) + weight_decay * sum(l2_loss) over the trainable variables -- all of them live in 'feature_extractor'
+        here.  labels: int64 tensor [B].  Returns (loss, data term, logits)."""
+        data, logits = pooled_xent(features, labels)
+        l2 = sum((p * p).sum() for p in self.params.values()) * 0.5
+        return data + self.weight_decay * l2, data, logits
+
     def step(self, images, ground_truth, lr):
+        """One `sess.run([train_op, loss])`.  Pretraining mode: `ground_truth` is the label vector [B] and the step
+        returns (loss, accuracy of the training-mode logits) like `sess.run([train_op, loss, accuracy])`."""
         stats = []
-        rows = self.forward_rows(images, True, stats)
-        loss, _ = self.total_loss(rows, ground_truth)
+        accuracy = None
+        if self.kind == "classify":
+            lab = self.E.check_class_labels(ground_truth, np.asarray(images).shape[0], self.features.C)
+            lab = torch.from_numpy(lab).to(self.device)
+            loss, _, logits = self.classify_loss(self.forward_features(images, True, stats), lab)
+            accuracy = float((torch.argmax(logits, dim=1) == lab).to(torch.float32).mean())
+        else:
+            rows = self.forward_rows(images, True, stats)
+            loss, _ = self.total_loss(rows, ground_truth)
         names = list(self.params)
         grads = torch.autograd.grad(loss, [self.params[k] for k in names], allow_unused=True)
         with torch.no_grad():
@@ -536,9 +567,18 @@ class GraphTrainer:
                 self.buffers[scope + "/moving_mean"].mul_(BN_MOMENTUM).add_(mean, alpha=1 - BN_MOMENTUM)
                 self.buffers[scope + "/moving_variance"].mul_(BN_MOMENTUM).add_(var, alpha=1 - BN_MOMENTUM)
         self.global_step += 1
+        if accuracy is not None:
+            return float(loss.detach()), accuracy
         return float(loss.detach())
 
     export = SSDTrainer.export
+
+
+def pooled_xent(features, labels):
+    """reduce_mean(features, [H, W]) -> logits [B, C]; tf.losses.sparse_softmax_cross_entropy(labels, logits) with
+    Reduction.MEAN (RetinaNet.py:125-126).  features NCHW, labels int64 [B].  Returns (mean loss, logits)."""
+    logits = features.mean(dim=(2, 3))
+    return F.cross_entropy(logits, labels, reduction="mean"), logits
 
 
 def _resize_bilinear_legacy(x, oh, ow):
