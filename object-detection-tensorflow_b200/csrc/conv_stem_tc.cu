@@ -446,8 +446,10 @@ extern "C" int odt_conv2d_stem_rgbx(const void* rgbx, const void* weights, const
   int variant = 0;
   if (ok && p->R == 3 && p->stride == 1 && p->Cout == 64 && p->in_halo == 1 && p->pad_t == 1 && p->pad_l == 1) variant = 1;
   if (ok && p->R == 3 && p->stride == 1 && p->Cout == 32 && p->in_halo == 1 && p->pad_t == 1 && p->pad_l == 1) variant = 2;
-  if (ok && p->R == 7 && p->stride == 2 && p->Cout == 16 && p->in_halo == 4 && (p->W & 1) == 0 && (p->pad_l & 1) == 0 &&
-      p->pad_t <= 4 && p->pad_l <= 4 &&
+  // 7x7 / 2: up to 16 real outputs.  The kernel computes and stores 16 channels per pixel, so the filter bank, scale and
+  // shift must hold 16 rows (Cout_pad), zero past Cout, and the output row must have room for 16.
+  if (ok && p->R == 7 && p->stride == 2 && p->Cout <= 16 && p->Cout_pad == 16 && p->out0_pix_stride >= 16 &&
+      p->in_halo == 4 && (p->W & 1) == 0 && (p->pad_l & 1) == 0 && p->pad_t <= 4 && p->pad_l <= 4 &&
       // the 8-pixel row window and the 7 filter rows of the last output pixel stay inside the padded image
       (p->OW - 1) * 2 - p->pad_l + 7 <= p->W - 1 + 4 && (p->OH - 1) * 2 - p->pad_t + 6 <= p->H - 1 + 4)
     variant = 3;

@@ -140,6 +140,14 @@ class _Detector:
                 raise tf_checkpoint.CheckpointError(
                     "%s lacks %d of the %d variables to restore (first: %s)" % (prefix, len(missing), len(require),
                                                                              ", ".join(missing[:3])))
+            # same names, other shapes: a checkpoint of the other ResNet unit (RetinaNet's is_bottleneck) -- refused
+            # before anything is restored
+            shapes = r.get_variable_to_shape_map()
+            wrong = [k for k in require if tuple(shapes[k]) != tuple(w[k].shape)]
+            if wrong:
+                raise tf_checkpoint.CheckpointError(
+                    "%s holds %d of the %d variables to restore with another shape (first: %s %s, expected %s)"
+                    % (prefix, len(wrong), len(require), wrong[0], tuple(shapes[wrong[0]]), tuple(w[wrong[0]].shape)))
         n = 0
         for k in (w if require is None else require):
             if r.has_tensor(k):
@@ -474,8 +482,14 @@ class RetinaNet(_Detector):
         self.is_bottleneck = config["is_bottleneck"]
         self.block_list = config["residual_block_list"]
         self.data_shape = config["data_shape"]
-        # ImageNet-pretraining mode (RetinaNet.py:61-69,120-135) classifies into 4 * filters[-1] classes; the
-        # configured num_classes is unused there
+        # the basic unit's first shortcut adds pool1 (init_conv_filters channels) to a 7-channel branch
+        # (RetinaNet.py:277-279,621-632): TF's shape check builds that graph only for 7 (or the broadcast 1, which this
+        # path does not reproduce: DESIGN.md section 1)
+        if not self.is_bottleneck and config["init_conv_filters"] != 7:
+            raise ValueError("is_bottleneck=False: block1_unit1 adds pool1 (init_conv_filters = %r channels) to its "
+                             "7-channel conv branch; init_conv_filters must be 7" % (config["init_conv_filters"],))
+        # ImageNet-pretraining mode (RetinaNet.py:61-69,120-135) classifies into num_logits classes; the configured
+        # num_classes is unused there
         if not self.is_pretraining:
             nets.check_num_classes(config)
         self.num_classes = config["num_classes"] + 1
@@ -492,8 +506,9 @@ class RetinaNet(_Detector):
     # ---- ImageNet-pretraining mode (ref RetinaNet.py:476-519) -------------------------------------------------------
     @property
     def num_logits(self):
-        """Width of the pretraining-mode logits: 4 * filters[-1] with filters = 7 * 2^i (RetinaNet.py:27)."""
-        return 4 * 7 * 2 ** (len(self.block_list) - 1)
+        """Width of the pretraining-mode logits, the last unit's output channels with filters = 7 * 2^i
+        (RetinaNet.py:27): 4 * filters[-1] for the bottleneck variant, filters[-1] for the basic one."""
+        return (4 if self.is_bottleneck else 1) * 7 * 2 ** (len(self.block_list) - 1)
 
     def test_one_image(self, images):
         """Detection: [scores, bbox, class_id] (ref RetinaNet.py:505-507).  Pretraining mode: int64 [B] = the first

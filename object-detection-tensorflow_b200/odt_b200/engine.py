@@ -214,8 +214,20 @@ class ConvOp(Op):
             force3 = os.environ.get("ODT_STEM_RGBX") == "2"
             if (R, self.stride, cout) in ((3, 1, 64), (3, 1, 32)) and force3:
                 self.rgbx = 1
-            elif (R, self.stride, cout) == (7, 2, 16) and Wd % 2 == 0 and pl % 2 == 0 and pl <= 4 and pt <= 4:
+            elif (R, self.stride) == (7, 2) and cout <= 16 and Wd % 2 == 0 and pl % 2 == 0 and pl <= 4 and pt <= 4:
                 self.rgbx = 4
+        if self.rgbx == 4 and cout < 16:
+            # the packed 7x7 stem computes 16 outputs (RetinaNet's basic variant has 7): filter rows, BN scale and
+            # shift are zero past `cout`, so the pad lanes its whole-sector store writes stay zero
+            wp = np.zeros((16,) + ohwi.shape[1:], np.float32)
+            wp[:cout] = ohwi
+            self.wdev = torch.from_numpy(wp).to(dev).to(adt).contiguous()
+            sc16, sh16 = np.zeros(16, np.float32), np.zeros(16, np.float32)
+            sc16[:cout] = 1.0 if scale is None else scale
+            sh16[:cout] = shift
+            self.scale, self.shift = torch.from_numpy(sc16).to(dev), torch.from_numpy(sh16).to(dev)
+            p.scale, p.shift = self.scale.data_ptr(), self.shift.data_ptr()
+            self.cout_pad = p.Cout_pad = 16
         if self.rgbx:
             P = self.rgbx
             net.image_rgbx = torch.zeros((B, H + 2 * P, Wd + 2 * P, 4), dtype=torch.float16, device=dev)
@@ -1137,6 +1149,11 @@ def init_weights(variables, seed=1, bn_mode="tf_init", stem_scale=1.0 / 64.0):
             # RetinaNet.py:641-643): halve the variance of each so random-init
             # activations do not double per block (2^16 over 16 blocks)
             if "/conv_branch/conv2d_2/" in name or "/identity_branch/conv2d/" in name:
+                out[name] *= np.float32(math.sqrt(0.5))
+            # basic units (RetinaNet.py:621-632) end their conv branch in conv2d_1 and add the unit's input at stride
+            # 1: damp that conv likewise, or the variance would double per unit
+            if name.endswith("/conv_branch/conv2d_1/kernel") and \
+                    name.replace("/conv2d_1/", "/conv2d_2/") not in variables:
                 out[name] *= np.float32(math.sqrt(0.5))
             # Darknet residual x + f(x) (YOLOv3.py:488-491): damp f's last conv likewise
             mres = re.match(r"backone/block\d+/conv2d_(\d+)/kernel", name)

@@ -126,8 +126,22 @@ def _bottleneck(net, x, f, stride, scope, norm):
     return y
 
 
-def _resnet(net, filters, blocks, stem_filters, norm):
-    """stem 7x7 s2 + norm + ReLU, maxpool 3/2, bottleneck stacks
+def _basic(net, x, f, stride, scope, norm):
+    """_residual_block (RetinaNet.py:621-632): two 3x3 convs + shortcut.  The shortcut is x itself at stride 1 (no
+    identity_branch variables) and a 3x3 conv of stride `stride` otherwise."""
+    with net.scope(scope):
+        sc = x
+        if stride != 1:
+            with net.scope("identity_branch"):
+                sc = _bac(net, x, f, 3, stride, norm)
+        with net.scope("conv_branch"):
+            y = _bac(net, x, f, 3, stride, norm)
+            y = _bac(net, y, f, 3, 1, norm, residual=sc)  # residual add fused
+    return y
+
+
+def _resnet(net, filters, blocks, stem_filters, norm, unit=_bottleneck):
+    """stem 7x7 s2 + norm + ReLU, maxpool 3/2, residual-unit stacks
     (RetinaNet.py:258-285, FCOS.py:72-97)."""
     if norm == "bn":
         y = net.conv(None, stem_filters, 7, 2, bn=True, act="relu")
@@ -136,12 +150,12 @@ def _resnet(net, filters, blocks, stem_filters, norm):
     y = net.maxpool(y, 3, 2)
     ends = []
     for i in range(blocks[0]):
-        y = _bottleneck(net, y, filters[0], 1, "block1_unit%d" % (i + 1), norm)
+        y = unit(net, y, filters[0], 1, "block1_unit%d" % (i + 1), norm)
     ends.append(y)
     for i in range(1, len(blocks)):
-        y = _bottleneck(net, y, filters[i], 2, "block%d_unit1" % (i + 1), norm)
+        y = unit(net, y, filters[i], 2, "block%d_unit1" % (i + 1), norm)
         for j in range(1, blocks[i]):
-            y = _bottleneck(net, y, filters[i], 1, "block%d_unit%d" % (i + 1, j + 1), norm)
+            y = unit(net, y, filters[i], 1, "block%d_unit%d" % (i + 1, j + 1), norm)
         ends.append(y)
     return ends[-3], ends[-2], ends[-1]
 
@@ -158,15 +172,16 @@ def _pyramid(net, feat, top, norm):
 def _retinanet_resnet(net, cfg):
     """RetinaNet's `_feature_extractor` (RetinaNet.py:258-285) under the 'feature_extractor' scope of `net`."""
     blocks = cfg["residual_block_list"]
-    assert cfg["is_bottleneck"], "only the bottleneck variant is on the hot path"
     filters = [7 * (2 ** i) for i in range(len(blocks))]  # RetinaNet.py:27 quirk
-    return _resnet(net, filters, blocks, cfg["init_conv_filters"], "bn")
+    unit = _bottleneck if cfg["is_bottleneck"] else _basic  # RetinaNet.py:272-275
+    return _resnet(net, filters, blocks, cfg["init_conv_filters"], "bn", unit)
 
 
 def build_retinanet_backbone(batch, cfg, precision="fp16", device="cuda", allow_tc=True):
     """ImageNet-pretraining graph (ref RetinaNet.py:120-127): the same ResNet as build_retinanet -- created first in
-    both graphs, so the variable names match -- and a classification tail on its last bottleneck output (the raw
-    conv + shortcut sum, 4 * 7 * 2^(stages-1) channels: 224 logits for four stages)."""
+    both graphs, so the variable names match -- and a classification tail on its last unit's output (the raw
+    conv + shortcut sum: 4 * 7 * 2^(stages-1) channels for the bottleneck variant, 224 logits for four stages;
+    7 * 2^(stages-1) for the basic one, 56 logits)."""
     H, W, _ = cfg["data_shape"]
     net = Net(batch, H, W, precision, device, allow_tc)
     with net.scope("feature_extractor"):
