@@ -192,19 +192,26 @@ int odt_upsample_bilinear_add(const void* top, const void* a, void* out, int dty
 int odt_upsample_nearest_concat(const void* a, const void* b, void* out, int dtype, int B, int H,
                                 int W, int Ca, int lda, int BH, int BW, int Cb, int ldb, int ldo,
                                 void* stream);
-/* GroupNorm(groups) statistics: stats[b][g] = (mean, rstd), eps inside.  `stats` must be
- * 8-byte aligned and hold B*groups*6 floats: the B*groups*2 results followed by an fp64
- * accumulation workspace.  ref: FCOS.py:438-446 */
+/* GroupNorm(groups) statistics: stats[b][g] = (mean, rstd), eps inside; stats holds B*groups*2 floats.
+ * One CTA per (group, image), two passes (mean, then the sum of squared deviations) in a fixed order: the result
+ * does not depend on B or on scheduling.  ref: FCOS.py:438-446 */
 int odt_groupnorm_stats(const void* in, float* stats, int dtype, int B, long long hw, int C,
                         int ld, int groups, float eps, void* stream);
 /* y = act((x-mean)*rstd*gamma[c] + beta[c]) */
 int odt_groupnorm_apply(const void* in, void* out, const float* stats, int dtype, int B,
                         long long hw, int C, int ld, int groups, const float* gamma,
                         const float* beta, int act, void* stream);
-/* GroupNorm + activation in two launches (power-of-two C and groups, 16-byte aligned tensors):
- * `acc_zeroed` = B*groups*2 doubles the CALLER has zeroed (e.g. one memset of an arena per forward);
- * returns ODT_ERR_UNSUPPORTED (nothing launched) for other shapes -- use stats + apply then. */
-int odt_groupnorm_act(const void* in, void* out, double* acc_zeroed, int dtype, int B, long long hw, int C,
+/* Bytes of the workspace odt_groupnorm_act needs for this shape; 0 when the shape is outside its two-launch path
+ * (C and groups powers of two, C a multiple of the vector width (8 fp16 / 4 fp32) and at most 256 vectors,
+ * groups <= 64, B*groups <= 6144). */
+long long odt_groupnorm_act_workspace_bytes(int dtype, int B, long long hw, int C, int groups);
+/* GroupNorm + activation in two launches.  Statistics: each image is cut into pixel slices chosen from (hw, C) alone;
+ * every slice is reduced two-pass in a fixed order and the last CTA of the image merges the slices in a fixed order in
+ * fp64, so the output is reproducible and does not depend on B.  `workspace`: odt_groupnorm_act_workspace_bytes()
+ * bytes, 8-byte aligned, zeroed by the caller before its first use (the launch leaves it zeroed where that matters:
+ * its per-image arrival counters).  Returns ODT_ERR_UNSUPPORTED (nothing launched) for other shapes or for tensors
+ * that are not 16-byte aligned -- use stats + apply then. */
+int odt_groupnorm_act(const void* in, void* out, void* workspace, int dtype, int B, long long hw, int C,
                       int ld, int groups, float eps, const float* gamma, const float* beta, int act,
                       void* stream);
 

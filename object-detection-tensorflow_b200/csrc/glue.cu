@@ -456,7 +456,7 @@ __global__ void groupnorm_stats_kernel(const T* __restrict__ in, float* __restri
   const int cpg = C / groups;
   const T* base = in + (long long)b * hw * ld + g * cpg;
   const long long n = hw * cpg;
-  __shared__ float red[32];
+  __shared__ float red[32], red2[32];
   __shared__ float s_mean;
   float acc = 0.f;
   for (long long i = threadIdx.x; i < n; i += blockDim.x)
@@ -473,81 +473,186 @@ __global__ void groupnorm_stats_kernel(const T* __restrict__ in, float* __restri
   }
   __syncthreads();
   const float mean = s_mean;
+  // sum (x - mean)^2 and sum (x - mean): the second corrects for the rounding of `mean` (corrected two-pass)
   acc = 0.f;
+  float accd = 0.f;
   for (long long i = threadIdx.x; i < n; i += blockDim.x) {
     float d = Elem<T>::ld(base + (i / cpg) * ld + (i % cpg)) - mean;
+    accd += d;
     acc = fmaf(d, d, acc);
   }
 #pragma unroll
-  for (int o = 16; o; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  for (int o = 16; o; o >>= 1) {
+    acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    accd += __shfl_xor_sync(0xffffffffu, accd, o);
+  }
   __syncthreads();
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
+  if ((threadIdx.x & 31) == 0) red2[threadIdx.x >> 5] = accd;
   __syncthreads();
   if (threadIdx.x < 32) {
     float v = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
+    float vd = threadIdx.x < (blockDim.x >> 5) ? red2[threadIdx.x] : 0.f;
 #pragma unroll
-    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    for (int o = 16; o; o >>= 1) {
+      v += __shfl_xor_sync(0xffffffffu, v, o);
+      vd += __shfl_xor_sync(0xffffffffu, vd, o);
+    }
     if (threadIdx.x == 0) {
-      float var = v / (float)n;
-      stats[((long long)b * groups + g) * 2 + 0] = mean;
+      const double sd = vd, m2 = (double)v - sd * sd / (double)n;
+      const float var = (float)(m2 > 0.0 ? m2 / (double)n : 0.0);
+      stats[((long long)b * groups + g) * 2 + 0] = (float)((double)mean + sd / (double)n);
       stats[((long long)b * groups + g) * 2 + 1] = __frsqrt_rn(var + eps);
     }
   }
 }
 
-// Parallel statistics: grid (blocks, B); every thread owns one channel vector
-// (so its group(s) are fixed) and a strided set of pixels; fp32 partials per
-// thread -> shared fp32 per group -> one fp64 atomicAdd per (block, group).
-template <typename T, int V>
-__global__ void __launch_bounds__(256)
-    groupnorm_partial_kernel(const T* __restrict__ in, double* __restrict__ acc, long long hw, int C,
-                             int ld, int groups, long long pix_per_block) {
+// Statistics of the two-launch path (odt_groupnorm_act), fixed-order and batch-invariant.  Every image is cut into
+// slices of kGnThreads * kGnSliceVecs channel vectors (the partition depends on hw and C only, never on B); one CTA per
+// (slice, image).  A thread owns one channel vector (so its group(s) are fixed) and kGnSliceVecs pixels, kept in
+// registers; the slice is reduced twice in a fixed order, no float atomics: the slice mean m, then sum (x - m)^2 and
+// sum (x - m) (which corrects for the rounding of m), giving (mean_s, M2_s) per group in fp64, stored to the slice's
+// slot.  The last CTA of an image to arrive (threadfence + an integer counter, which it resets) merges the image's
+// slots in a fixed order in fp64 about the first slice's mean, and writes (mean, rstd) for groupnorm_apply_kernel.
+constexpr int kGnThreads = 256, kGnSliceVecs = 8, kGnMaxGroups = 64;
+
+// pixels per slice for C channels in vectors of V
+static inline long long gn_slice_pixels(int C, int V) { return (long long)(kGnThreads / (C / V)) * kGnSliceVecs; }
+
+// GPV: groups per channel vector (1 when a group spans whole vectors)
+template <typename T, int V, int GPV>
+__global__ void __launch_bounds__(kGnThreads)
+    groupnorm_slice_kernel(const T* __restrict__ in, double* __restrict__ slots, float* __restrict__ stats,
+                           unsigned* __restrict__ arrivals, long long hw, int C, int ld, int groups, int pps,
+                           float eps) {
   pdl_launch_dependents();
-  constexpr int NGMAX = 8;
-  __shared__ float s_acc[64][2];
-  const int b = blockIdx.y;
+  constexpr int NG = GPV, QPG = V / GPV;  // (QPG: channels of one group in a vector when GPV > 1)
+  __shared__ float s_a[kGnThreads][NG], s_b[kGnThreads][NG];
+  __shared__ double s_mean[kGnMaxGroups];
+  __shared__ double s_m[kGnThreads][2];
+  __shared__ bool s_last;
+  const int S = gridDim.x, s = blockIdx.x, b = blockIdx.y;
   const int cv = C / V, cpg = C / groups;
-  const int cvi = threadIdx.x % cv, pl = threadIdx.x / cv, pstep = blockDim.x / cv;
-  const int c0 = cvi * V;
-  const int ng = cpg >= V ? 1 : V / cpg;  // groups spanned by one vector
-  for (int i = threadIdx.x; i < groups * 2; i += blockDim.x) (&s_acc[0][0])[i] = 0.f;
-  __syncthreads();
-  float sum[NGMAX], sq[NGMAX];
+  const int cvi = threadIdx.x % cv, pl = threadIdx.x / cv, pstep = kGnThreads / cv;
+  const long long p0 = (long long)s * pps, p1 = min(hw, p0 + pps);
+  const T* base = in + (long long)b * hw * ld + cvi * V;
+  uint4 raw[kGnSliceVecs];
+  int nv = 0;  // valid pixels of this thread: a prefix of j
 #pragma unroll
-  for (int q = 0; q < NGMAX; ++q) sum[q] = sq[q] = 0.f;
-  const long long p0 = (long long)blockIdx.x * pix_per_block;
-  const long long p1 = min(hw, p0 + pix_per_block);
-  const T* base = in + (long long)b * hw * ld + c0;
-  for (long long p = p0 + pl; p < p1; p += pstep) {
-    float v[V];
-    VecIO<T, V>::ld(base + p * ld, v);
-#pragma unroll
-    for (int q = 0; q < V; ++q) {
-      const int gl = cpg >= V ? 0 : q / cpg;
-      sum[gl] += v[q];
-      sq[gl] = fmaf(v[q], v[q], sq[gl]);
+  for (int j = 0; j < kGnSliceVecs; ++j) {
+    const long long p = p0 + pl + (long long)j * pstep;
+    if (p < p1) {
+      raw[j] = __ldg(reinterpret_cast<const uint4*>(base + p * ld));
+      nv = j + 1;
     }
   }
-  const int g0 = c0 / cpg;
-  for (int q = 0; q < ng; ++q) {
-    atomicAdd(&s_acc[g0 + q][0], sum[q]);
-    atomicAdd(&s_acc[g0 + q][1], sq[q]);
+  // pass 1: slice mean per group
+  float acc[NG], acc2[NG];
+#pragma unroll
+  for (int q = 0; q < NG; ++q) acc[q] = 0.f;
+#pragma unroll
+  for (int j = 0; j < kGnSliceVecs; ++j) {
+    if (j < nv) {
+      float v[V];
+      VecIO<T, V>::ld(reinterpret_cast<const T*>(&raw[j]), v);
+#pragma unroll
+      for (int q = 0; q < V; ++q) acc[GPV == 1 ? 0 : q / QPG] += v[q];
+    }
+  }
+#pragma unroll
+  for (int q = 0; q < NG; ++q) s_a[threadIdx.x][q] = acc[q];
+  __syncthreads();
+  // the threads of group g, in a fixed order: (pixel lane, channel vector[, group within the vector])
+  const int vpg = GPV == 1 ? cpg / V : 1;
+  const double n_s = (double)(p1 - p0) * cpg;
+  if (threadIdx.x < groups) {
+    const int g = threadIdx.x;
+    const int c0 = GPV == 1 ? g * vpg : g / GPV, gq = GPV == 1 ? 0 : g % GPV;
+    double a = 0.0;
+    for (int l = 0; l < pstep; ++l)
+      for (int k = 0; k < vpg; ++k) a += s_a[l * cv + c0 + k][gq];
+    s_mean[g] = a / n_s;
   }
   __syncthreads();
-  for (int i = threadIdx.x; i < groups * 2; i += blockDim.x)
-    atomicAdd(acc + (long long)b * groups * 2 + i, (double)(&s_acc[0][0])[i]);
-}
-
-__global__ void groupnorm_finalize_kernel(const double* __restrict__ acc, float* __restrict__ stats,
-                                          int total, double n, float eps) {
-  pdl_launch_dependents();
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= total) return;
-  const double mean = acc[2 * i] / n;
-  double var = acc[2 * i + 1] / n - mean * mean;
-  if (var < 0.0) var = 0.0;
-  stats[2 * i] = (float)mean;
-  stats[2 * i + 1] = (float)(1.0 / sqrt(var + (double)eps));
+  // pass 2 (from registers): sum (x - m) and sum (x - m)^2 about the fp32 slice mean m
+  const int g0 = cvi * V / cpg;
+  float m[NG];
+#pragma unroll
+  for (int q = 0; q < NG; ++q) {
+    m[q] = (float)s_mean[g0 + q];
+    acc[q] = acc2[q] = 0.f;
+  }
+#pragma unroll
+  for (int j = 0; j < kGnSliceVecs; ++j) {
+    if (j < nv) {
+      float v[V];
+      VecIO<T, V>::ld(reinterpret_cast<const T*>(&raw[j]), v);
+#pragma unroll
+      for (int q = 0; q < V; ++q) {
+        const int gl = GPV == 1 ? 0 : q / QPG;
+        const float d = v[q] - m[gl];
+        acc[gl] += d;
+        acc2[gl] = fmaf(d, d, acc2[gl]);
+      }
+    }
+  }
+#pragma unroll
+  for (int q = 0; q < NG; ++q) {
+    s_a[threadIdx.x][q] = acc[q];
+    s_b[threadIdx.x][q] = acc2[q];
+  }
+  __syncthreads();
+  if (threadIdx.x < groups) {
+    const int g = threadIdx.x;
+    const int c0 = GPV == 1 ? g * vpg : g / GPV, gq = GPV == 1 ? 0 : g % GPV;
+    double sd = 0.0, sq = 0.0;
+    for (int l = 0; l < pstep; ++l)
+      for (int k = 0; k < vpg; ++k) {
+        sd += s_a[l * cv + c0 + k][gq];
+        sq += s_b[l * cv + c0 + k][gq];
+      }
+    const double m2 = sq - sd * sd / n_s;
+    double* slot = slots + (((long long)b * S + s) * groups + g) * 2;
+    slot[0] = (double)(float)s_mean[g] + sd / n_s;
+    slot[1] = m2 > 0.0 ? m2 : 0.0;
+  }
+  // the last CTA of this image merges its S slots
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) s_last = atomicAdd(arrivals + b, 1u) == (unsigned)S - 1;
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  const int L = kGnThreads / groups;  // lanes per group; lane l takes slices l, l + L, ...
+  const int g = threadIdx.x % groups, l = threadIdx.x / groups;
+  const double* sl = slots + (long long)b * S * groups * 2;
+  const double K = __ldcg(sl + g * 2);  // shift: the first slice's mean
+  if (l < L) {
+    double A = 0.0, Q = 0.0;
+    for (int t = l; t < S; t += L) {
+      const double mt = __ldcg(sl + ((long long)t * groups + g) * 2), m2t = __ldcg(sl + ((long long)t * groups + g) * 2 + 1);
+      const long long q0 = (long long)t * pps;
+      const double nt = (double)(min(hw, q0 + pps) - q0) * cpg, d = mt - K;
+      A = fma(nt, d, A);
+      Q += fma(nt * d, d, m2t);
+    }
+    s_m[threadIdx.x][0] = A;
+    s_m[threadIdx.x][1] = Q;
+  }
+  __syncthreads();
+  if (threadIdx.x < groups) {
+    double A = 0.0, Q = 0.0;
+    for (int k = 0; k < L; ++k) {
+      A += s_m[k * groups + g][0];
+      Q += s_m[k * groups + g][1];
+    }
+    const double N = (double)hw * cpg;
+    // sum over the image of (x - mean)^2 = Q - N (mean - K)^2, with N (mean - K) = A
+    const double m2 = Q - A * A / N, var = m2 > 0.0 ? m2 / N : 0.0;
+    stats[((long long)b * groups + g) * 2] = (float)(K + A / N);
+    stats[((long long)b * groups + g) * 2 + 1] = (float)(1.0 / sqrt(var + (double)eps));
+  }
+  if (threadIdx.x == 0) arrivals[b] = 0u;
 }
 
 template <typename T, int V>
@@ -582,22 +687,16 @@ __global__ void groupnorm_apply_kernel(const T* __restrict__ in, T* __restrict__
   }
 }
 
-// apply with the finalisation folded in: every block first turns the (sum, sum of squares)
-// accumulators of all (image, group) pairs into (mean, rstd) in shared memory
+// apply of the two-launch path: every block first copies the (mean, rstd) of all (image, group) pairs that
+// groupnorm_slice_kernel wrote into shared memory
 template <typename T, int V>
 __global__ void __launch_bounds__(256)
-    groupnorm_apply_acc_kernel(const T* __restrict__ in, T* __restrict__ out, const double* __restrict__ acc,
-                               int B, long long hw, int C, int ld, int groups, double n, float eps,
+    groupnorm_apply_acc_kernel(const T* __restrict__ in, T* __restrict__ out, const float* __restrict__ stats,
+                               int B, long long hw, int C, int ld, int groups,
                                const float* __restrict__ gamma, const float* __restrict__ beta, int act) {
   pdl_launch_dependents();
   extern __shared__ float s_stat[];  // [B*groups][2]
-  for (int i = threadIdx.x; i < B * groups; i += blockDim.x) {
-    const double mean = acc[2 * i] / n;
-    double var = acc[2 * i + 1] / n - mean * mean;
-    if (var < 0.0) var = 0.0;
-    s_stat[2 * i] = (float)mean;
-    s_stat[2 * i + 1] = (float)(1.0 / sqrt(var + (double)eps));
-  }
+  for (int i = threadIdx.x; i < B * groups * 2; i += blockDim.x) s_stat[i] = stats[i];
   __syncthreads();
   const int cv = C / V;
   const int cpg = C / groups;
@@ -827,38 +926,11 @@ extern "C" int odt_upsample_nearest_concat(const void* a, const void* b, void* o
 
 extern "C" int odt_groupnorm_stats(const void* in, float* stats, int dtype, int B, long long hw,
                                    int C, int ld, int groups, float eps, void* stream) {
-  ODT_CHECK_ARG(in && stats && B > 0 && hw > 0 && C > 0 && ld >= C && groups > 0 && C % groups == 0,
+  ODT_CHECK_ARG(in && stats && B > 0 && B <= 65535 && hw > 0 && C > 0 && ld >= C && groups > 0 && C % groups == 0,
                 "args");
   cudaStream_t st = (cudaStream_t)stream;
-  const int cpg = C / groups;
-  const bool pow2 = (C & (C - 1)) == 0 && (groups & (groups - 1)) == 0;
   DISPATCH_DTYPE(dtype, {
-    constexpr int V = FullVec<T>::V;
-    const int cv = C / V;
-    const bool fast = pow2 && C % V == 0 && cv <= 256 && groups <= 64 && ld % V == 0 &&
-                      ((uintptr_t)in % 16) == 0 && (cpg >= V ? cpg % V == 0 : V % cpg == 0) &&
-                      (cpg >= V || V / cpg <= 8);
-    if (fast) {
-      // workspace: B*groups*2 doubles behind the B*groups*2 result floats
-      double* acc = reinterpret_cast<double*>(stats + (long long)B * groups * 2);
-      ODT_CHECK_ARG(((uintptr_t)acc & 7) == 0, "stats must be 8-byte aligned");
-      ODT_CUDA_OK(cudaMemsetAsync(acc, 0, sizeof(double) * (size_t)B * groups * 2, st));
-      long long blocks = (long long)kNumSMs * 4 / B;
-      if (blocks < 1) blocks = 1;
-      long long ppb = (hw + blocks - 1) / blocks;
-      const long long min_ppb = 256 / cv * 8;  // at least 8 vectors per thread
-      if (ppb < min_ppb) ppb = min_ppb;
-      blocks = (hw + ppb - 1) / ppb;
-      groupnorm_partial_kernel<T, V><<<dim3((unsigned)blocks, B), 256, 0, st>>>(
-          (const T*)in, acc, hw, C, ld, groups, ppb);
-      ODT_LAUNCH_OK();
-      const int total = B * groups;
-      groupnorm_finalize_kernel<<<(total + 127) / 128, 128, 0, st>>>(acc, stats, total,
-                                                                     (double)hw * cpg, eps);
-    } else {
-      dim3 grid(groups, B);
-      groupnorm_stats_kernel<T><<<grid, 1024, 0, st>>>((const T*)in, stats, hw, C, ld, groups, eps);
-    }
+    groupnorm_stats_kernel<T><<<dim3(groups, B), 1024, 0, st>>>((const T*)in, stats, hw, C, ld, groups, eps);
   })
   ODT_LAUNCH_OK();
   return ODT_OK;
@@ -887,38 +959,71 @@ extern "C" int odt_groupnorm_apply(const void* in, void* out, const float* stats
   return ODT_OK;
 }
 
-// GroupNorm + activation in two launches: parallel (sum, sum^2) accumulation into the caller's
-// PRE-ZEROED fp64 workspace, then normalise with the finalisation done per block.
-extern "C" int odt_groupnorm_act(const void* in, void* out, double* acc_zeroed, int dtype, int B, long long hw,
+// ---- GroupNorm + activation in two launches -----------------------------------
+// workspace: slots [B][S][groups] x (mean_s, M2_s) doubles | stats [B][groups] x (mean, rstd) floats | B arrival counters
+static bool gn_fused_shape(int V, int B, int C, int groups) {
+  return B > 0 && B <= 65535 && C > 0 && groups > 0 && (C & (C - 1)) == 0 && (groups & (groups - 1)) == 0 &&
+         C % groups == 0 && C % V == 0 && C / V <= kGnThreads && groups <= kGnMaxGroups &&
+         (long long)B * groups * 2 * sizeof(float) <= 48 * 1024;  // the apply kernel's shared-memory copy of the stats
+}
+
+static long long gn_slices(long long hw, int C, int V) {
+  const long long pps = gn_slice_pixels(C, V);
+  return (hw + pps - 1) / pps;
+}
+
+static long long gn_workspace_bytes(int V, int B, long long hw, int C, int groups) {
+  return (long long)sizeof(double) * B * gn_slices(hw, C, V) * groups * 2 + (long long)sizeof(float) * B * groups * 2 +
+         (long long)sizeof(unsigned) * B;
+}
+
+extern "C" long long odt_groupnorm_act_workspace_bytes(int dtype, int B, long long hw, int C, int groups) {
+  const int V = dtype == ODT_F16 ? FullVec<__half>::V : dtype == ODT_F32 ? FullVec<float>::V : 0;
+  if (V == 0 || hw <= 0 || !gn_fused_shape(V, B, C, groups)) return 0;
+  return gn_workspace_bytes(V, B, hw, C, groups);
+}
+
+template <typename T, int V, int GPV>
+static void gn_launch_slices(dim3 grid, cudaStream_t st, const T* in, double* slots, float* stats, unsigned* arrivals,
+                             long long hw, int C, int ld, int groups, int pps, float eps) {
+  if constexpr (GPV <= V)
+    groupnorm_slice_kernel<T, V, GPV><<<grid, kGnThreads, 0, st>>>(in, slots, stats, arrivals, hw, C, ld, groups, pps,
+                                                                   eps);
+}
+
+extern "C" int odt_groupnorm_act(const void* in, void* out, void* workspace, int dtype, int B, long long hw,
                                  int C, int ld, int groups, float eps, const float* gamma, const float* beta,
                                  int act, void* stream) {
-  ODT_CHECK_ARG(in && out && acc_zeroed && B > 0 && hw > 0 && C > 0 && ld >= C && groups > 0 && C % groups == 0,
+  ODT_CHECK_ARG(in && out && workspace && B > 0 && hw > 0 && C > 0 && ld >= C && groups > 0 && C % groups == 0,
                 "args");
-  ODT_CHECK_ARG(((uintptr_t)acc_zeroed & 7) == 0, "workspace must be 8-byte aligned");
-  ODT_CHECK_ARG((long long)B * groups * 2 * 4 <= 48 * 1024, "B * groups too large for the in-kernel finalisation");
+  ODT_CHECK_ARG(((uintptr_t)workspace & 7) == 0, "workspace must be 8-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
-  const int cpg = C / groups;
-  const bool pow2 = (C & (C - 1)) == 0 && (groups & (groups - 1)) == 0;
   int rc = ODT_ERR_UNSUPPORTED;
   DISPATCH_DTYPE(dtype, {
     constexpr int V = FullVec<T>::V;
-    const int cv = C / V;
-    const bool fast = pow2 && C % V == 0 && cv <= 256 && groups <= 64 && ld % V == 0 &&
-                      ((uintptr_t)in % 16) == 0 && ((uintptr_t)out % 16) == 0 &&
-                      (cpg >= V ? cpg % V == 0 : V % cpg == 0) && (cpg >= V || V / cpg <= 8);
+    const bool fast = gn_fused_shape(V, B, C, groups) && ld % V == 0 && ((uintptr_t)in % 16) == 0 &&
+                      ((uintptr_t)out % 16) == 0 && gn_slices(hw, C, V) <= 0x7fffffff;
     if (fast) {
-      long long blocks = (long long)kNumSMs * 4 / B;
-      if (blocks < 1) blocks = 1;
-      long long ppb = (hw + blocks - 1) / blocks;
-      const long long min_ppb = 256 / cv * 8;
-      if (ppb < min_ppb) ppb = min_ppb;
-      blocks = (hw + ppb - 1) / ppb;
-      groupnorm_partial_kernel<T, V><<<dim3((unsigned)blocks, B), 256, 0, st>>>((const T*)in, acc_zeroed, hw, C, ld,
-                                                                             groups, ppb);
+      const int cpg = C / groups, gpv = cpg >= V ? 1 : V / cpg;
+      const long long S = gn_slices(hw, C, V);
+      double* slots = (double*)workspace;
+      float* stats = (float*)(slots + (long long)B * S * groups * 2);
+      unsigned* arrivals = (unsigned*)(stats + (long long)B * groups * 2);
+      const dim3 grid((unsigned)S, (unsigned)B);
+      const int pps = (int)gn_slice_pixels(C, V);
+      const T* x = (const T*)in;
+      if (gpv == 1)
+        gn_launch_slices<T, V, 1>(grid, st, x, slots, stats, arrivals, hw, C, ld, groups, pps, eps);
+      else if (gpv == 2)
+        gn_launch_slices<T, V, 2>(grid, st, x, slots, stats, arrivals, hw, C, ld, groups, pps, eps);
+      else if (gpv == 4)
+        gn_launch_slices<T, V, 4>(grid, st, x, slots, stats, arrivals, hw, C, ld, groups, pps, eps);
+      else
+        gn_launch_slices<T, V, 8>(grid, st, x, slots, stats, arrivals, hw, C, ld, groups, pps, eps);
       ODT_LAUNCH_OK();
-      const long long work = (long long)B * hw * cv;
+      const long long work = (long long)B * hw * (C / V);
       groupnorm_apply_acc_kernel<T, V><<<grid_for(work, 256), 256, (size_t)B * groups * 2 * sizeof(float), st>>>(
-          (const T*)in, (T*)out, acc_zeroed, B, hw, C, ld, groups, (double)hw * cpg, eps, gamma, beta, act);
+          x, (T*)out, stats, B, hw, C, ld, groups, gamma, beta, act);
       ODT_LAUNCH_OK();
       rc = ODT_OK;
     }

@@ -346,19 +346,23 @@ class GroupNormActOp(Op):
     def __init__(self, x, y, gn, act, groups=8):
         self.x, self.y, self.gn, self.act, self.groups = x, y, gn, act, groups
         self.reads, self.writes = (x,), (y,)
-        self.acc = None  # slice of the net's fp64 arena (zeroed once per forward): the two-launch path
+        self.acc = None  # slice of the net's arena (zeroed once per forward): the two-launch path's workspace
 
     def prepare(self, net):
         dev = net.device
         self.gamma = torch.from_numpy(np.asarray(net.weights[self.gn + "/gamma"], np.float32)).to(dev)
         self.beta = torch.from_numpy(np.asarray(net.weights[self.gn + "/beta"], np.float32)).to(dev)
         self.stats = torch.zeros(self.x.B * self.groups * 6, dtype=torch.float32, device=dev)
-        x = self.x
-        C_, g = x.C, self.groups
-        self.two_launch = (net.gn_arena is not None and (C_ & (C_ - 1)) == 0 and (g & (g - 1)) == 0
-                           and x.B * g * 8 <= 48 * 1024)
+        n = self.workspace_doubles(net)
+        self.two_launch = net.gn_arena is not None and n > 0
         if self.two_launch:
-            self.acc = net.gn_take(x.B * g * 2)
+            self.acc = net.gn_take(n)
+
+    def workspace_doubles(self, net):
+        """fp64 words of odt_groupnorm_act's workspace for this op; 0 outside its two-launch path."""
+        x = self.x
+        nbytes = net.lib.odt_groupnorm_act_workspace_bytes(net.dt, x.B, x.H * x.W, x.C, self.groups)
+        return (nbytes + 7) // 8
 
     def launch(self, net, stream):
         x = self.x
@@ -691,8 +695,9 @@ class Net:
         self.head_buf = torch.zeros((self.batch, self.N, 25), dtype=torch.float32, device=dev)
         self.tail = tail
         tail.prepare(self)
-        # one fp64 arena for the (sum, sum^2) accumulators of every GroupNorm, zeroed once per forward
-        n_gn = sum(op.x.B * op.groups * 2 for op in self.ops if isinstance(op, GroupNormActOp))
+        # one fp64 arena for the workspaces of every GroupNorm (per-slice moments, statistics, arrival counters),
+        # zeroed once per forward
+        n_gn = sum(op.workspace_doubles(self) for op in self.ops if isinstance(op, GroupNormActOp))
         use_arena = n_gn > 0 and os.environ.get("ODT_GN_FUSED", "1") != "0"
         self.gn_arena = torch.zeros(n_gn, dtype=torch.float64, device=dev) if use_arena else None
         self._gn_used = 0

@@ -81,6 +81,7 @@ SYMBOLS = {
     "odt_upsample_nearest_concat": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     "odt_groupnorm_stats": (_I, [_P, _P, _I, _I, _L, _I, _I, _I, _F, _P]),
     "odt_groupnorm_apply": (_I, [_P, _P, _P, _I, _I, _L, _I, _I, _I, _P, _P, _I, _P]),
+    "odt_groupnorm_act_workspace_bytes": (_L, [_I, _I, _L, _I, _I]),
     "odt_groupnorm_act": (_I, [_P, _P, _P, _I, _I, _L, _I, _I, _I, _F, _P, _P, _I, _P]),
     "odt_decode_candidates": (_I, [_P, C.POINTER(TailParams), _I, _P, _P, _P]),
     "odt_nms_per_class": (_I, [_P, C.POINTER(TailParams), _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _L, _L, _P]),
