@@ -142,6 +142,10 @@ int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_conv_params
 /* the N tile (32 .. 128, or 256) odt_conv2d_f16_tc picks for an im2col-mode layer of M = B*OH*OW output
  * pixels, Cout_pad channels and kblocks = R*S*in_ld/64 K blocks (host only; honours ODT_TC_WIDE) */
 int odt_conv_tc_pick_bn(int cout_pad, long long M, int kblocks);
+/* whether odt_conv2d_f16_tc runs the layer on the transposed 64-cout x 256-pixel tiles (narrow 3x3 halo layers, fp16
+ * out0 alone; host only; honours ODT_TC_SWAP): 1 and *rp = rows per row-block tile (0: halo-flat), *tiles = 256-pixel
+ * tiles, *waste_permille = computed positions that are no output pixel, per thousand; else 0.  Outputs may be null. */
+int odt_conv_tc_swap_plan(const odt_conv_params* p, int* rp, long long* tiles, int* waste_permille);
 /* generic direct convolution on CUDA cores: any Cin/Cout/filter; `dtype` is
  * the activation dtype (ODT_F32: reference-precision path, ODT_F16: stems and
  * shapes the tensor-core kernel does not take).  Same call sites as above. */

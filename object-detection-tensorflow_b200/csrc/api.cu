@@ -50,6 +50,11 @@ int wide_mode() {
   const char* e = getenv("ODT_TC_WIDE");  // read every call: lets one process compare both tiles
   return (e && e[0] >= '0' && e[0] <= '2') ? e[0] - '0' : 1;
 }
+int swap_mode() {
+  // conv_tc_swap.cu (transposed tiles): 0 = off, 1 = where its planner takes the layer (default), 2 = wherever eligible
+  const char* e = getenv("ODT_TC_SWAP");  // read every call: lets one process compare both paths
+  return (e && e[0] >= '0' && e[0] <= '2') ? e[0] - '0' : 1;
+}
 bool wres_enabled() {
   const char* e = getenv("ODT_TC_WRES");
   return !(e && e[0] == '0');

@@ -96,6 +96,8 @@ int tapn_mode();       // ODT_TC_TAPN: 1 = narrow 3x3 halo layers go through con
                        // cost model predicts a gain, 2 = wherever the layer qualifies, 0 / unset = never
 int pw_mode();         // ODT_TC_PW: 1 = narrow 1x1 / stride-1 layers go through the staged pointwise kernel of conv_pw.cu
                        // (tried before conv_thin.cu), 2 = wherever the layer qualifies, 0 = never
+int swap_mode();       // ODT_TC_SWAP: 1 = narrow 3x3 halo layers (Cout_pad 64 / 128, fp16 out0 alone) run the transposed 64-cout x
+                       // 256-pixel tiles of conv_tc_swap.cu where its planner takes them, 2 = wherever eligible, 0 = never
 bool wres_enabled();  // ODT_TC_WRES=0 disables shared-memory-resident filter banks in the flat path
 
 }  // namespace odt

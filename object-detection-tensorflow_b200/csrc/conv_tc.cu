@@ -14,6 +14,8 @@
 //     tiled box with the row dimension second, the pooling window in four lanes of one warp.
 // * B operand (weights, KRSC = K-major): tiled TMA loads [BN x 64], optionally resident in shared
 //   memory for small filter banks.
+//   (Layers of these two modes with Cout_pad = 64 / 128, fp16 out0 alone and enough tiles go to conv_tc_swap.cu, which
+//   puts the pixels on the wgmma N side; this kernel keeps the small maps and every other epilogue.)
 // * MMA: wgmma m64nBNk16 (BN <= 128), both operands from shared memory.  Two consumer warpgroups
 //   in a ping-pong schedule: each owns whole 128-row tiles (two m64 accumulator sets, one per
 //   64-row half) and they take alternate tiles of the CTA's list.  An ordering barrier pair makes
@@ -684,6 +686,7 @@ int tc_rowblock_rp(int OH, int OW, long long* tiles) {
   return t4 < t2 ? 4 : 2;
 }
 
+int conv_swap_try(const void* in, const void* weights, const odt_conv_params* p, void* stream);  // conv_tc_swap.cu
 int conv_tapn_try(const void* in, const void* weights, const odt_conv_params* p, void* stream);  // conv_tapn.cu
 int conv_thin_try(const void* in, const void* weights, const odt_conv_params* p, void* stream);  // conv_thin.cu
 int conv_pw_try(const void* in, const void* weights, const odt_conv_params* p, void* stream);    // conv_pw.cu
@@ -788,6 +791,10 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
   }
   if (tapn_mode()) {  // opt-in: narrow 3x3 layers with the horizontal taps folded into N (conv_tapn.cu)
     const int rt = conv_tapn_try(in, weights, p, stream);
+    if (rt != ODT_ERR_UNSUPPORTED) return rt;
+  }
+  {  // narrow 3x3 halo layers with enough tiles: pixels on the wgmma N side (conv_tc_swap.cu; ODT_TC_SWAP)
+    const int rt = conv_swap_try(in, weights, p, stream);
     if (rt != ODT_ERR_UNSUPPORTED) return rt;
   }
   TcGeom g;

@@ -101,6 +101,13 @@ __device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t
                "r"(r2), "r"(r3)
                : "memory");
 }
+// the transposed store: register k holds this lane's pair (column l/4, rows 2*(l%4) + {0,1}) of matrix k, so a
+// [channel][pixel] accumulator fragment lands as [pixel][channel] rows (lane l still addresses row l%8 of matrix l/8)
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0),
+               "r"(r1), "r"(r2), "r"(r3)
+               : "memory");
+}
 __device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
   asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }

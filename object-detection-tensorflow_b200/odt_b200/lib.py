@@ -69,6 +69,7 @@ SYMBOLS = {
     "odt_normalize_input": (_I, [_P, _P, _I, _I, _I, _I, _I, C.POINTER(_F), _P]),
     "odt_conv2d_f16_tc": (_I, [_P, _P, C.POINTER(ConvParams), _P]),
     "odt_conv_tc_pick_bn": (_I, [_I, _L, _I]),
+    "odt_conv_tc_swap_plan": (_I, [C.POINTER(ConvParams), C.POINTER(_I), C.POINTER(_L), C.POINTER(_I)]),
     "odt_conv2d_direct": (_I, [_P, _P, _I, C.POINTER(ConvParams), _P]),
     "odt_conv2d_stem": (_I, [_P, C.POINTER(_F), _P, _I, C.POINTER(ConvParams), _P]),
     "odt_pack_input_rgbx": (_I, [_P, _P, _I, _I, _I, _I, C.POINTER(_F), _P]),

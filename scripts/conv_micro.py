@@ -67,6 +67,7 @@ def setup(a):
         L.check(lib.odt_conv2d_f16_tc(x.data_ptr(), w.data_ptr(), C.byref(p), st), "conv")
 
     launch.keep = (x, w, y, shift, keep)
+    launch.swap = bool(lib.odt_conv_tc_swap_plan(C.byref(p), None, None, None))  # conv_tc_swap.cu takes it (ODT_TC_SWAP)
     return lib, launch, 2.0 * B * OH * OW * Cout * k * k * Cin, reps
 
 
@@ -87,8 +88,9 @@ def main():
     e1.record()
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / reps
-    print("conv %s pool=%d halo=%d/%d extra=%r thin/tapn launches %d/%d: %.4f ms  %.1f TFLOP/s" % (
-        a[:7], pool, ih, oh, extra, lib.odt_debug_thin_launches(), lib.odt_debug_tapn_launches(), ms, fl / ms / 1e9))
+    print("conv %s pool=%d halo=%d/%d extra=%r thin/tapn launches %d/%d, transposed tiles %s: %.4f ms  %.1f TFLOP/s" % (
+        a[:7], pool, ih, oh, extra, lib.odt_debug_thin_launches(), lib.odt_debug_tapn_launches(),
+        "yes" if launch.swap else "no", ms, fl / ms / 1e9))
 
 
 if __name__ == "__main__":

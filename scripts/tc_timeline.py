@@ -5,6 +5,7 @@ of the mainloops, and the share of the kernel during which no warpgroup has MMAs
   --probe=feed  consumers wait for each stage and release it without MMAs: the rate the TMA feed alone sustains
   --probe=mma   the producer loads nothing and consumers do not wait: the rate of the MMAs alone (im2col mode)
 Both probes compute wrong results by design.  ODT_TC_WIDE=0 / 2 pins the 128-wide / 256-wide tile of im2col layers.
+conv_tc_swap.cu's kernel carries no stamps: a layer its planner takes is timed here with ODT_TC_SWAP=0 (forced below).
 usage (on a GPU box): tc_timeline.py [--probe=feed|mma] B H W Cin Cout k stride [pool] [in_halo] [out_halo]
 (conv_micro.py's arguments)"""
 import os
@@ -59,6 +60,7 @@ def main():
     probe = None
     if argv and argv[0].startswith("--probe="):
         probe = argv.pop(0).split("=", 1)[1]
+    os.environ["ODT_TC_SWAP"] = "0"
     L.LIB_PATH = build_debug_lib(probe)
     L._lib = None  # __graft_entry__.build() has loaded the product library: bind the debug build instead
     import conv_micro
