@@ -239,9 +239,10 @@ typedef struct {
   int kind;       /* ODT_DECODE_*                                              */
   int num_levels;
   int N;          /* candidates (rows) per image                               */
-  int num_fg;     /* classes thresholded (SSD/RetinaNet: 20 of 21; YOLO 20;
-                     FCOS 20)                                                  */
-  int nms_classes;/* classes the NMS loop visits (FCOS: 19, ref FCOS.py:252)   */
+  int num_fg;     /* classes thresholded (SSD/RetinaNet: 20 of 21; YOLOv3 /
+                     FCOS: 1..128); a candidate row is num_fg + 5 floats       */
+  int nms_classes;/* classes the NMS loop visits, 0..num_fg (FCOS: num_fg - 1,
+                     ref FCOS.py:252)                                          */
   float score_thr, iou_thr;
   int max_boxes;
   int cap;        /* candidate capacity per (image, class)                     */
@@ -249,7 +250,7 @@ typedef struct {
 } odt_tail_params;
 
 /* fused: score activation + anchor/prior generation + threshold + candidate
- * compaction.  head: fp32 [B,N,25] rows (layout per kind, see DESIGN.md).
+ * compaction.  head: fp32 [B,N,num_fg+5] rows (layout per kind, see DESIGN.md).
  * cand_keys: u64 [B,num_fg,cap]; cand_count: i32 [B,num_fg] (zeroed here).
  * ref: SSD300.py:157-172,323-343; RetinaNet.py:224-239,328-355;
  *      YOLOv3.py:320-351,419-433; FCOS.py:130-150,197-248 */
@@ -264,7 +265,8 @@ int odt_decode_candidates(const float* head, const odt_tail_params* p, int B,
  * rows receive (float) det_count and its overflow flag (0 / 1): `dets` is then the packed
  * fixed-size record [B, D*6+2] that one all-gather / one device->host copy ships.  work: i32 [round_up(B,2) + 2] zero-initialised, 8-byte aligned scratch
  * (per-image completion counters reset by the kernel, then the 64-bit bump pointer
- * of the box pool).  box_pool: optional f32 [box_pool_entries][4]
+ * of the box pool).  nms_classes = 0: no list is visited, only the counts / flags are written.
+ * box_pool: optional f32 [box_pool_entries][4]
  * scratch where lists longer than the 1024-entry shared-memory window cache their
  * decoded boxes when they take the full-list path (the prefilter subset ran dry, or more
  * than 1024 scores tie at the top); NULL / exhausted -> boxes are re-decoded every round.
@@ -278,7 +280,8 @@ int odt_nms_per_class(const float* head, const odt_tail_params* p, int B,
 long long odt_nms_scratch_bytes(const odt_tail_params* p, int B);
 
 /* Training-loss forwards, one per family.  All four share one calling convention:
- *   head: the [B,N,25] candidate rows the inference tail reads; gt: f32 [B,G,5] rows (y,x,h,w,id)
+ *   head: the [B,N,num_fg+5] candidate rows the inference tail reads (SSD / RetinaNet: num_fg = 20;
+ *   YOLOv3 / FCOS: 1..128); gt: f32 [B,G,5] rows (y,x,h,w,id)
  *   padded with -1 (G <= 128); loss_out: f32 [B] per-image loss (the reference averages them over the
  *   batch and adds weight decay on the host side of the graph);
  *   scratch: odt_<family>_loss_scratch_bytes(p, B) bytes, 8-byte aligned, owned by the call until it

@@ -216,7 +216,8 @@ __global__ void __launch_bounds__(kLossThreads)
     s_best[g] = best[b * G + g];
   }
   __syncthreads();
-  const float* hb = head + (long long)b * p.N * kRow;
+  const int row = row_floats(p.num_fg);
+  const float* hb = head + (long long)b * p.N * row;
   float conf = 0.f, coord = 0.f, npos = 0.f;
   auto positive = [&](const float* r, const Anchor& a, int g, float cls) {  // row r, anchor a matched to GT g
     conf += cls;
@@ -246,7 +247,7 @@ __global__ void __launch_bounds__(kLossThreads)
         }
         const bool pos = bv > 0.5f, neg = kSsd || bv < 0.4f;  // RetinaNet ignores best IoUs in [0.4, 0.5]
         if (pos || neg) {
-          const float* r = hb + (long long)n * kRow;
+          const float* r = hb + (long long)n * row;
           const float cls = class_loss<kSsd>(r, pos ? (int)gb[bg * 5 + 4] : 20, alpha, gamma);
           if (pos) {
             positive(r, a, bg, cls);
@@ -278,7 +279,7 @@ __global__ void __launch_bounds__(kLossThreads)
     for (int g = threadIdx.x; g < cnt; g += blockDim.x) {
       int n = s_best[g];
       Cell c = locate(p, n);
-      const float* r = hb + (long long)n * kRow;
+      const float* r = hb + (long long)n * row;
       positive(r, anchor_ssd(p, c), g, class_loss<kSsd>(r, (int)gb[g * 5 + 4], alpha, gamma));
     }
   }
@@ -407,12 +408,17 @@ __device__ __forceinline__ float softplus_f(float x) {  // log(1 + exp(x)), stab
   return fmaxf(x, 0.f) + log1pf(expf(-fabsf(x)));
 }
 
+// NFG = 20: the 25-float rows, class loop fixed at compile time; NFG = 0: num_fg (1..kMaxFg) from the parameters,
+// the per-location class mask in kMaskWords words.
+template <int NFG>
 __global__ void __launch_bounds__(kLossThreads)
     fcos_loss_kernel(const float* __restrict__ head, const __grid_constant__ TailP tp,
                      const float* __restrict__ gt, int G, float* __restrict__ partial,
                      int* __restrict__ level_cnt) {
+  constexpr int W = NFG ? (NFG + 31) / 32 : kMaskWords;  // class-mask words
   pdl_launch_dependents();
   const odt_tail_params& p = tp.p;
+  const int nfg = NFG ? NFG : p.num_fg, row = row_floats(nfg);
   const int b = blockIdx.y, blk = blockIdx.x;
   const float* gb = gt + (long long)b * G * 5;
   __shared__ float s_box[kMaxGT][kFcosLevels][4];  // y1,x1,y2,x2 in stride units of each level
@@ -447,7 +453,7 @@ __global__ void __launch_bounds__(kLossThreads)
     for (int g = 0; g < cnt; ++g) c += (s_lv[g] >> threadIdx.x) & 1;
     level_cnt[b * kFcosLevels + threadIdx.x] = c;
   }
-  const float* hb = head + (long long)b * p.N * kRow;
+  const float* hb = head + (long long)b * p.N * row;
   float acc[kFcosLevels][4];  // iou, focal, centre, #positive class cells
 #pragma unroll
   for (int l = 0; l < kFcosLevels; ++l)
@@ -461,14 +467,22 @@ __global__ void __launch_bounds__(kLossThreads)
     const float yy = (float)c.y, xx = (float)c.x;
     bool loc = false;
     float amin = 3.0e38f, dl = 0.f, dr = 0.f, dt = 0.f, db = 0.f;
-    unsigned cmask = 0u;
+    unsigned cmask[W];
+#pragma unroll
+    for (int w = 0; w < W; ++w) cmask[w] = 0u;
     for (int g = 0; g < cnt; ++g) {
       if (!((s_lv[g] >> l) & 1)) continue;
       const float l_ = __fsub_rn(xx, s_box[g][l][1]), r_ = __fsub_rn(s_box[g][l][3], xx);
       const float t_ = __fsub_rn(yy, s_box[g][l][0]), b_ = __fsub_rn(s_box[g][l][2], yy);
       if (!(l_ > 0.f && r_ > 0.f && t_ > 0.f && b_ > 0.f)) continue;
       loc = true;
-      cmask |= 1u << s_cls[g];
+      if (W == 1) {
+        cmask[0] |= 1u << s_cls[g];
+      } else {
+#pragma unroll
+        for (int w = 0; w < W; ++w)
+          if (s_cls[g] >> 5 == w) cmask[w] |= 1u << (s_cls[g] & 31);
+      }
       const float area = __fmul_rn(__fadd_rn(l_, r_), __fadd_rn(t_, b_));
       if (area < amin) {
         amin = area;
@@ -477,15 +491,15 @@ __global__ void __launch_bounds__(kLossThreads)
         dl = fmaxf(dl, l_); dr = fmaxf(dr, r_); dt = fmaxf(dt, t_); db = fmaxf(db, b_);
       }
     }
-    const float* r = hb + (long long)n * kRow;
+    const float* r = hb + (long long)n * row;
     // centre-ness BCE with logits, every location (:331-334); target 0 where no GT covers the cell
     const float lrmin = fminf(dl, dr), tbmin = fminf(dt, db), lrmax = fmaxf(dl, dr), tbmax = fmaxf(dt, db);
     const float cgt = __fsqrt_rn(__fdiv_rn(__fmul_rn(lrmin, tbmin), __fadd_rn(__fmul_rn(lrmax, tbmax), 1e-12f)));
-    const float cx = r[20];
+    const float cx = r[nfg];
     float centre = fmaxf(cx, 0.f) - cx * cgt + log1pf(expf(-fabsf(cx)));
     float iou_l = 0.f;
     if (loc) {
-      const float pl = expf(r[21]), pr = expf(r[22]), pt = expf(r[23]), pb = expf(r[24]);
+      const float pl = expf(r[nfg + 1]), pr = expf(r[nfg + 2]), pt = expf(r[nfg + 3]), pb = expf(r[nfg + 4]);
       const float iw = __fadd_rn(fminf(dl, pl), fminf(dr, pr)), ih = __fadd_rn(fminf(dt, pt), fminf(db, pb));
       const float inter = __fmul_rn(iw, ih);
       const float uni = __fsub_rn(__fadd_rn(__fmul_rn(__fadd_rn(dl, dr), __fadd_rn(dt, db)),
@@ -494,17 +508,21 @@ __global__ void __launch_bounds__(kLossThreads)
       iou_l = -logf(__fadd_rn(iou, 1e-12f));
     }
     float focal_l = 0.f, npos = 0.f;
+#pragma unroll
+    for (int w = 0; w < W; ++w) {
+      const int kend = NFG ? (NFG - 32 * w < 32 ? NFG - 32 * w : 32) : min(32, nfg - 32 * w);
 #pragma unroll 4
-    for (int k = 0; k < 20; ++k) {
-      const float x = r[k];
-      const float ls = -softplus_f(-x);                 // log sigmoid(x)
-      const float sg = __fdiv_rn(1.f, __fadd_rn(1.f, expf(-x)));
-      if ((cmask >> k) & 1u) {
-        const float om = 1.f - sg;
-        focal_l += -0.25f * om * om * ls;
-        npos += 1.f;
-      } else {
-        focal_l += -0.25f * sg * sg * (-x + ls);
+      for (int k = 0; k < kend; ++k) {
+        const float x = r[32 * w + k];
+        const float ls = -softplus_f(-x);                 // log sigmoid(x)
+        const float sg = __fdiv_rn(1.f, __fadd_rn(1.f, expf(-x)));
+        if ((cmask[w] >> k) & 1u) {
+          const float om = 1.f - sg;
+          focal_l += -0.25f * om * om * ls;
+          npos += 1.f;
+        } else {
+          focal_l += -0.25f * sg * sg * (-x + ls);
+        }
       }
     }
 #pragma unroll
@@ -577,13 +595,16 @@ __device__ __forceinline__ YoloGt yolo_gt(const float* gb, int g, int k) {
   return n;
 }
 
-// K1: one block per image, one thread per GT: level / prior assignment, positive terms, cell occupancy
+// K1: one block per image, one thread per GT: level / prior assignment, positive terms, cell occupancy.
+// NFG = 20: the 25-float rows, class loop fixed at compile time; NFG = 0: num_fg from the parameters.
+template <int NFG>
 __global__ void __launch_bounds__(kMaxGT)
     yolo_loss_pos_kernel(const float* __restrict__ head, const __grid_constant__ TailP tp,
                          const float* __restrict__ gt, int G, unsigned char* __restrict__ occ,
                          float* __restrict__ pos_out) {
   pdl_launch_dependents();
   const odt_tail_params& p = tp.p;
+  const int nfg = NFG ? NFG : p.num_fg, row = row_floats(nfg);
   const int b = blockIdx.x, g = threadIdx.x;
   const float* gb = gt + (long long)b * G * 5;
   __shared__ float s_red[3][kMaxGT];
@@ -620,15 +641,16 @@ __global__ void __launch_bounds__(kMaxGT)
     else if (mx[1] > mx[0] && mx[1] > mx[2]) k = 1;
     const odt_level& L = p.level[k];
     const YoloGt n = yolo_gt(gb, g, k);
-    const float* r = head + ((long long)b * p.N + L.offset + (long long)(cy[k] * L.W + cx[k]) * 3 + arg[k]) * kRow;
+    const float* r = head + ((long long)b * p.N + L.offset + (long long)(cy[k] * L.W + cx[k]) * 3 + arg[k]) * row;
     const float ty = __fsub_rn(n.y, floorf(n.y)), tx = __fsub_rn(n.x, floorf(n.x));
     const float th = logf(__fdiv_rn(n.h, L.prior_h[arg[k]])), tw = logf(__fdiv_rn(n.w, L.prior_w[arg[k]]));
-    coord = sig_xent(ty, r[20]) + sig_xent(tx, r[21]);
-    const float dh = __fsub_rn(r[22], th), dw = __fsub_rn(r[23], tw);
+    const float* t = r + nfg;  // y, x, h, w, obj behind the class scores
+    coord = sig_xent(ty, t[0]) + sig_xent(tx, t[1]);
+    const float dh = __fsub_rn(t[2], th), dw = __fsub_rn(t[3], tw);
     coord += 0.5f * (dh * dh + dw * dw);
     const int label = (int)gb[g * 5 + 4];
-    for (int c = 0; c < 20; ++c) cls += sig_xent(c == label ? 1.f : 0.f, r[c]);
-    obj = sig_xent(1.f, r[24]);
+    for (int c = 0; c < nfg; ++c) cls += sig_xent(c == label ? 1.f : 0.f, r[c]);
+    obj = sig_xent(1.f, t[4]);
   }
   block_sum(s_red, {coord, cls, obj});
   if (threadIdx.x < 3) pos_out[b * 4 + threadIdx.x] = s_red[threadIdx.x][0];
@@ -659,7 +681,8 @@ __global__ void __launch_bounds__(kLossThreads)
   }
   __syncthreads();
   const long long cells = p.N / 3;
-  const float* hb = head + (long long)b * p.N * kRow;
+  const int row = row_floats(p.num_fg);
+  const float* hb = head + (long long)b * p.N * row;
   float acc = 0.f;
   const int per = (p.N + kLossBlocks - 1) / kLossBlocks;
   const int n_begin = blk * per, n_end = min(p.N, n_begin + per);
@@ -678,7 +701,7 @@ __global__ void __launch_bounds__(kLossThreads)
     for (int g = 0; g < cnt; ++g)
       best = fmaxf(best, iou_unclamped(s_g[g][c.lvl][0], s_g[g][c.lvl][1], s_g[g][c.lvl][2], s_g[g][c.lvl][3], by1,
                                        bx1, by2, bx2, aarea));
-    if (best <= 0.5f) acc += sig_xent(0.f, hb[(long long)n * kRow + 24]);
+    if (best <= 0.5f) acc += sig_xent(0.f, hb[(long long)n * row + p.num_fg + 4]);  // objectness
   }
   block_sum(s_red, {acc});
   if (threadIdx.x == 0) partial[(long long)b * kLossBlocks + blk] = s_red[0][0];
@@ -782,7 +805,7 @@ extern "C" long long odt_yolo_loss_scratch_bytes(const odt_tail_params* p, int B
 extern "C" int odt_retina_loss_fwd(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
                                    float alpha, float gamma, void* scratch, float* loss_out, void* stream) {
   ODT_CHECK_ARG(head && p && gt && scratch && loss_out, "null pointer");
-  ODT_CHECK_ARG(p->kind == ODT_DECODE_SSD, "softmax-family head expected");
+  ODT_CHECK_ARG(p->kind == ODT_DECODE_SSD && p->num_fg == 20, "softmax-family head with 20 classes expected");
   ODT_CHECK_ARG(B > 0 && G > 0 && G <= kMaxGT, "B/G (G <= 128)");
   ODT_CHECK_ARG(((uintptr_t)scratch & 7) == 0, "scratch must be 8-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
@@ -802,7 +825,7 @@ extern "C" int odt_retina_loss_fwd(const float* head, const odt_tail_params* p, 
 extern "C" int odt_ssd_loss_fwd(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
                                 void* scratch, float* loss_out, int* info_out, void* stream) {
   ODT_CHECK_ARG(head && p && gt && scratch && loss_out, "null pointer");
-  ODT_CHECK_ARG(p->kind == ODT_DECODE_SSD, "softmax-family head expected");
+  ODT_CHECK_ARG(p->kind == ODT_DECODE_SSD && p->num_fg == 20, "softmax-family head with 20 classes expected");
   ODT_CHECK_ARG(B > 0 && G > 0 && G <= kMaxGT, "B/G (G <= 128)");
   ODT_CHECK_ARG(((uintptr_t)scratch & 7) == 0, "scratch must be 8-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
@@ -823,15 +846,18 @@ extern "C" int odt_ssd_loss_fwd(const float* head, const odt_tail_params* p, int
 extern "C" int odt_fcos_loss_fwd(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
                                  void* scratch, float* loss_out, void* stream) {
   ODT_CHECK_ARG(head && p && gt && scratch && loss_out, "null pointer");
-  ODT_CHECK_ARG(p->kind == ODT_DECODE_FCOS && p->num_levels == kFcosLevels && p->num_fg == 20,
-                "FCOS head with 5 levels and 20 classes expected");
+  ODT_CHECK_ARG(p->kind == ODT_DECODE_FCOS && p->num_levels == kFcosLevels && p->num_fg >= 1 && p->num_fg <= kMaxFg,
+                "FCOS head with 5 levels and 1..128 classes expected");
   ODT_CHECK_ARG(B > 0 && G > 0 && G <= kMaxGT, "B/G (G <= 128)");
   ODT_CHECK_ARG(((uintptr_t)scratch & 7) == 0, "scratch must be 8-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
   const FcosScratch s = fcos_scratch(*p, B, scratch);
   TailP tp;
   tp.p = *p;
-  fcos_loss_kernel<<<dim3(kLossBlocks, B), kLossThreads, 0, st>>>(head, tp, gt, G, s.partial, s.level_cnt);
+  if (p->num_fg == 20)
+    fcos_loss_kernel<20><<<dim3(kLossBlocks, B), kLossThreads, 0, st>>>(head, tp, gt, G, s.partial, s.level_cnt);
+  else
+    fcos_loss_kernel<0><<<dim3(kLossBlocks, B), kLossThreads, 0, st>>>(head, tp, gt, G, s.partial, s.level_cnt);
   ODT_LAUNCH_OK();
   fcos_loss_final_kernel<<<(B + 63) / 64, 64, 0, st>>>(s.partial, s.level_cnt, B, loss_out);
   ODT_LAUNCH_OK();
@@ -842,8 +868,8 @@ extern "C" int odt_yolo_loss_fwd(const float* head, const odt_tail_params* p, in
                                  float coord_scale, float noobj_scale, float obj_scale, float class_scale,
                                  void* scratch, float* loss_out, void* stream) {
   ODT_CHECK_ARG(head && p && gt && scratch && loss_out, "null pointer");
-  ODT_CHECK_ARG(p->kind == ODT_DECODE_YOLO3 && p->num_levels == kYoloLevels && p->num_fg == 20,
-                "YOLOv3 head with 3 levels and 20 classes expected");
+  ODT_CHECK_ARG(p->kind == ODT_DECODE_YOLO3 && p->num_levels == kYoloLevels && p->num_fg >= 1 && p->num_fg <= kMaxFg,
+                "YOLOv3 head with 3 levels and 1..128 classes expected");
   for (int i = 0; i < kYoloLevels; ++i) ODT_CHECK_ARG(p->level[i].A == 3, "3 priors per level expected");
   ODT_CHECK_ARG(B > 0 && G > 0 && G <= kMaxGT, "B/G (G <= 128)");
   ODT_CHECK_ARG(((uintptr_t)scratch & 7) == 0, "scratch must be 8-byte aligned");
@@ -852,7 +878,10 @@ extern "C" int odt_yolo_loss_fwd(const float* head, const odt_tail_params* p, in
   ODT_CUDA_OK(cudaMemsetAsync(s.occ, 0, (size_t)B * (p->N / 3), st));
   TailP tp;
   tp.p = *p;
-  yolo_loss_pos_kernel<<<B, kMaxGT, 0, st>>>(head, tp, gt, G, s.occ, s.pos);
+  if (p->num_fg == 20)
+    yolo_loss_pos_kernel<20><<<B, kMaxGT, 0, st>>>(head, tp, gt, G, s.occ, s.pos);
+  else
+    yolo_loss_pos_kernel<0><<<B, kMaxGT, 0, st>>>(head, tp, gt, G, s.occ, s.pos);
   ODT_LAUNCH_OK();
   yolo_loss_noobj_kernel<<<dim3(kLossBlocks, B), kLossThreads, 0, st>>>(head, tp, gt, G, s.occ, s.partial);
   ODT_LAUNCH_OK();

@@ -17,14 +17,16 @@
 
 namespace odt {
 
+// Two families of instantiations.  NFG = 20: the 25-float rows of every model at the VOC class count, 8 warps per
+// CTA, row width and class loop fixed at compile time.  NFG = 0 ("wide"): YOLOv3 / FCOS with any num_fg in
+// 1..kMaxFg, row width read from the parameters, 4 warps per CTA (32 rows x 133 floats = 17 KB per warp stage at
+// num_fg = 128: 8 warps x 2 stages would need 272 KB).  Shared memory: [WARPS][STAGES][32 * row] floats, then the
+// [WARPS][STAGES] mbarriers; the dynamic size is sized by the actual row width.
 constexpr int kDecodeWarps = 8;
-constexpr int kGroupFloats = 32 * kRow;          // one warp iteration = 32 candidate rows = 3200 contiguous bytes
-constexpr int kGroupBytes = kGroupFloats * 4;
-template <int STAGES>
-struct DecodeSmem {
-  float rows[kDecodeWarps][STAGES][kGroupFloats];  // 25 600 B per stage
-  unsigned long long bar[kDecodeWarps][STAGES];
-};
+constexpr int kDecodeWarpsWide = 4;
+__host__ __device__ constexpr long long decode_smem_bytes(int warps, int stages, int row) {
+  return (long long)warps * stages * 32 * row * 4 + (long long)warps * stages * 8;
+}
 
 __device__ __forceinline__ void bulk_load_1d(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
@@ -32,23 +34,31 @@ __device__ __forceinline__ void bulk_load_1d(uint32_t dst, const void* src, uint
                : "memory");
 }
 
-// One warp = 32 consecutive candidate rows per iteration.  The 3200-byte group is fetched by ONE bulk copy (TMA,
-// cp.async.bulk) into a per-warp double buffer and signalled on an mbarrier, so no thread holds load registers or
-// issues load instructions while it computes (round 1 kept 7 float4 per lane in flight: 80 registers, 3 CTAs / SM,
-// 826 warp instructions per group; this kernel: KIND at compile time, no 64-bit divisions, the row's scores stay in
-// registers only).  Then one lane per row: score activation, background filter, threshold, per-class ballots and ONE
-// atomic per (warp, class) to reserve the candidate slots.
-template <int KIND, int OCC, int STAGES>
-__global__ void __launch_bounds__(kDecodeWarps * 32, OCC)
+// One warp = 32 consecutive candidate rows per iteration.  The group (32 rows, 3200 bytes at num_fg = 20) is fetched
+// by ONE bulk copy (TMA, cp.async.bulk) into a per-warp double buffer and signalled on an mbarrier, so no thread holds
+// load registers or issues load instructions while it computes (round 1 kept 7 float4 per lane in flight: 80
+// registers, 3 CTAs / SM, 826 warp instructions per group; this kernel: KIND at compile time, no 64-bit divisions,
+// the row's scores stay in registers only).  Then one lane per row: score activation, background filter, threshold,
+// per-class ballots and ONE atomic per (warp, class) to reserve the candidate slots.  Classes come in words of 32:
+// pass[w] bit i = class 32 w + i of this row passes, and the ballot / reservation loop runs word by word.
+template <int KIND, int WARPS, int OCC, int STAGES, int NFG>
+__global__ void __launch_bounds__(WARPS * 32, OCC)
     decode_candidates_kernel(const float* __restrict__ head, const __grid_constant__ TailP tp,
                              long long total_rows, unsigned long long* __restrict__ cand_keys,
                              int* __restrict__ cand_count) {
+  static_assert(NFG == 0 ? KIND != ODT_DECODE_SSD : NFG == 20, "instantiations: NFG = 20, or 0 for YOLOv3 / FCOS");
+  constexpr int W = NFG ? (NFG + 31) / 32 : kMaskWords;  // pass-mask words per row
   pdl_launch_dependents();
   const odt_tail_params& p = tp.p;
+  const int nfg = NFG ? NFG : p.num_fg;
+  const int row = row_floats(nfg);
+  const int group_floats = 32 * row;
+  const uint32_t group_bytes = (uint32_t)group_floats * 4u;
   extern __shared__ __align__(128) unsigned char dsm_raw[];
-  DecodeSmem<STAGES>& sm = *reinterpret_cast<DecodeSmem<STAGES>*>(dsm_raw);
+  float* rows_sm = reinterpret_cast<float*>(dsm_raw);
+  unsigned long long* bars = reinterpret_cast<unsigned long long*>(dsm_raw + (size_t)WARPS * STAGES * group_bytes);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t bar0 = smem_u32(&sm.bar[warp][0]);
+  const uint32_t bar0 = smem_u32(&bars[warp * STAGES]);
   if (lane == 0) {
 #pragma unroll
     for (int s = 0; s < STAGES; ++s) mbar_init(bar0 + 8u * s, 1);
@@ -57,16 +67,17 @@ __global__ void __launch_bounds__(kDecodeWarps * 32, OCC)
   __syncwarp();
   const long long groups = (total_rows + 31) / 32;
   const long long full_groups = total_rows / 32;  // groups below this index are whole (bulk-copy eligible)
-  const int step = (int)gridDim.x * kDecodeWarps;  // groups between two iterations of one warp
-  long long g = (long long)blockIdx.x * kDecodeWarps + warp;
+  const int step = (int)gridDim.x * WARPS;        // groups between two iterations of one warp
+  long long g = (long long)blockIdx.x * WARPS + warp;
   // (image, row) of the group's first row, advanced incrementally: no 64-bit division in the loop
   const int N = p.N;
   int b = (int)((g * 32) / N), n = (int)((g * 32) % N);
   const int adv_b = (int)(((long long)step * 32) / N), adv_n = (int)(((long long)step * 32) % N);
   auto issue = [&](long long gg, int slot) {  // lane 0 only
     if (gg < full_groups) {
-      mbar_expect_tx(bar0 + 8u * slot, kGroupBytes);
-      bulk_load_1d(smem_u32(&sm.rows[warp][slot][0]), head + gg * kGroupFloats, kGroupBytes, bar0 + 8u * slot);
+      mbar_expect_tx(bar0 + 8u * slot, group_bytes);
+      bulk_load_1d(smem_u32(rows_sm + (size_t)(warp * STAGES + slot) * group_floats), head + gg * group_floats,
+                   group_bytes, bar0 + 8u * slot);
     }
   };
   // STAGES - 1 groups in flight ahead of the one being decoded
@@ -79,7 +90,7 @@ __global__ void __launch_bounds__(kDecodeWarps * 32, OCC)
   int slot = 0;
   for (; g < groups; g += step) {
     const int nrows = (int)min((long long)32, total_rows - g * 32);
-    float* my = &sm.rows[warp][slot][0];
+    float* my = rows_sm + (size_t)(warp * STAGES + slot) * group_floats;
     {
       // refill the stage that was drained in the previous iteration (its readers passed the __syncwarp below)
       const long long gn = g + (long long)(STAGES - 1) * step;
@@ -90,8 +101,8 @@ __global__ void __launch_bounds__(kDecodeWarps * 32, OCC)
       mbar_wait(bar0 + 8u * slot, (phase >> slot) & 1u);
       phase ^= 1u << slot;
     } else {  // ragged last group: plain loads
-      const float* src = head + g * kGroupFloats;
-      for (int i = lane; i < nrows * kRow; i += 32) my[i] = __ldg(src + i);
+      const float* src = head + g * group_floats;
+      for (int i = lane; i < nrows * row; i += 32) my[i] = __ldg(src + i);
       __syncwarp();
     }
     const bool active = lane < nrows;
@@ -101,11 +112,12 @@ __global__ void __launch_bounds__(kDecodeWarps * 32, OCC)
       ++lb;
     }
     const bool one_image = (n + nrows <= N);  // warp-uniform
-    const float* r = my + lane * kRow;
-    // pass_bits: bit c = class c of this row passes the score threshold.  The scores themselves are NOT kept in
-    // registers across the ballot section: score(c) recomputes the (few) passing ones from the staged row and
-    // two saved scalars, bit-identically.
-    unsigned pass_bits = 0u;
+    const float* r = my + lane * row;
+    // pass bits: the scores themselves are NOT kept in registers across the ballot section: score(c) recomputes the
+    // (few) passing ones from the staged row and two saved scalars, bit-identically.
+    unsigned pass[W];
+#pragma unroll
+    for (int w = 0; w < W; ++w) pass[w] = 0u;
     float k0 = 0.f, k1 = 0.f;  // SSD: (max logit, 1/sum); YOLO / FCOS: (sigmoid(obj | ctr), unused)
     if (KIND == ODT_DECODE_SSD) {
       // softmax over 21 logits, TF form exp(x-max) * (1/sum); rows whose arg-max (first maximum) is the
@@ -125,33 +137,49 @@ __global__ void __launch_bounds__(kDecodeWarps * 32, OCC)
       }
       const float inv = __frcp_rn(s);
       float best_fg = -1.f;
+      unsigned bits = 0u;
 #pragma unroll
       for (int i = 0; i < 20; ++i) {
         const float pi = __fmul_rn(e[i], inv);
         best_fg = fmaxf(best_fg, pi);
-        pass_bits |= (pi >= p.score_thr) ? (1u << i) : 0u;
+        bits |= (pi >= p.score_thr) ? (1u << i) : 0u;
       }
-      if (!active || __fmul_rn(e[20], inv) > best_fg) pass_bits = 0u;
+      if (!active || __fmul_rn(e[20], inv) > best_fg) bits = 0u;
+      pass[0] = bits;
       k0 = m;
       k1 = inv;
     } else {
-      k0 = sigmoid_score(r[KIND == ODT_DECODE_YOLO3 ? 24 : 20]);  // ref YOLOv3.py:338-339,349; FCOS.py:197-201
+      // ref YOLOv3.py:338-339,349; FCOS.py:197-201: objectness / centre-ness behind the class scores
+      k0 = sigmoid_score(r[KIND == ODT_DECODE_YOLO3 ? nfg + 4 : nfg]);
+      // sigmoid_score <= 1 and rounding is monotone, so __fmul_rn(sigmoid_score(x), k0) <= k0: when k0 is below the
+      // threshold no class of the row can pass (exact).  Most YOLO rows have a low objectness.
+      if (active && (NFG || !(k0 < p.score_thr))) {
 #pragma unroll
-      for (int i = 0; i < 20; ++i)
-        pass_bits |= (__fmul_rn(sigmoid_score(r[i]), k0) >= p.score_thr) ? (1u << i) : 0u;
-      if (!active) pass_bits = 0u;
+        for (int w = 0; w < W; ++w) {
+          const int cend = NFG ? (NFG - 32 * w < 32 ? NFG - 32 * w : 32) : min(32, nfg - 32 * w);
+          unsigned bits = 0u;
+#pragma unroll(NFG ? 32 : 4)
+          for (int i = 0; i < cend; ++i)
+            bits |= (__fmul_rn(sigmoid_score(r[32 * w + i]), k0) >= p.score_thr) ? (1u << i) : 0u;
+          pass[w] = bits;
+        }
+      }
     }
-    if (p.num_fg < 20) pass_bits &= (1u << p.num_fg) - 1u;
     auto score = [&](int c) -> float {
       if (KIND == ODT_DECODE_SSD) return __fmul_rn(exp_score(__fsub_rn(r[c], k0)), k1);
       return __fmul_rn(sigmoid_score(r[c]), k0);
     };
-    // classes with at least one candidate in this warp: the work below is proportional to their number
-    const unsigned any = __reduce_or_sync(0xffffffffu, pass_bits);
-    if (any != 0u) {
+#pragma unroll
+    for (int w = 0; w < W; ++w) {
+      if (32 * w >= nfg) break;  // warp-uniform
+      const unsigned pass_bits = pass[w];
+      const int cbase = 32 * w;
+      // classes with at least one candidate in this warp: the work below is proportional to their number
+      const unsigned any = __reduce_or_sync(0xffffffffu, pass_bits);
+      if (any == 0u) continue;
       if (one_image) {
-        // lane c collects the ballot of class c, then reserves the slots of its class with ONE atomic: up to 20
-        // independent atomics in flight instead of dependent round trips
+        // lane i collects the ballot of class cbase + i, then reserves the slots of its class with ONE atomic: up to
+        // 32 independent atomics in flight instead of dependent round trips
         unsigned my_mask = 0u;
         for (unsigned rem = any; rem; rem &= rem - 1u) {
           const int c = __ffs(rem) - 1;  // warp-uniform
@@ -161,7 +189,7 @@ __global__ void __launch_bounds__(kDecodeWarps * 32, OCC)
         // image index b (warp-uniform), NOT the lane's own lb: lane c only carries class c's ballot and may be an
         // inactive lane of a ragged last group, whose row index lies past the image
         int my_base = 0;
-        if (my_mask) my_base = atomicAdd(&cand_count[b * p.num_fg + lane], __popc(my_mask));
+        if (my_mask) my_base = atomicAdd(&cand_count[b * p.num_fg + cbase + lane], __popc(my_mask));
         for (unsigned rem = any; rem; rem &= rem - 1u) {
           const int c = __ffs(rem) - 1;
           const unsigned mk = __shfl_sync(0xffffffffu, my_mask, c);
@@ -169,31 +197,31 @@ __global__ void __launch_bounds__(kDecodeWarps * 32, OCC)
           if ((pass_bits >> c) & 1u) {
             const int slot_i = base + __popc(mk & ((1u << lane) - 1));
             if (slot_i < p.cap)
-              cand_keys[((long long)b * p.num_fg + c) * p.cap + slot_i] =
-                  ((unsigned long long)__float_as_uint(score(c)) << 32) | (0xFFFFFFFFu - (unsigned)ln);
+              cand_keys[((long long)b * p.num_fg + cbase + c) * p.cap + slot_i] =
+                  ((unsigned long long)__float_as_uint(score(cbase + c)) << 32) | (0xFFFFFFFFu - (unsigned)ln);
           }
         }
       } else {
         for (unsigned rem_c = any; rem_c; rem_c &= rem_c - 1u) {
           const int c = __ffs(rem_c) - 1;
-          const bool pass = (pass_bits >> c) & 1u;
-          const unsigned mask = __ballot_sync(0xffffffffu, pass);
+          const bool ok = (pass_bits >> c) & 1u;
+          const unsigned mask = __ballot_sync(0xffffffffu, ok);
           // rows of this warp straddle images: aggregate the counter update per image
           unsigned rem = mask;
           int slot_i = -1;
           while (rem) {
             const int leader = __ffs(rem) - 1;
             const int bl = __shfl_sync(0xffffffffu, lb, leader);
-            const unsigned grp = __ballot_sync(0xffffffffu, pass && lb == bl);
+            const unsigned grp = __ballot_sync(0xffffffffu, ok && lb == bl);
             int base = 0;
-            if (lane == leader) base = atomicAdd(&cand_count[bl * p.num_fg + c], __popc(grp));
+            if (lane == leader) base = atomicAdd(&cand_count[bl * p.num_fg + cbase + c], __popc(grp));
             base = __shfl_sync(0xffffffffu, base, leader);
-            if (pass && lb == bl) slot_i = base + __popc(grp & ((1u << lane) - 1));
+            if (ok && lb == bl) slot_i = base + __popc(grp & ((1u << lane) - 1));
             rem &= ~grp;
           }
-          if (pass && slot_i < p.cap)
-            cand_keys[((long long)lb * p.num_fg + c) * p.cap + slot_i] =
-                ((unsigned long long)__float_as_uint(score(c)) << 32) | (0xFFFFFFFFu - (unsigned)ln);
+          if (ok && slot_i < p.cap)
+            cand_keys[((long long)lb * p.num_fg + cbase + c) * p.cap + slot_i] =
+                ((unsigned long long)__float_as_uint(score(cbase + c)) << 32) | (0xFFFFFFFFu - (unsigned)ln);
         }
       }
     }
@@ -216,8 +244,8 @@ constexpr int kNselOverflowBit = 1 << 30;  // per-(image, class) "list was trunc
 
 // Class-major compaction of one image's per-class results into its packed record, run by whoever finishes the
 // image's LAST list: `nt` cooperating threads with ranks `t` (nt = 32 -> one warp, barriers are __syncwarp; nt = block
-// size -> __syncthreads), `s_off`: C + 1 ints of shared memory.  The first warp of the group computes the prefix sum
-// (one load per lane: one L2 round trip instead of C dependent ones).
+// size -> __syncthreads), `s_off`: C + 1 ints of shared memory (C <= kMaxFg).  The first warp of the group computes the
+// prefix sum, 32 classes per pass with a running carry (one load per lane and pass: one L2 round trip for C <= 32).
 __device__ __forceinline__ void compact_image(int b, int C, int MB, int t, int nt, int* s_off, const int* nsel_all,
                                               const float* st_det, const int* st_anchor, float* dets,
                                               long long det_img_stride, int* det_anchor, int* det_count, int* work) {
@@ -225,17 +253,20 @@ __device__ __forceinline__ void compact_image(int b, int C, int MB, int t, int n
   float* img_dets = dets + (long long)b * det_img_stride;
   if (t < 32) {
     const int lane = t;
-    const int v = lane < C ? __ldcg(nsel_all + (long long)b * C + lane) : 0;
-    const int n_l = v & ~kNselOverflowBit;
-    int incl = n_l;
+    int acc = 0, ovf = 0;
+    for (int c0 = 0; c0 < C; c0 += 32) {
+      const int v = c0 + lane < C ? __ldcg(nsel_all + (long long)b * C + c0 + lane) : 0;
+      const int n_l = v & ~kNselOverflowBit;
+      int incl = n_l;
 #pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const int up = __shfl_up_sync(0xffffffffu, incl, d);
-      if (lane >= d) incl += up;
+      for (int d = 1; d < 32; d <<= 1) {
+        const int up = __shfl_up_sync(0xffffffffu, incl, d);
+        if (lane >= d) incl += up;
+      }
+      if (c0 + lane < C) s_off[c0 + lane] = acc + incl - n_l;
+      acc += __shfl_sync(0xffffffffu, incl, 31);
+      ovf |= __any_sync(0xffffffffu, (v & kNselOverflowBit) != 0);
     }
-    if (lane < C) s_off[lane] = incl - n_l;
-    const int acc = __shfl_sync(0xffffffffu, incl, 31);
-    const int ovf = __any_sync(0xffffffffu, (v & kNselOverflowBit) != 0);
     if (lane == 0) {
       s_off[C] = acc;
       det_count[b] = acc;
@@ -347,7 +378,8 @@ __global__ void __launch_bounds__(kNmsThreads)
     cnt = p.cap;
   }
   unsigned long long* gkeys = cand_keys + ((long long)b * p.num_fg + c) * p.cap;
-  const float* hb = head + (long long)b * p.N * kRow;
+  const int row = row_floats(p.num_fg);
+  const float* hb = head + (long long)b * p.N * row;
   const int cnt_all = cnt;
   int nsel = 0;
   {
@@ -417,7 +449,7 @@ __global__ void __launch_bounds__(kNmsThreads)
             sm.keys[slot] = k;
             const int n = (int)(0xFFFFFFFFu - (unsigned)(k & 0xFFFFFFFFull));
             Cell cell = locate(p, n);
-            sm.box[slot] = decode_box(p, cell, hb + (long long)n * kRow);
+            sm.box[slot] = decode_box(p, cell, hb + (long long)n * row);
           }
         }
       }
@@ -440,7 +472,7 @@ __global__ void __launch_bounds__(kNmsThreads)
       sm.keys[i] = k;
       const int n = (int)(0xFFFFFFFFu - (unsigned)(k & 0xFFFFFFFFull));
       Cell cell = locate(p, n);
-      sm.box[i] = decode_box(p, cell, hb + (long long)n * kRow);
+      sm.box[i] = decode_box(p, cell, hb + (long long)n * row);
     }
   } else {
     if (tid == 0) {
@@ -458,7 +490,7 @@ __global__ void __launch_bounds__(kNmsThreads)
       for (int i = tid; i < cnt; i += blockDim.x) {
         const int n = (int)(0xFFFFFFFFu - (unsigned)(gkeys[i] & 0xFFFFFFFFull));
         Cell cell = locate(p, n);
-        wb[i] = decode_box(p, cell, hb + (long long)n * kRow);
+        wb[i] = decode_box(p, cell, hb + (long long)n * row);
       }
       pbox = wb;
     }
@@ -520,7 +552,7 @@ __global__ void __launch_bounds__(kNmsThreads)
       cur = pbox[hp];
     } else {
       Cell cell = locate(p, hn);
-      cur = decode_box(p, cell, hb + (long long)hn * kRow);
+      cur = decode_box(p, cell, hb + (long long)hn * row);
     }
     if (tid == 0) {
       float* d = st_det + (bc * MB + nsel) * 6;
@@ -552,7 +584,7 @@ __global__ void __launch_bounds__(kNmsThreads)
       } else {
         const int n = (int)(0xFFFFFFFFu - (unsigned)(kj & 0xFFFFFFFFull));
         Cell cell = locate(p, n);
-        bj = decode_box(p, cell, hb + (long long)n * kRow);
+        bj = decode_box(p, cell, hb + (long long)n * row);
       }
       if (iou_tf(bj, cur) > p.iou_thr) keys[j] = 0ull;
     }
@@ -577,7 +609,7 @@ __global__ void __launch_bounds__(kNmsThreads)
   __syncthreads();
   if (!s_last) return;
   __threadfence();
-  __shared__ int s_off[33];
+  __shared__ int s_off[kMaxFg + 1];
   compact_image(b, C, MB, tid, kNmsThreads, s_off, nsel_all, st_det, st_anchor, dets, det_img_stride, det_anchor,
                 det_count, work);
 }
@@ -590,13 +622,29 @@ static int check_tail(const odt_tail_params* p) {
   ODT_CHECK_ARG(p != nullptr, "params null");
   ODT_CHECK_ARG(p->kind >= 0 && p->kind <= 2, "kind");
   ODT_CHECK_ARG(p->num_levels >= 1 && p->num_levels <= ODT_MAX_LEVELS, "num_levels");
-  ODT_CHECK_ARG(p->num_fg >= 1 && p->num_fg <= 20, "num_fg must be 1..20");
-  ODT_CHECK_ARG(p->nms_classes >= 1 && p->nms_classes <= p->num_fg && p->nms_classes <= 32,
-                "nms_classes");
+  // the softmax family (SSD / RetinaNet) decodes 21 logits; YOLOv3 / FCOS rows carry 1..kMaxFg class scores
+  if (p->kind == ODT_DECODE_SSD) ODT_CHECK_ARG(p->num_fg == 20, "num_fg must be 20 for the softmax family");
+  else ODT_CHECK_ARG(p->num_fg >= 1 && p->num_fg <= kMaxFg, "num_fg must be 1..128");
+  // 0 NMS classes: FCOS with one class visits range(num_classes - 1) = no class (ref FCOS.py:252)
+  ODT_CHECK_ARG(p->nms_classes >= 0 && p->nms_classes <= p->num_fg, "nms_classes");
   ODT_CHECK_ARG(p->N > 0 && p->cap > 0 && p->max_boxes > 0, "N/cap/max_boxes");
   for (int i = 0; i < p->num_levels; ++i)
     ODT_CHECK_ARG(p->level[i].A >= 1 && p->level[i].A <= ODT_MAX_PRIORS, "level.A");
   return ODT_OK;
+}
+
+// Records of a tail without NMS classes: every image's count and overflow flag are 0 (D = 0).
+__global__ void empty_records_kernel(int B, float* __restrict__ dets, long long det_img_stride,
+                                     int* __restrict__ det_count, int* __restrict__ work) {
+  pdl_launch_dependents();
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  det_count[b] = 0;
+  work[b] = 0;
+  if (det_img_stride >= 2) {
+    dets[(long long)b * det_img_stride] = 0.f;
+    dets[(long long)b * det_img_stride + 1] = 0.f;
+  }
 }
 
 extern "C" int odt_decode_candidates(const float* head, const odt_tail_params* p, int B,
@@ -612,36 +660,51 @@ extern "C" int odt_decode_candidates(const float* head, const odt_tail_params* p
   tp.p = *p;
   long long rows = (long long)B * p->N;
   long long groups = (rows + 31) / 32;
-  int blocks = (int)((groups + kDecodeWarps - 1) / kDecodeWarps);
+  // 25-float rows (num_fg = 20, every family): 8 warps per CTA.  Two builds per kind (A/B by ODT_DECODE_CFG): "3x2" =
+  // 3 CTAs / SM with 2 stages per warp (24 warps x 1 group in flight ahead, the default), "2x4" = 2 CTAs / SM with 4
+  // stages (16 warps x 3 groups ahead: more bytes in flight per SM, fewer warps to hide instruction latency).  The
+  // default is carried over from the previous target; it has not been re-measured on the H100.
+  // Other class counts (YOLOv3 / FCOS): 4 warps x 2 stages, as many CTAs per SM as their staging allows.
+  const bool wide = p->num_fg != 20;
+  const int warps = wide ? kDecodeWarpsWide : kDecodeWarps;
+  int blocks = (int)((groups + warps - 1) / warps);
   int per_sm = 6;  // 2-3 CTAs resident per SM: two to three waves
+  if (wide) {
+    const long long smem = decode_smem_bytes(kDecodeWarpsWide, 2, row_floats(p->num_fg));
+    per_sm = (int)(2 * ((228 * 1024) / (smem + 1024)));  // two waves of the CTAs that fit (1 KB reserved per CTA)
+  }
   if (const char* e = getenv("ODT_DECODE_BLOCKS_PER_SM")) per_sm = atoi(e) > 0 ? atoi(e) : per_sm;
   int maxb = kNumSMs * per_sm;
   if (blocks > maxb) blocks = maxb;
-  // Two builds per kind (A/B by ODT_DECODE_CFG): "3x2" = 3 CTAs / SM with 2 stages per warp (24 warps x 1 group in
-  // flight ahead, the default), "2x4" = 2 CTAs / SM with 4 stages (16 warps x 3 groups ahead: more bytes in flight per
-  // SM, fewer warps to hide instruction latency).  The default is carried over from the previous target; it has not
-  // been re-measured on the H100.
   int deep = 0;
   if (const char* e = getenv("ODT_DECODE_CFG")) deep = strcmp(e, "2x4") == 0 ? 1 : 0;
-#define ODT_DECODE_LAUNCH(KIND_, OCC_, ST_)                                                                      \
+#define ODT_DECODE_LAUNCH(KIND_, WARPS_, OCC_, ST_, NFG_, SMEM_MAX_)                                               \
   do {                                                                                                           \
     static bool attr_done = false;                                                                               \
     if (!attr_done) {                                                                                            \
-      ODT_CUDA_OK(cudaFuncSetAttribute(decode_candidates_kernel<KIND_, OCC_, ST_>,                               \
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize,                              \
-                                       (int)sizeof(DecodeSmem<ST_>)));                                           \
+      ODT_CUDA_OK(cudaFuncSetAttribute(decode_candidates_kernel<KIND_, WARPS_, OCC_, ST_, NFG_>,                 \
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(SMEM_MAX_)));           \
       attr_done = true;                                                                                          \
     }                                                                                                            \
-    decode_candidates_kernel<KIND_, OCC_, ST_><<<blocks, kDecodeWarps * 32, sizeof(DecodeSmem<ST_>), st>>>(      \
-        head, tp, rows, cand_keys, cand_count);                                                                  \
+    decode_candidates_kernel<KIND_, WARPS_, OCC_, ST_, NFG_>                                                     \
+        <<<blocks, (WARPS_) * 32, decode_smem_bytes(WARPS_, ST_, row_floats(p->num_fg)), st>>>(                  \
+            head, tp, rows, cand_keys, cand_count);                                                              \
   } while (0)
+#define ODT_DECODE_LAUNCH20(KIND_, OCC_, ST_) \
+  ODT_DECODE_LAUNCH(KIND_, kDecodeWarps, OCC_, ST_, 20, decode_smem_bytes(kDecodeWarps, ST_, row_floats(20)))
+#define ODT_DECODE_LAUNCH_WIDE(KIND_) \
+  ODT_DECODE_LAUNCH(KIND_, kDecodeWarpsWide, 1, 2, 0, decode_smem_bytes(kDecodeWarpsWide, 2, row_floats(kMaxFg)))
   if (p->kind == ODT_DECODE_SSD) {
-    if (deep) ODT_DECODE_LAUNCH(ODT_DECODE_SSD, 2, 4); else ODT_DECODE_LAUNCH(ODT_DECODE_SSD, 3, 2);
+    if (deep) ODT_DECODE_LAUNCH20(ODT_DECODE_SSD, 2, 4); else ODT_DECODE_LAUNCH20(ODT_DECODE_SSD, 3, 2);
   } else if (p->kind == ODT_DECODE_YOLO3) {
-    if (deep) ODT_DECODE_LAUNCH(ODT_DECODE_YOLO3, 2, 4); else ODT_DECODE_LAUNCH(ODT_DECODE_YOLO3, 3, 2);
+    if (wide) ODT_DECODE_LAUNCH_WIDE(ODT_DECODE_YOLO3);
+    else if (deep) ODT_DECODE_LAUNCH20(ODT_DECODE_YOLO3, 2, 4); else ODT_DECODE_LAUNCH20(ODT_DECODE_YOLO3, 3, 2);
   } else {
-    if (deep) ODT_DECODE_LAUNCH(ODT_DECODE_FCOS, 2, 4); else ODT_DECODE_LAUNCH(ODT_DECODE_FCOS, 3, 2);
+    if (wide) ODT_DECODE_LAUNCH_WIDE(ODT_DECODE_FCOS);
+    else if (deep) ODT_DECODE_LAUNCH20(ODT_DECODE_FCOS, 2, 4); else ODT_DECODE_LAUNCH20(ODT_DECODE_FCOS, 3, 2);
   }
+#undef ODT_DECODE_LAUNCH_WIDE
+#undef ODT_DECODE_LAUNCH20
 #undef ODT_DECODE_LAUNCH
   ODT_LAUNCH_OK();
   return ODT_OK;
@@ -660,10 +723,17 @@ extern "C" int odt_nms_per_class(const float* head, const odt_tail_params* p, in
                                  long long dets_img_stride, void* stream) {
   int rc = check_tail(p);
   if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (p->nms_classes == 0) {  // no list to visit (D = 0): the records still get their count and overflow flag
+    ODT_CHECK_ARG(dets && det_count && work && status && B > 0, "null pointer / B");
+    ODT_CUDA_OK(cudaMemsetAsync(status, 0, sizeof(int), st));
+    empty_records_kernel<<<(B + 127) / 128, 128, 0, st>>>(B, dets, dets_img_stride, det_count, work);
+    ODT_LAUNCH_OK();
+    return ODT_OK;
+  }
   ODT_CHECK_ARG(head && cand_keys && cand_count && dets && det_anchor && det_count &&
                     sel_scratch && work && status && B > 0,
                 "null pointer / B");
-  cudaStream_t st = (cudaStream_t)stream;
   static bool attr_set = false;
   if (!attr_set) {
     ODT_CUDA_OK(cudaFuncSetAttribute(nms_per_class_kernel,

@@ -5,7 +5,15 @@
 
 namespace odt {
 
-constexpr int kRow = 25;  // floats per candidate row in the head buffer
+// Floats per candidate row in the head buffer: num_fg class scores + 5 (DESIGN.md section 2).  SSD / RetinaNet:
+// 20 + background + 4 = 25; YOLOv3: [cls(num_fg), y, x, h, w, obj]; FCOS: [cls(num_fg), ctr, l, r, t, b].  Every row
+// stride and column offset of the tail and the loss kernels goes through this function.
+__host__ __device__ __forceinline__ constexpr int row_floats(int num_fg) { return num_fg + 5; }
+
+// Largest num_fg of the sigmoid families (YOLOv3 / FCOS): the decode kernel stages 32 rows of row_floats(128) = 133
+// floats (17 KB) per warp and stage, and keeps one pass mask of kMaxFg / 32 = 4 words per row in registers.
+constexpr int kMaxFg = 128;
+constexpr int kMaskWords = kMaxFg / 32;
 
 struct TailP {
   odt_tail_params p;
@@ -81,16 +89,17 @@ __device__ __forceinline__ Anchor anchor_ssd(const odt_tail_params& p, const Cel
   return a;
 }
 
-// Box (y1,x1,y2,x2) of candidate row `r` (25 floats) at cell c.
+// Box (y1,x1,y2,x2) of candidate row `row` (row_floats(p.num_fg) floats) at cell c.
 __device__ __forceinline__ float4 decode_box(const odt_tail_params& p, const Cell& c,
-                                             const float* __restrict__ r) {
+                                             const float* __restrict__ row) {
   const odt_level& L = p.level[c.lvl];
+  const float* __restrict__ r = row + p.num_fg;  // the 5 columns behind the class scores
   float4 o;
   if (p.kind == ODT_DECODE_SSD) {
-    // ref SSD300.py:323-343 (anchors), :167-171 (decode); RetinaNet.py:328-355,:234-238
+    // ref SSD300.py:323-343 (anchors), :167-171 (decode); RetinaNet.py:328-355,:234-238.  r[0]: background logit
     const Anchor an = anchor_ssd(p, c);
     const float ay = an.cy, ax = an.cx, ah = an.h, aw = an.w;
-    float ty = r[21], tx = r[22], th = r[23], tw = r[24];
+    float ty = r[1], tx = r[2], th = r[3], tw = r[4];
     float dy = __fadd_rn(__fmul_rn(ty, ah), ay);
     float dx = __fadd_rn(__fmul_rn(tx, aw), ax);
     float dh = __fmul_rn(ah, expf(th));
@@ -103,19 +112,19 @@ __device__ __forceinline__ float4 decode_box(const odt_tail_params& p, const Cel
   } else if (p.kind == ODT_DECODE_YOLO3) {
     // ref YOLOv3.py:419-433 (priors), :340-348 (additive exp, x stride multiplier)
     float ay = (float)c.y + 0.5f, ax = (float)c.x + 0.5f;
-    float by = __fadd_rn(ay, sigmoid_rn(r[20]));
-    float bx = __fadd_rn(ax, sigmoid_rn(r[21]));
-    float bh = __fadd_rn(L.prior_h[c.a], expf(r[22]));
-    float bw = __fadd_rn(L.prior_w[c.a], expf(r[23]));
+    float by = __fadd_rn(ay, sigmoid_rn(r[0]));
+    float bx = __fadd_rn(ax, sigmoid_rn(r[1]));
+    float bh = __fadd_rn(L.prior_h[c.a], expf(r[2]));
+    float bw = __fadd_rn(L.prior_w[c.a], expf(r[3]));
     float h2 = __fmul_rn(bh, 0.5f), w2 = __fmul_rn(bw, 0.5f);
     o.x = __fmul_rn(__fsub_rn(by, h2), L.out_mul);
     o.y = __fmul_rn(__fsub_rn(bx, w2), L.out_mul);
     o.z = __fmul_rn(__fadd_rn(by, h2), L.out_mul);
     o.w = __fmul_rn(__fadd_rn(bx, w2), L.out_mul);
   } else {
-    // FCOS: ref FCOS.py:130-150 (grid, no +0.5), :363 (exp), :216-240
+    // FCOS: ref FCOS.py:130-150 (grid, no +0.5), :363 (exp), :216-240.  r[0]: centre-ness
     float gy = (float)c.y, gx = (float)c.x;
-    float l = expf(r[21]), rr = expf(r[22]), t = expf(r[23]), bb = expf(r[24]);
+    float l = expf(r[1]), rr = expf(r[2]), t = expf(r[3]), bb = expf(r[4]);
     o.x = __fmul_rn(__fsub_rn(gy, t), L.out_mul);
     o.y = __fmul_rn(__fsub_rn(gx, l), L.out_mul);
     o.z = __fmul_rn(__fadd_rn(gy, bb), L.out_mul);

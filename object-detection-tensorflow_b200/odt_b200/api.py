@@ -101,9 +101,10 @@ class _Detector:
         from .engine import Net
         Net.spec_only = True
         try:
-            net, _ = self._build(1, "fp32", False)
+            net, tail = self._build(1, "fp32", False)
         finally:
             Net.spec_only = False
+        net.tail = tail  # never prepared: it describes the head rows (Tail.row) for the training step
         return net
 
     def _initial_weights(self, variables):
@@ -630,6 +631,7 @@ class YOLOv3(_Detector):
 
     def __init__(self, config, data_provider):
         assert len(config["data_shape"]) == 3
+        nets.check_sigmoid_num_classes(config)
         self._common_init(config, data_provider)
         self.data_shape = config["data_shape"]
         self.num_classes = config["num_classes"]
@@ -654,6 +656,7 @@ class FCOS(_Detector):
     loss_kind = "fcos"
 
     def __init__(self, config, data_provider):
+        nets.check_sigmoid_num_classes(config)
         self._common_init(config, data_provider)
         self.data_shape = config["data_shape"]
         self.num_classes = config["num_classes"]

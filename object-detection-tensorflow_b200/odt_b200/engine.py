@@ -9,7 +9,7 @@ A model file (nets.py) describes its layers once through `Builder`; the builder
   * fuses what the reference expresses as separate TF ops into conv epilogues:
     bias / folded inference BN / ReLU / LeakyReLU / residual add / the
     consumer's pre-activation BN+ReLU (second output) / direct scatter of the
-    head convolutions into the [B, N, 25] candidate-row buffer.
+    head convolutions into the [B, N, Tail.row] candidate-row buffer.
 """
 import ctypes as C
 import math
@@ -157,12 +157,12 @@ class ConvOp(Op):
         p.in_halo = 0 if self.is_image else x.halo
         p.out0_halo = 0
         if self.head is not None:
-            hb = net.head_buf
+            hb, row = net.head_buf, net.tail.row
             lvl_off, col, group, gstride, A = self.head
-            p.out0 = hb.data_ptr() + 4 * (lvl_off * 25 + col)
+            p.out0 = hb.data_ptr() + 4 * (lvl_off * row + col)
             p.out0_dtype = L.ODT_F32
-            p.out0_img_stride = net.N * 25
-            p.out0_pix_stride = A * 25
+            p.out0_img_stride = net.N * row
+            p.out0_pix_stride = A * row
             p.out0_group, p.out0_group_stride = group, gstride
         else:
             y = self.y
@@ -692,7 +692,8 @@ class Net:
                 continue  # raw output nobody reads (only its fused pre-activations are consumed)
             t.buf = torch.zeros((t.B, t.H + 2 * t.halo, t.W + 2 * t.halo, t.ld), dtype=self.tdtype, device=dev)
         self.N = sum(h * w * a for h, w, a in self.levels)
-        self.head_buf = torch.zeros((self.batch, self.N, 25), dtype=torch.float32, device=dev)
+        # candidate rows of a detection tail (a classification tail has no head levels and no rows)
+        self.head_buf = torch.zeros((self.batch, self.N, getattr(tail, "row", 0)), dtype=torch.float32, device=dev)
         self.tail = tail
         tail.prepare(self)
         # one fp64 arena for the workspaces of every GroupNorm (per-slice moments, statistics, arrival counters),
@@ -906,10 +907,13 @@ class Net:
 
 
 class Tail:
-    """decode + per-class NMS (+ optional class-major compaction) on [B,N,25] rows."""
+    """decode + per-class NMS (+ optional class-major compaction) on [B,N,row] candidate rows."""
 
     def __init__(self, kind, num_fg, nms_classes, score_thr, iou_thr, max_boxes, level_fn, cap=None):
         self.kind, self.num_fg, self.nms_classes = kind, num_fg, nms_classes
+        # floats per candidate row, the one place the host decides it (DESIGN.md section 2): num_fg class scores + 5
+        # (SSD / RetinaNet: 20 + background + 4 box; YOLOv3: 4 box + objectness; FCOS: centre-ness + 4 distances)
+        self.row = num_fg + 5
         self.score_thr, self.iou_thr, self.max_boxes = score_thr, iou_thr, max_boxes
         self.level_fn, self.cap = level_fn, cap
         self.pool_cap = 8 << 20  # box-pool entries (16 B each) for lists beyond the shared-memory window
@@ -942,7 +946,7 @@ class Tail:
         self.det_anchor = torch.zeros((B, D), dtype=torch.int32, device=dev)
         self.det_count = torch.zeros((B,), dtype=torch.int32, device=dev)
         nbytes = net.lib.odt_nms_scratch_bytes(C.byref(p), B)
-        self.scratch = torch.zeros((nbytes + 3) // 4, dtype=torch.int32, device=dev)
+        self.scratch = torch.zeros(max(1, (nbytes + 3) // 4), dtype=torch.int32, device=dev)  # 0 NMS classes: 0 bytes
         self.work = torch.zeros((B + (B & 1) + 2,), dtype=torch.int32, device=dev)
         self.status = torch.zeros((1,), dtype=torch.int32, device=dev)
         # box cache for candidate lists longer than the NMS shared-memory window
@@ -959,7 +963,7 @@ class Tail:
     def launch_nms(self, net, stream):
         L.check(net.lib.odt_nms_per_class(self.head_buf.data_ptr(), C.byref(self.p), net.batch,
                                           self.cand_keys.data_ptr(), self.cand_count.data_ptr(),
-                                          self.dets.data_ptr(), self.det_anchor.data_ptr(),
+                                          self.rec.data_ptr(), self.det_anchor.data_ptr(),  # dets: a view at offset 0
                                           self.det_count.data_ptr(), self.scratch.data_ptr(),
                                           self.work.data_ptr(), self.status.data_ptr(),
                                           self.box_pool.data_ptr() if self.box_pool is not None else None,
@@ -1104,7 +1108,7 @@ def unpack_records(rec, cap=None):
 
 
 class RowsHarness:
-    """Runs a Tail on caller-provided candidate rows [B,N,25] (no backbone):
+    """Runs a Tail on caller-provided candidate rows [B,N,tail.row] (no backbone):
     the tail kernels in isolation, for parity tests and the decode/NMS microbench."""
 
     def __init__(self, tail, levels, rows, device="cuda"):
@@ -1113,7 +1117,7 @@ class RowsHarness:
         self.levels = list(levels)
         self.head_buf = torch.as_tensor(np.ascontiguousarray(rows, dtype=np.float32)).to(self.device)
         self.batch, self.N = self.head_buf.shape[0], self.head_buf.shape[1]
-        assert self.N == sum(h * w * a for h, w, a in self.levels) and self.head_buf.shape[2] == 25
+        assert self.N == sum(h * w * a for h, w, a in self.levels) and self.head_buf.shape[2] == tail.row
         self.tail = tail
         tail.prepare(self)
 

@@ -32,6 +32,19 @@ def check_num_classes(cfg):
                          "foreground classes (VOC)" % (cfg["num_classes"],))
 
 
+MAX_SIGMOID_CLASSES = 128
+
+
+def check_sigmoid_num_classes(cfg):
+    """YOLOv3 and FCOS score each class with its own sigmoid, so their candidate rows hold num_classes + 5 floats
+    (DESIGN.md section 2) and any count from 1 to 128 runs.  The limit of 128 comes from the decode kernel: it stages 32
+    rows of up to 133 floats (17 KB) per warp in shared memory and keeps one 4-word pass mask per row in registers."""
+    nc = cfg["num_classes"]
+    if isinstance(nc, bool) or not isinstance(nc, (int, np.integer)) or not 1 <= nc <= MAX_SIGMOID_CLASSES:
+        raise ValueError("num_classes = %r: YOLOv3 and FCOS support 1 to %d classes"
+                         % (nc, MAX_SIGMOID_CLASSES))
+
+
 # ------------------------------------------------------------------- SSD ----
 def ssd_scales(size):
     """ref SSD300.py:112-113, SSD512.py:116-118 (Python doubles like the reference)."""
@@ -209,11 +222,11 @@ def build_retinanet(batch, cfg, precision="fp16", device="cuda", allow_tc=True):
             y = p
             for _ in range(4):
                 y = _bac(net, y, 256, 3, 1, "bn")
-            _bac(net, y, nc * A, 3, 1, "bn", head=(off, 0, nc, 25, A), bias_init="pi")
+            _bac(net, y, nc * A, 3, 1, "bn", head=(off, 0, nc, nc + 4, A), bias_init="pi")
             y = p
             for _ in range(4):
                 y = _bac(net, y, 256, 3, 1, "bn")
-            _bac(net, y, 4 * A, 3, 1, "bn", head=(off, nc, 4, 25, A))
+            _bac(net, y, 4 * A, 3, 1, "bn", head=(off, nc, 4, nc + 4, A))
     return net, retina_tail(cfg)
 
 
@@ -243,8 +256,9 @@ def retina_tail(cfg):
 def build_yolov3(batch, cfg, precision="fp16", device="cuda", allow_tc=True):
     """ref YOLOv3.py:81-113,387-417,485-507."""
     H, W, _ = cfg["data_shape"]
+    check_sigmoid_num_classes(cfg)
     nc, npri = cfg["num_classes"], cfg["num_priors"]
-    assert npri == 3 and nc == 20, "row layout is 20 classes + 4 box + 1 obj"
+    assert npri == 3, "3 priors per level"
     net = Net(batch, H, W, precision, device, allow_tc)
 
     def cl(x, f, k, s, act=True, residual=None, head=None):  # conv -> BN -> leaky (:494-507)
@@ -310,10 +324,10 @@ def yolo_tail(cfg):
 
 # ------------------------------------------------------------------ FCOS ----
 def build_fcos(batch, cfg, precision="fp16", device="cuda", allow_tc=True, share_heads=True):
-    """ref FCOS.py:70-107,350-364.  Row layout: [cls(20), ctr, l, r, t, b] raw."""
+    """ref FCOS.py:70-107,350-364.  Row layout: [cls(num_classes), ctr, l, r, t, b] raw."""
+    check_sigmoid_num_classes(cfg)
     H, W, _ = cfg["data_shape"]
     nc = cfg["num_classes"]
-    assert nc == 20, "row layout is 20 classes + centerness + 4 regressions"
     net = Net(batch, H, W, precision, device, allow_tc)
     filters = [16 * (2 ** i) for i in range(4)]
     with net.scope("backone"):
@@ -347,7 +361,8 @@ def build_fcos(batch, cfg, precision="fp16", device="cuda", allow_tc=True, share
 
 
 def fcos_tail(cfg):
-    """decode/NMS tail of FCOS (ref FCOS.py:130-150,197-264); NMS visits 19 classes (:252)."""
+    """decode/NMS tail of FCOS (ref FCOS.py:130-150,197-264); NMS visits num_classes - 1 classes (:252): 19 for VOC,
+    none for a single class."""
     nc = cfg["num_classes"]
     strides = [8.0, 16.0, 32.0, 64.0, 128.0]
 

@@ -259,6 +259,7 @@ class GraphTrainer:
         self.dtype = dtype
         self.net = model._build_spec()            # unfused op list, no CUDA
         self.features = self.net.ops[-1].y        # the last tensor of the list (forward_features)
+        self.row = getattr(self.net.tail, "row", None)  # floats per candidate row (engine.Tail.row)
         w = model.get_weights()
         self.params, self.buffers, self.slots = {}, {}, {}
         for name, arr in w.items():
@@ -289,9 +290,9 @@ class GraphTrainer:
         return x * inv.view(1, -1, 1, 1) + (b - mean * inv).view(1, -1, 1, 1)
 
     def forward_rows(self, images, training=True, stats=None):
-        """images [B,H,W,3] -> candidate rows [B,N,25] in the layout of DESIGN.md section 2."""
+        """images [B,H,W,3] -> candidate rows [B,N,row] in the layout of DESIGN.md section 2."""
         _, rows = self._replay(images, training, stats)
-        return rows.view(rows.shape[0], rows.shape[1] // 25, 25)
+        return rows.view(rows.shape[0], rows.shape[1] // self.row, self.row)
 
     def forward_features(self, images, training=True, stats=None):
         """images [B,H,W,3] -> the last tensor of the layer list, NCHW (pretraining mode: the last bottleneck's
@@ -300,7 +301,7 @@ class GraphTrainer:
         return val[id(self.features)]
 
     def _replay(self, images, training, stats):
-        """The layer list with torch ops -> ({id(Act): NCHW value}, head rows [B, N*25])."""
+        """The layer list with torch ops -> ({id(Act): NCHW value}, head rows [B, N*row])."""
         E, P = self.E, self.params
         stats = [] if stats is None else stats
         x0 = torch.as_tensor(images, device=self.device, dtype=self.dtype)
@@ -308,7 +309,7 @@ class GraphTrainer:
         x0 = (x0 - mean).permute(0, 3, 1, 2)
         B = x0.shape[0]
         N = sum(h * w * a for h, w, a in self.net.levels)
-        rows = torch.zeros((B, N * 25), device=self.device, dtype=self.dtype)
+        rows = torch.zeros((B, N * (self.row or 0)), device=self.device, dtype=self.dtype)
         val = {}
         for op in self.net.ops:
             if isinstance(op, E.ConvOp):
@@ -327,7 +328,7 @@ class GraphTrainer:
                 n = torch.arange(C, device=self.device)
                 ch = (n // group) * gstride + (n % group) if group > 0 else n
                 pix = torch.arange(H * W, device=self.device)
-                idx = ((lvl_off + pix * A) * 25 + col).view(-1, 1) + ch.view(1, -1)
+                idx = ((lvl_off + pix * A) * self.row + col).view(-1, 1) + ch.view(1, -1)
                 rows = rows.index_add(1, idx.reshape(-1), y.permute(0, 2, 3, 1).reshape(Bc, -1))
             elif isinstance(op, E.PoolOp):
                 val[id(op.y)] = max_pool_same(val[id(op.x)], op.k, op.stride)
@@ -419,14 +420,15 @@ class GraphTrainer:
         size = torch.sqrt(g[:, 2] * g[:, 3])
         sel = [size <= 64, (size >= 64) & (size <= 128), (size >= 128) & (size <= 256), (size >= 256) & (size <= 512),
                size >= 512]
+        nc = self.row - 5
         total, off = 0.0, 0
         for (h, w, _), m, s in zip(self.net.levels, sel, [8, 16, 32, 64, 128]):
-            r = row[off:off + h * w].view(h, w, 25)
+            r = row[off:off + h * w].view(h, w, self.row)
             off += h * w
             if not bool(m.any()):
                 continue
             gl = g[m]
-            cls, ctr, reg = r[..., :20], r[..., 20], r[..., 21:25]
+            cls, ctr, reg = r[..., :nc], r[..., nc], r[..., nc + 1:nc + 5]
             with torch.no_grad():
                 gy, gx, gh, gw = [gl[:, i] / s for i in range(4)]
                 cid = gl[:, 4].long()
@@ -445,7 +447,7 @@ class GraphTrainer:
                 lrmin, tbmin = torch.minimum(dl, dr), torch.minimum(dt, db)
                 lrmax, tbmax = torch.maximum(dl, dr), torch.maximum(dt, db)
                 cgt = torch.sqrt(lrmin * tbmin / (lrmax * tbmax + 1e-12))
-                hgt = torch.zeros((h, w, 20), device=self.device, dtype=self.dtype)
+                hgt = torch.zeros((h, w, nc), device=self.device, dtype=self.dtype)
                 for c in torch.unique(cid).tolist():
                     hgt[..., c] = heat[..., cid == c].max(dim=-1).values
             p = torch.exp(reg)
@@ -462,7 +464,7 @@ class GraphTrainer:
 
     def yolo_image_loss(self, row, gt):
         """YOLOv3.py:115-318 for one image, quirks kept (see oracle/loss.py::yolo_image_loss): returns pos_loss + neg_loss."""
-        nc = 20
+        nc = self.row - 5
         cs, ns = float(self.cfg["coord_scale"]), float(self.cfg["noobj_scale"])
         os_, ks = float(self.cfg["obj_scale"]), float(self.cfg["class_scale"])
         gt = torch.as_tensor(gt, device=self.device, dtype=self.dtype)
@@ -471,7 +473,7 @@ class GraphTrainer:
         norm, pstride = [32.0, 16.0, 8.0], [8.0, 16.0, 32.0]
         lv, off = [], 0
         for k, (h, w, a) in enumerate(self.net.levels):
-            r = row[off:off + h * w * a].view(h, w, a, 25)
+            r = row[off:off + h * w * a].view(h, w, a, self.row)
             off += h * w * a
             with torch.no_grad():
                 pri = torch.tensor(self.cfg["priors"][k], device=self.device, dtype=self.dtype) / pstride[k]
@@ -494,7 +496,7 @@ class GraphTrainer:
             r, pri = L_["r"], L_["pri"]
             gi = torch.nonzero(m).squeeze(1)
             if gi.numel():
-                rws = r[L_["fl"][gi, 0], L_["fl"][gi, 1], L_["idx"][gi]]                 # [n,25]
+                rws = r[L_["fl"][gi, 0], L_["fl"][gi, 1], L_["idx"][gi]]                 # [n,row]
                 tyx = L_["gyx"][gi] - torch.floor(L_["gyx"][gi])
                 thw = torch.log(L_["ghw"][gi] / pri[L_["idx"][gi]])
                 coord = coord + bce(rws[:, nc:nc + 2], tyx, reduction="sum") \
