@@ -155,13 +155,12 @@ int odt_conv2d_direct(const void* in, const void* weights, int dtype, const odt_
 int odt_conv2d_stem(const float* images, const float* mean3_host, const void* weights, int dtype,
                     const odt_conv_params* p, void* stream);
 
-/* Tensor-core (wgmma) stem on the packed image of odt_pack_input_rgbx (p->in_ld = 4, p->in_halo = its pad: 1 for the
- * 3x3/stride-1 stems with 64 / 32 outputs, 4 for the 7x7/stride-2 stem with even W / left pad and Cout <= 16 real
- * outputs: it always computes and stores 16 channels, so Cout_pad = 16 and weights / scale / shift hold 16 rows, zero
- * past Cout, and out0_pix_stride >= 16);
+/* Tensor-core (wgmma) 7x7/stride-2 stem on the packed image of odt_pack_input_rgbx (p->in_ld = 4, p->in_halo = its
+ * pad = 4), with even W / left pad and Cout <= 16 real outputs: it always computes and stores 16 channels, so
+ * Cout_pad = 16 and weights / scale / shift hold 16 rows, zero past Cout, and out0_pix_stride >= 16;
  * every filter row of an output pixel is one aligned span of the image, so the im2col rows are built with
  * wide loads and no arithmetic.  ODT_ERR_UNSUPPORTED for other shapes (use odt_conv2d_stem).
- * ref: conv1_1 SSD300.py:193-200; YOLOv3.py:388; RetinaNet.py:260-265; FCOS.py:73-78 */
+ * ref: RetinaNet.py:260-265; FCOS.py:73-78 */
 int odt_conv2d_stem_rgbx(const void* rgbx, const void* weights, const odt_conv_params* p, void* stream);
 
 /* --------------------------------------------------------------- glue ---- */

@@ -13,52 +13,15 @@ void set_error(const char* fmt, ...) {
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
 }
-bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("ODT_PDL");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
-bool flat_enabled() {
-  const char* e = getenv("ODT_TC_FLAT");  // read every call: lets one process compare both paths
-  return !(e && e[0] == '0');
-}
-// Defaults carried over from the previous target (all three on); not re-measured on the H100.
-bool kskip_enabled() {
-  const char* e = getenv("ODT_TC_KSKIP");  // default on: all-zero K steps of thin layers are not issued (TcGeom::klast)
-  return !(e && e[0] == '0');
-}
-int thin_mode() {
-  // conv_thin.cu: 0 = off, 1 = where its cost rule takes the layer (default), 2 = wherever the layer qualifies
-  const char* e = getenv("ODT_TC_THIN");
+static int conv_mode(const char* var) {
+  const char* e = getenv(var);  // read every call: lets one process compare both paths
   return (e && e[0] >= '0' && e[0] <= '2') ? e[0] - '0' : 1;
 }
-int tapn_mode() {
-  // conv_tapn.cu: 0 = off, 1 = where its cost model predicts a gain (default), 2 = wherever the layer qualifies
-  const char* e = getenv("ODT_TC_TAPN");
-  return (e && e[0] >= '0' && e[0] <= '2') ? e[0] - '0' : 1;
-}
-int pw_mode() {
-  // conv_pw.cu (staged pointwise kernel): 0 = off, 1 = where its planner takes the layer (default), 2 = wherever it qualifies
-  const char* e = getenv("ODT_TC_PW");
-  return (e && e[0] >= '0' && e[0] <= '2') ? e[0] - '0' : 1;
-}
-int wide_mode() {
-  // conv_tc's 128 x 256 tile: 0 = off, 1 = where pick_bn's cost model takes it (default), 2 = wherever Cout_pad % 256 == 0
-  const char* e = getenv("ODT_TC_WIDE");  // read every call: lets one process compare both tiles
-  return (e && e[0] >= '0' && e[0] <= '2') ? e[0] - '0' : 1;
-}
-int swap_mode() {
-  // conv_tc_swap.cu (transposed tiles): 0 = off, 1 = where its planner takes the layer (default), 2 = wherever eligible
-  const char* e = getenv("ODT_TC_SWAP");  // read every call: lets one process compare both paths
-  return (e && e[0] >= '0' && e[0] <= '2') ? e[0] - '0' : 1;
-}
-bool wres_enabled() {
-  const char* e = getenv("ODT_TC_WRES");
-  return !(e && e[0] == '0');
-}
+int pw_mode() { return conv_mode("ODT_TC_PW"); }
+int thin_mode() { return conv_mode("ODT_TC_THIN"); }
+int tapn_mode() { return conv_mode("ODT_TC_TAPN"); }
+int swap_mode() { return conv_mode("ODT_TC_SWAP"); }
+int wide_mode() { return conv_mode("ODT_TC_WIDE"); }
 }  // namespace odt
 
 extern "C" int odt_abi_version(void) { return 5; }

@@ -68,10 +68,9 @@ __device__ __forceinline__ void pdl_launch_dependents() {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-bool pdl_enabled();   // ODT_PDL=0 disables the launch attribute (api.cu)
 
-// Launch with the programmatic-serialisation attribute unless ODT_PDL=0.  For kernels that call pdl_wait() before
-// they touch what the previous kernel in the stream wrote.
+// Launch with the programmatic-serialisation attribute.  For kernels that call pdl_wait() before they touch what the
+// previous kernel in the stream wrote.
 template <typename... KArgs, typename... Args>
 cudaError_t launch_pdl(void (*kern)(KArgs...), unsigned grid, int block, int smem, cudaStream_t st, Args... args) {
   cudaLaunchConfig_t cfg = {};
@@ -83,21 +82,20 @@ cudaError_t launch_pdl(void (*kern)(KArgs...), unsigned grid, int block, int sme
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kern, args...);
 }
 
-bool flat_enabled();  // ODT_TC_FLAT=0 disables the halo-flat 3x3 path (A/B measurements)
-bool kskip_enabled();  // ODT_TC_KSKIP=1: do not issue the all-zero 16-deep K steps of thin layers (Cin padded to 64)
-int wide_mode();     // ODT_TC_WIDE: conv_tc's 128 x 256 im2col tile, 0 off / 1 cost model (default) / 2 always
-int thin_mode();       // ODT_TC_THIN: 1 = very thin layers (Cin, Cout <= 32, few multiply-adds per pixel) go through the
-                       // CUDA-core kernel of conv_thin.cu, 2 = wherever the layer qualifies, 0 / unset = never
-int tapn_mode();       // ODT_TC_TAPN: 1 = narrow 3x3 halo layers go through conv_tapn.cu (taps folded into N) where its
-                       // cost model predicts a gain, 2 = wherever the layer qualifies, 0 / unset = never
-int pw_mode();         // ODT_TC_PW: 1 = narrow 1x1 / stride-1 layers go through the staged pointwise kernel of conv_pw.cu
-                       // (tried before conv_thin.cu), 2 = wherever the layer qualifies, 0 = never
-int swap_mode();       // ODT_TC_SWAP: 1 = narrow 3x3 halo layers (Cout_pad 64 / 128, fp16 out0 alone) run the transposed 64-cout x
-                       // 256-pixel tiles of conv_tc_swap.cu where its planner takes them, 2 = wherever eligible, 0 = never
-bool wres_enabled();  // ODT_TC_WRES=0 disables shared-memory-resident filter banks in the flat path
+// The per-kernel convolution switches, read on every call (api.cu): 0 = never, 1 = where the kernel's planner or
+// cost model takes the layer (the default, also when the variable is unset), 2 = wherever the layer qualifies.  They
+// stay because the tests need both ends: mode 2 pins a kernel onto shapes small enough to test, mode 0 gives the
+// bit-exact reference the kernel is compared with.  One function per kernel, so that the CPU harnesses of
+// tests/native/ can pin their kernel by defining its function alone.
+int pw_mode();    // ODT_TC_PW: narrow 1x1 / stride-1 layers on the staged pointwise kernel of conv_pw.cu (tried first)
+int thin_mode();  // ODT_TC_THIN: very thin layers (Cin, Cout <= 32, few multiply-adds per pixel) on conv_thin.cu
+int tapn_mode();  // ODT_TC_TAPN: narrow 3x3 halo layers with the horizontal taps folded into N (conv_tapn.cu)
+int swap_mode();  // ODT_TC_SWAP: narrow 3x3 halo layers (Cout_pad 64 / 128, fp16 out0 alone) on the transposed
+                  // 64-cout x 256-pixel tiles of conv_tc_swap.cu
+int wide_mode();  // ODT_TC_WIDE: conv_tc's 128 x 256 im2col tile (mode 2: wherever Cout_pad % 256 == 0)
 
 }  // namespace odt

@@ -13,13 +13,13 @@
 // (image read + activation write); the tensor pipe is idle most of the time.
 //
 //
-// H4 variants (round 2): the image arrives as mean-subtracted fp16 RGBX ([B][H+2P][W+2P][4], zero border, written by
-// odt_pack_input_rgbx).  A filter row of an output pixel is then ONE contiguous, aligned span of the image
-// (7x7/2: 8 pixels = 64 bytes = four 16-byte chunks, the eighth tap has zero weights; 3x3/1: 3 pixels = 24 bytes), so
-// a producer thread issues all of its loads back to back (28 LDG.128 or 9 LDG.64, adjacent lanes on adjacent
-// addresses) and copies registers straight into the swizzled rows: no conversion, no bounds logic, no dependent
-// address arithmetic.  The fp32 gather above is latency-bound (7 dependent batches of 11 strided loads per pixel:
-// 0.36 ms for RetinaNet-800 B=16 against ~0.05 ms of traffic).
+// H4 variant (7x7 / stride 2 only): the image arrives as mean-subtracted fp16 RGBX ([B][H+2P][W+2P][4], zero border,
+// written by odt_pack_input_rgbx).  A filter row of an output pixel is then ONE contiguous, aligned span of the image
+// (8 pixels = 64 bytes = four 16-byte chunks, the eighth tap has zero weights), so a producer thread issues all of its
+// loads back to back (28 LDG.128, adjacent lanes on adjacent addresses) and copies registers straight into the
+// swizzled rows: no conversion, no bounds logic, no dependent address arithmetic.  The fp32 gather above is
+// latency-bound (7 dependent batches of 11 strided loads per pixel: 0.36 ms for RetinaNet-800 B=16 against ~0.05 ms
+// of traffic).
 //
 // ref: conv1_1 SSD300.py:193-200 (+mean :52-66); YOLOv3.py:388; RetinaNet.py:260-265; FCOS.py:73-78.
 #include "epilogue.cuh"
@@ -47,7 +47,8 @@ constexpr int ST_WARP_STAGE = 32 * ST_PITCH;   // staging bytes per epilogue war
 // K extent of one im2col row: fp32 path KS*KS*3; H4 path KS rows of KSP pixels x 4 channels
 template <int KS, bool H4>
 struct StemK {
-  static constexpr int KSP = KS == 7 ? 8 : KS;                 // pixels per filter row in the H4 layout
+  static_assert(!H4 || KS == 7, "the packed-image (H4) stem is 7x7 only");
+  static constexpr int KSP = 8;                                // pixels per filter row in the H4 layout
   static constexpr int KREAL = H4 ? KS * KSP * 4 : KS * KS * 3;
   static constexpr int KSTEPS = (KREAL + 15) / 16;
   static constexpr int NBLK = (KSTEPS * 16 + 63) / 64;
@@ -146,44 +147,20 @@ __global__ void __launch_bounds__(ST_THREADS)
         const __half* src = reinterpret_cast<const __half*>(img_any) +
                             (((long long)b * g.iph + (iy0 + g.in_pad)) * g.ipw + (ix0 + g.in_pad)) * 4;
         const int rs = g.ipw * 4;  // halves per padded image row
-        if (KS == 7) {
-          uint4 q[KS][4];
+        uint4 q[KS][4];
 #pragma unroll
-          for (int r = 0; r < KS; ++r) {
-            const uint4* p4 = reinterpret_cast<const uint4*>(src + (long long)r * rs);
+        for (int r = 0; r < KS; ++r) {
+          const uint4* p4 = reinterpret_cast<const uint4*>(src + (long long)r * rs);
 #pragma unroll
-            for (int c = 0; c < 4; ++c) q[r][c] = __ldg(p4 + c);
-          }
-          mbar_wait(empty_bar(stage), phase ^ 1u);
+          for (int c = 0; c < 4; ++c) q[r][c] = __ldg(p4 + c);
+        }
+        mbar_wait(empty_bar(stage), phase ^ 1u);
 #pragma unroll
-          for (int r = 0; r < KS; ++r) {
+        for (int r = 0; r < KS; ++r) {
 #pragma unroll
-            for (int c = 0; c < 4; ++c) {
-              const int id = 4 * r + c, blk = id >> 3, cc = id & 7;
-              *reinterpret_cast<uint4*>(arow + blk * (128 * 128) + ((cc ^ (t & 7)) << 4)) = q[r][c];
-            }
-          }
-        } else {
-          // 3 pixels x 4 channels = 6 words per filter row, 8-byte aligned
-          uint32_t v[NCHUNK * 4];
-#pragma unroll
-          for (int i = 0; i < NCHUNK * 4; ++i) v[i] = 0u;
-#pragma unroll
-          for (int r = 0; r < KS; ++r) {
-            const uint2* p2 = reinterpret_cast<const uint2*>(src + (long long)r * rs);
-#pragma unroll
-            for (int c = 0; c < KS; ++c) {
-              const uint2 w2 = __ldg(p2 + c);
-              v[(r * KS + c) * 2] = w2.x;
-              v[(r * KS + c) * 2 + 1] = w2.y;
-            }
-          }
-          mbar_wait(empty_bar(stage), phase ^ 1u);
-#pragma unroll
-          for (int c = 0; c < NCHUNK; ++c) {
-            const int blk = c >> 3, cc = c & 7;
-            *reinterpret_cast<uint4*>(arow + blk * (128 * 128) + ((cc ^ (t & 7)) << 4)) =
-                make_uint4(v[4 * c], v[4 * c + 1], v[4 * c + 2], v[4 * c + 3]);
+          for (int c = 0; c < 4; ++c) {
+            const int id = 4 * r + c, blk = id >> 3, cc = id & 7;
+            *reinterpret_cast<uint4*>(arow + blk * (128 * 128) + ((cc ^ (t & 7)) << 4)) = q[r][c];
           }
         }
         fence_proxy_async_smem();
@@ -433,8 +410,8 @@ int odt_conv2d_stem_tc_try(const float* images, const float* mean3_host, const v
   return ODT_OK;
 }
 
-// Stem on the packed fp16 RGBX image (see the header comment).  `rgbx`: [B][H+2P][W+2P][4] fp16 with a zero border,
-// P = p->in_halo: 1 for the 3x3 / stride-1 stems, 4 for the 7x7 / stride-2 stem (even W, even left pad).
+// 7x7 / stride-2 stem on the packed fp16 RGBX image (see the header comment).  `rgbx`: [B][H+2P][W+2P][4] fp16 with a
+// zero border, P = p->in_halo = 4 (even W, even left pad).
 extern "C" int odt_conv2d_stem_rgbx(const void* rgbx, const void* weights, const odt_conv_params* p, void* stream) {
   int rc0 = check_conv_params(p);
   if (rc0) return rc0;
@@ -443,17 +420,13 @@ extern "C" int odt_conv2d_stem_rgbx(const void* rgbx, const void* weights, const
                   p->dil == 1 && p->in_ld == 4 && p->Cin == 3 && p->out0_dtype == ODT_F16 &&
                   p->out0_pool == 0 && ((uintptr_t)p->out0 % 16) == 0 && p->out0_pix_stride % 8 == 0 &&
                   p->out0_pix_stride >= p->Cout && p->out0_img_stride % 8 == 0 && ((uintptr_t)rgbx % 16) == 0;
-  int variant = 0;
-  if (ok && p->R == 3 && p->stride == 1 && p->Cout == 64 && p->in_halo == 1 && p->pad_t == 1 && p->pad_l == 1) variant = 1;
-  if (ok && p->R == 3 && p->stride == 1 && p->Cout == 32 && p->in_halo == 1 && p->pad_t == 1 && p->pad_l == 1) variant = 2;
-  // 7x7 / 2: up to 16 real outputs.  The kernel computes and stores 16 channels per pixel, so the filter bank, scale and
-  // shift must hold 16 rows (Cout_pad), zero past Cout, and the output row must have room for 16.
-  if (ok && p->R == 7 && p->stride == 2 && p->Cout <= 16 && p->Cout_pad == 16 && p->out0_pix_stride >= 16 &&
-      p->in_halo == 4 && (p->W & 1) == 0 && (p->pad_l & 1) == 0 && p->pad_t <= 4 && p->pad_l <= 4 &&
-      // the 8-pixel row window and the 7 filter rows of the last output pixel stay inside the padded image
-      (p->OW - 1) * 2 - p->pad_l + 7 <= p->W - 1 + 4 && (p->OH - 1) * 2 - p->pad_t + 6 <= p->H - 1 + 4)
-    variant = 3;
-  if (!variant) return ODT_ERR_UNSUPPORTED;
+  // up to 16 real outputs.  The kernel computes and stores 16 channels per pixel, so the filter bank, scale and shift
+  // must hold 16 rows (Cout_pad), zero past Cout, and the output row must have room for 16.
+  if (!(ok && p->R == 7 && p->stride == 2 && p->Cout <= 16 && p->Cout_pad == 16 && p->out0_pix_stride >= 16 &&
+        p->in_halo == 4 && (p->W & 1) == 0 && (p->pad_l & 1) == 0 && p->pad_t <= 4 && p->pad_l <= 4 &&
+        // the 8-pixel row window and the 7 filter rows of the last output pixel stay inside the padded image
+        (p->OW - 1) * 2 - p->pad_l + 7 <= p->W - 1 + 4 && (p->OH - 1) * 2 - p->pad_t + 6 <= p->H - 1 + 4))
+    return ODT_ERR_UNSUPPORTED;
   StemGeom g;
   g.B = p->B; g.H = p->H; g.W = p->W; g.OH = p->OH; g.OW = p->OW; g.ohw = p->OH * p->OW;
   g.pad_t = p->pad_t; g.pad_l = p->pad_l; g.w_ld = p->w_ld;
@@ -467,10 +440,7 @@ extern "C" int odt_conv2d_stem_rgbx(const void* rgbx, const void* weights, const
   g.iph = p->H + 2 * p->in_halo;
   Epi e = make_epi(*p);
   cudaStream_t st = (cudaStream_t)stream;
-  int rc = ODT_OK;
-  if (variant == 1) rc = launch_stem_tc<64, 3, 1, true>(rgbx, weights, g, e, st);
-  if (variant == 2) rc = launch_stem_tc<32, 3, 1, true>(rgbx, weights, g, e, st);
-  if (variant == 3) rc = launch_stem_tc<16, 7, 2, true>(rgbx, weights, g, e, st);
+  const int rc = launch_stem_tc<16, 7, 2, true>(rgbx, weights, g, e, st);
   if (rc) return rc;
   ODT_LAUNCH_OK();
   return ODT_OK;

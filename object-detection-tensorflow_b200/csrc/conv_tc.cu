@@ -108,9 +108,9 @@ struct TcGeom {
   // flat modes with a small filter bank: all 9*cchunks weight tiles [BN x 64] stay resident
   // in shared memory (loaded once per CTA); the pipeline stages then carry activations only
   int bres;
-  int klast;        // 16-deep K steps of the LAST 64-channel chunk that hold real input channels (1..4); with
-                    // ODT_TC_KSKIP=1 the all-zero steps of a thin layer (Cin = 7..48 padded to 64 on both
-                    // operands) are not issued (warpgroup-uniform branch); 4 otherwise
+  int klast;        // 16-deep K steps of the LAST 64-channel chunk that hold real input channels (1..4): the
+                    // all-zero steps of a thin layer (Cin = 7..48 padded to 64 on both operands) are not issued
+                    // (warpgroup-uniform branch)
 };
 constexpr int TC_FLAT_ROWS = 136;                    // 128 + 2 neighbours, padded to 1024 B
 constexpr int TC_FLAT_A_BYTES = TC_FLAT_ROWS * 128;  // 17408
@@ -785,11 +785,11 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
     const int rt = conv_pw_try(in, weights, p, stream);
     if (rt != ODT_ERR_UNSUPPORTED) return rt;
   }
-  if (thin_mode()) {  // opt-in: very thin layers on CUDA cores with sector-granular traffic (conv_thin.cu)
+  if (thin_mode()) {  // very thin layers on CUDA cores with sector-granular traffic (conv_thin.cu)
     const int rt = conv_thin_try(in, weights, p, stream);
     if (rt != ODT_ERR_UNSUPPORTED) return rt;
   }
-  if (tapn_mode()) {  // opt-in: narrow 3x3 layers with the horizontal taps folded into N (conv_tapn.cu)
+  if (tapn_mode()) {  // narrow 3x3 layers with the horizontal taps folded into N (conv_tapn.cu)
     const int rt = conv_tapn_try(in, weights, p, stream);
     if (rt != ODT_ERR_UNSUPPORTED) return rt;
   }
@@ -811,10 +811,8 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
   g.lower_h = -p->pad_t + ih;
   g.cchunks = p->in_ld / 64;
   {
-    // ODT_TC_KSKIP (default on, carried over from the previous target, not re-measured on the H100): with the knob
-    // off every step is issued
     const int rem = p->Cin - (g.cchunks - 1) * TC_BK;  // real channels in the last chunk
-    g.klast = !kskip_enabled() || rem >= TC_BK ? TC_BK / 16 : (rem <= 0 ? 1 : (rem + 15) / 16);
+    g.klast = rem >= TC_BK ? TC_BK / 16 : (rem <= 0 ? 1 : (rem + 15) / 16);
   }
   g.out_halo = p->out0_halo;
   g.H = p->H;
@@ -836,7 +834,7 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
                       ((uintptr_t)p->out0 & 15) == 0 && p->out0_pix_stride >= p->Cout_pad,
                   "fused pooling: out0 alignment / channel stride");
   }
-  g.flat = p->out0_pool ? 2 : ((flat_shape && flat_enabled()) ? 1 : 0);
+  g.flat = p->out0_pool ? 2 : (flat_shape ? 1 : 0);
   g.a_tx = TC_A_BYTES;
   int stage_bytes;
   if (g.flat == 2) {
@@ -875,7 +873,7 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
   // small filter banks of the flat modes stay resident in shared memory if at least three
   // activation stages still fit beside them
   const long long wres = 9ll * g.cchunks * g.BN * 128;
-  if (g.flat && wres_enabled() && g.BN >= 128 && wres + 3 * TC_FLAT_A_BYTES + fixed_bytes <= TC_SMEM_LIMIT) {
+  if (g.flat && g.BN >= 128 && wres + 3 * TC_FLAT_A_BYTES + fixed_bytes <= TC_SMEM_LIMIT) {
     g.bres = 1;
     g.b_bytes = 0;
     stage_bytes = g.a_bytes;

@@ -386,7 +386,7 @@ int conv_swap_try(const void* in, const void* weights, const odt_conv_params* p,
   g.cchunks = p->in_ld / 64;
   {
     const int rem = p->Cin - (g.cchunks - 1) * SW_BK;  // real channels in the last chunk (see TcGeom::klast)
-    g.klast = !kskip_enabled() || rem >= SW_BK ? SW_BK / 16 : (rem <= 0 ? 1 : (rem + 15) / 16);
+    g.klast = rem >= SW_BK ? SW_BK / 16 : (rem <= 0 ? 1 : (rem + 15) / 16);
   }
   g.halves = p->Cout_pad / SW_CO;
   g.num_ptiles = (int)plan.ptiles;
@@ -406,7 +406,7 @@ int conv_swap_try(const void* in, const void* weights, const odt_conv_params* p,
     g.a_tx = (g.XB + 2) * g.RP * 128;
   }
   const long long wres = 9ll * g.cchunks * SW_W_BYTES;
-  g.bres = g.halves == 1 && wres_enabled() && wres + 3 * SW_SLAB_BYTES + SW_FIXED_BYTES <= SW_SMEM_LIMIT;
+  g.bres = g.halves == 1 && wres + 3 * SW_SLAB_BYTES + SW_FIXED_BYTES <= SW_SMEM_LIMIT;
   const int stage_bytes = SW_SLAB_BYTES + (g.bres ? 0 : 3 * SW_W_BYTES);
   int stages = (SW_SMEM_LIMIT - SW_FIXED_BYTES - (g.bres ? (int)wres : 0)) / stage_bytes;
   if (stages > SW_MAX_STAGES) stages = SW_MAX_STAGES;

@@ -776,9 +776,8 @@ extern "C" int odt_maxpool(const void* in, void* out, int dtype, int B, int H, i
   {
     const long long work = (long long)B * OH * OW * (C / 8);
     const bool shape = (k == 2 && stride == 2) || (k == 3 && stride == 1);
-    const char* env = getenv("ODT_POOL_FAST");  // 0: the generic kernel (A/B)
     if (dtype == ODT_F16 && shape && can_vec(in, out, C, ld, 8, 2) && work < (1ll << 31) - 256 &&
-        (long long)B * (H + 2) * (W + 2) < (1ll << 31) && !(env && env[0] == '0')) {
+        (long long)B * (H + 2) * (W + 2) < (1ll << 31)) {
       const int blocks = (int)((work + 255) / 256);
       const __half* ip = (const __half*)in;
       __half* op = (__half*)out;

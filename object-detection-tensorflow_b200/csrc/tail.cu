@@ -10,7 +10,6 @@
 // Reference call sites restated here (never copied): SSD300.py:157-190,323-343;
 // RetinaNet.py:224-256,328-355; YOLOv3.py:320-368,419-433; FCOS.py:130-150,197-264.
 #include <stdlib.h>
-#include <string.h>
 
 #include "tail_common.cuh"
 #include "tc_ptx.cuh"
@@ -350,7 +349,7 @@ __global__ void __launch_bounds__(kNmsThreads)
                          int* __restrict__ det_anchor, int* __restrict__ det_count,
                          int* __restrict__ scratch, int* __restrict__ work,
                          int* __restrict__ status, float4* __restrict__ box_pool,
-                         long long box_pool_entries, long long det_img_stride, int adapt) {
+                         long long box_pool_entries, long long det_img_stride) {
   pdl_launch_dependents();
   const odt_tail_params& p = tp.p;
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -500,8 +499,8 @@ __global__ void __launch_bounds__(kNmsThreads)
   // Greedy rounds.  A round costs every participating warp ~150 instructions whatever the list length, and with all
   // lists of a batch resident (SSD300 B=64: 1 280 blocks, 8 per SM) the kernel is bound by that instruction count:
   // only as many warps as the list can feed (64 candidates each, at least 2) take part; the others wait at the
-  // block barrier after the loop.  adapt == 0 (ODT_NMS_ADAPT=0): all 8 warps, as in round 1.
-  const int nw = adapt ? min(kNmsThreads / 32, max(2, (cnt + 63) / 64)) : kNmsThreads / 32;
+  // block barrier after the loop.
+  const int nw = min(kNmsThreads / 32, max(2, (cnt + 63) / 64));
   const int nthr = nw * 32;
   nsel = 0;
   if (tid < nthr) {
@@ -660,11 +659,9 @@ extern "C" int odt_decode_candidates(const float* head, const odt_tail_params* p
   tp.p = *p;
   long long rows = (long long)B * p->N;
   long long groups = (rows + 31) / 32;
-  // 25-float rows (num_fg = 20, every family): 8 warps per CTA.  Two builds per kind (A/B by ODT_DECODE_CFG): "3x2" =
-  // 3 CTAs / SM with 2 stages per warp (24 warps x 1 group in flight ahead, the default), "2x4" = 2 CTAs / SM with 4
-  // stages (16 warps x 3 groups ahead: more bytes in flight per SM, fewer warps to hide instruction latency).  The
-  // default is carried over from the previous target; it has not been re-measured on the H100.
-  // Other class counts (YOLOv3 / FCOS): 4 warps x 2 stages, as many CTAs per SM as their staging allows.
+  // 25-float rows (num_fg = 20, every family): 8 warps per CTA, 3 CTAs / SM with 2 stages per warp (24 warps x 1
+  // group in flight ahead).  Other class counts (YOLOv3 / FCOS): 4 warps x 2 stages, as many CTAs per SM as their
+  // staging allows.
   const bool wide = p->num_fg != 20;
   const int warps = wide ? kDecodeWarpsWide : kDecodeWarps;
   int blocks = (int)((groups + warps - 1) / warps);
@@ -673,11 +670,10 @@ extern "C" int odt_decode_candidates(const float* head, const odt_tail_params* p
     const long long smem = decode_smem_bytes(kDecodeWarpsWide, 2, row_floats(p->num_fg));
     per_sm = (int)(2 * ((228 * 1024) / (smem + 1024)));  // two waves of the CTAs that fit (1 KB reserved per CTA)
   }
+  // a smaller grid makes every warp iterate several times at sizes a test can afford
   if (const char* e = getenv("ODT_DECODE_BLOCKS_PER_SM")) per_sm = atoi(e) > 0 ? atoi(e) : per_sm;
   int maxb = kNumSMs * per_sm;
   if (blocks > maxb) blocks = maxb;
-  int deep = 0;
-  if (const char* e = getenv("ODT_DECODE_CFG")) deep = strcmp(e, "2x4") == 0 ? 1 : 0;
 #define ODT_DECODE_LAUNCH(KIND_, WARPS_, OCC_, ST_, NFG_, SMEM_MAX_)                                               \
   do {                                                                                                           \
     static bool attr_done = false;                                                                               \
@@ -690,18 +686,16 @@ extern "C" int odt_decode_candidates(const float* head, const odt_tail_params* p
         <<<blocks, (WARPS_) * 32, decode_smem_bytes(WARPS_, ST_, row_floats(p->num_fg)), st>>>(                  \
             head, tp, rows, cand_keys, cand_count);                                                              \
   } while (0)
-#define ODT_DECODE_LAUNCH20(KIND_, OCC_, ST_) \
-  ODT_DECODE_LAUNCH(KIND_, kDecodeWarps, OCC_, ST_, 20, decode_smem_bytes(kDecodeWarps, ST_, row_floats(20)))
+#define ODT_DECODE_LAUNCH20(KIND_) \
+  ODT_DECODE_LAUNCH(KIND_, kDecodeWarps, 3, 2, 20, decode_smem_bytes(kDecodeWarps, 2, row_floats(20)))
 #define ODT_DECODE_LAUNCH_WIDE(KIND_) \
   ODT_DECODE_LAUNCH(KIND_, kDecodeWarpsWide, 1, 2, 0, decode_smem_bytes(kDecodeWarpsWide, 2, row_floats(kMaxFg)))
   if (p->kind == ODT_DECODE_SSD) {
-    if (deep) ODT_DECODE_LAUNCH20(ODT_DECODE_SSD, 2, 4); else ODT_DECODE_LAUNCH20(ODT_DECODE_SSD, 3, 2);
+    ODT_DECODE_LAUNCH20(ODT_DECODE_SSD);
   } else if (p->kind == ODT_DECODE_YOLO3) {
-    if (wide) ODT_DECODE_LAUNCH_WIDE(ODT_DECODE_YOLO3);
-    else if (deep) ODT_DECODE_LAUNCH20(ODT_DECODE_YOLO3, 2, 4); else ODT_DECODE_LAUNCH20(ODT_DECODE_YOLO3, 3, 2);
+    if (wide) ODT_DECODE_LAUNCH_WIDE(ODT_DECODE_YOLO3); else ODT_DECODE_LAUNCH20(ODT_DECODE_YOLO3);
   } else {
-    if (wide) ODT_DECODE_LAUNCH_WIDE(ODT_DECODE_FCOS);
-    else if (deep) ODT_DECODE_LAUNCH20(ODT_DECODE_FCOS, 2, 4); else ODT_DECODE_LAUNCH20(ODT_DECODE_FCOS, 3, 2);
+    if (wide) ODT_DECODE_LAUNCH_WIDE(ODT_DECODE_FCOS); else ODT_DECODE_LAUNCH20(ODT_DECODE_FCOS);
   }
 #undef ODT_DECODE_LAUNCH_WIDE
 #undef ODT_DECODE_LAUNCH20
@@ -752,10 +746,9 @@ extern "C" int odt_nms_per_class(const float* head, const odt_tail_params* p, in
   const long long dense = (long long)p->nms_classes * p->max_boxes * 6;
   if (dets_img_stride == 0) dets_img_stride = dense;
   ODT_CHECK_ARG(dets_img_stride >= dense, "dets_img_stride smaller than nms_classes*max_boxes*6");
-  const char* ad = getenv("ODT_NMS_ADAPT");  // 0: every round uses all 8 warps of the block (A/B against round 1)
   nms_per_class_kernel<<<grid, kNmsThreads, sizeof(NmsSmem), st>>>(
       head, tp, B, cand_keys, cand_count, dets, det_anchor, det_count, sel_scratch, work, status,
-      reinterpret_cast<float4*>(box_pool), box_pool ? box_pool_entries : 0, dets_img_stride, !(ad && ad[0] == '0'));
+      reinterpret_cast<float4*>(box_pool), box_pool ? box_pool_entries : 0, dets_img_stride);
   ODT_LAUNCH_OK();
   return ODT_OK;
 }

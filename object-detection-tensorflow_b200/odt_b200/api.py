@@ -257,6 +257,7 @@ class _Detector:
             ev.record(main)
         prefetch(cur, 0)
         i, pending = 0, None
+        # ODT_PIPELINE=0: one graph per batch (bench.py reads the same switch for its own loop)
         pipelined = net.graph is not None and os.environ.get("ODT_PIPELINE", "1") != "0"
         if pipelined:
             # two-stage pipeline (engine.Net.run_pipelined): decode + NMS + gather + read-back of batch i on the tail

@@ -42,6 +42,7 @@ def cabi_ctx():
     then go through torch.distributed."""
     if _CTX["ctx"] is not None or _CTX["failed"]:
         return _CTX["ctx"]
+    # ODT_COLLECTIVES=torch is the functional fallback for hosts where NCCL cannot be loaded through the C ABI
     if (os.environ.get("ODT_COLLECTIVES", "cabi") == "torch" or not torch.cuda.is_available()
             or not dist.is_initialized() or dist.get_world_size() == 1):
         _CTX["failed"] = True

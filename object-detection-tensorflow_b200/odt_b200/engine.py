@@ -204,18 +204,12 @@ class ConvOp(Op):
             p.out2_halo = t.halo
         self.p = p
         self.flops = 2 * B * OH * OW * cout * R * S * cin
-        # stems: the tensor-core variants read a packed fp16 RGBX copy of the image (mean subtracted, zero border of
-        # `rgbx` pixels) so that every filter row is one aligned span -- see csrc/conv_stem_tc.cu
+        # the 7x7 / stride-2 stem reads a packed fp16 RGBX copy of the image (mean subtracted, zero border of `rgbx`
+        # pixels) so that every filter row is one aligned span -- see csrc/conv_stem_tc.cu
         self.rgbx = 0
         if (self.is_image and f16 and net.allow_tc and self.pre is None and self.head is None
-                and os.environ.get("ODT_STEM_RGBX", "1") != "0"):
-            # the 7x7 / stride-2 stem takes the packed image by default, the 3x3 / stride-1 stems only with
-            # ODT_STEM_RGBX=2 (a choice carried over from the previous target, not re-measured on the H100)
-            force3 = os.environ.get("ODT_STEM_RGBX") == "2"
-            if (R, self.stride, cout) in ((3, 1, 64), (3, 1, 32)) and force3:
-                self.rgbx = 1
-            elif (R, self.stride) == (7, 2) and cout <= 16 and Wd % 2 == 0 and pl % 2 == 0 and pl <= 4 and pt <= 4:
-                self.rgbx = 4
+                and (R, self.stride) == (7, 2) and cout <= 16 and Wd % 2 == 0 and pl % 2 == 0 and pl <= 4 and pt <= 4):
+            self.rgbx = 4
         if self.rgbx == 4 and cout < 16:
             # the packed 7x7 stem computes 16 outputs (RetinaNet's basic variant has 7): filter rows, BN scale and
             # shift are zero past `cout`, so the pad lanes its whole-sector store writes stay zero
@@ -354,7 +348,7 @@ class GroupNormActOp(Op):
         self.beta = torch.from_numpy(np.asarray(net.weights[self.gn + "/beta"], np.float32)).to(dev)
         self.stats = torch.zeros(self.x.B * self.groups * 6, dtype=torch.float32, device=dev)
         n = self.workspace_doubles(net)
-        self.two_launch = net.gn_arena is not None and n > 0
+        self.two_launch = n > 0
         if self.two_launch:
             self.acc = net.gn_take(n)
 
@@ -440,6 +434,7 @@ class Net:
         self.levels = []    # (H, W, A) per head level, in candidate order
         self.tail = None
         self.mean3 = (C.c_float * 3)(123.68, 116.779, 103.979)  # ref SSD300.py:55
+        # ODT_HALO=0 keeps every tensor dense: the end-to-end reference the halo layouts are tested against
         self.use_halo = os.environ.get("ODT_HALO", "1") != "0"
         self.weights = None
         self.graph = None
@@ -575,7 +570,7 @@ class Net:
                 # second pre-activation of the same tensor: tensor-core convs (third epilogue output) and pools
                 second = (not ok and isinstance(q, ConvOp) and q.head is None and q.pre is not None
                           and q.pre2 is None and not q.is_image and self.precision == "fp16" and self.allow_tc
-                          and q.x.ld % 64 == 0 and os.environ.get("ODT_FUSE_PRE2", "1") != "0")
+                          and q.x.ld % 64 == 0)
                 second = second or (not ok and isinstance(q, PoolOp) and q.pre is not None and q.pre2 is None)
                 if ok or second:
                     if ok:
@@ -610,7 +605,7 @@ class Net:
                     # fused second / third outputs: the tensor-core convolutions (conv_tc / conv_tapn / conv_thin
                     # epilogues) and the fused pool write them in the halo layout too; other producers stay dense
                     can = ((isinstance(op, ConvOp) and not op.is_image and op.head is None and op.x.ld % 64 == 0)
-                           or isinstance(op, PoolOp)) and os.environ.get("ODT_HALO_AUX", "1") != "0"
+                           or isinstance(op, PoolOp))
                     producer[id(pr[2])] = "fused" if can else None
         for t in self.acts:
             prod = producer.get(id(t))
@@ -645,7 +640,7 @@ class Net:
     def fuse_pools(self):
         """Fold a 2x2/2 max-pool into the epilogue of the halo-flat 3x3 conv that feeds it
         (a4: SSD300.py:539-547 after conv1_2 / conv2_2): the unpooled tensor is never stored."""
-        if self.precision != "fp16" or not self.allow_tc or os.environ.get("ODT_POOL_FUSE", "1") == "0":
+        if self.precision != "fp16" or not self.allow_tc:
             return
         readers, producer = {}, {}
         for op in self.ops:
@@ -699,8 +694,7 @@ class Net:
         # one fp64 arena for the workspaces of every GroupNorm (per-slice moments, statistics, arrival counters),
         # zeroed once per forward
         n_gn = sum(op.workspace_doubles(self) for op in self.ops if isinstance(op, GroupNormActOp))
-        use_arena = n_gn > 0 and os.environ.get("ODT_GN_FUSED", "1") != "0"
-        self.gn_arena = torch.zeros(n_gn, dtype=torch.float64, device=dev) if use_arena else None
+        self.gn_arena = torch.zeros(n_gn, dtype=torch.float64, device=dev) if n_gn > 0 else None
         self._gn_used = 0
         for op in self.ops:
             op.prepare(self)
@@ -728,10 +722,8 @@ class Net:
     # Independent branches of the op list (FPN levels, the two towers, SSD/YOLO heads
     # next to the rest of the backbone) are captured on separate stream lanes so that
     # launches with fewer CTAs than SMs overlap inside the graph.
-    def plan_lanes(self, max_lanes=None):
+    def plan_lanes(self, max_lanes=12):
         """Dataflow -> (lane of every op, cross-lane waits).  Pure host logic."""
-        if max_lanes is None:
-            max_lanes = int(os.environ.get("ODT_STREAMS", "12"))
         producer, deps = {}, []
         for i, op in enumerate(self.ops):
             deps.append(sorted({producer[id(t)] for t in op.reads if id(t) in producer}))

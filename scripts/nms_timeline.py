@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-round timeline of block (0, 0) of nms_per_class_kernel (debug build, -DODT_NMS_TIMELINE): where a greedy
 round's latency goes (round top -> arg-max barrier -> suppression barrier), on one model's real head rows.
-Also times the kernel (CUDA graph, 50 replays) with ODT_NMS_ADAPT=0 / 1.
+Also times the kernel (CUDA graph, 50 replays).
 usage (on a GPU box): nms_timeline.py model batch"""
 import ctypes as C
 import os
@@ -60,48 +60,46 @@ def main():
     lib.odt_debug_nms_timeline.restype = C.c_int
     lib.odt_debug_nms_timeline.argtypes = [C.c_void_p, C.c_int]
     cap = 4096
-    for adapt in ("0", "1"):
-        os.environ["ODT_NMS_ADAPT"] = adapt
-        for _ in range(3):
-            decode(); nms()
-        torch.cuda.synchronize()
-        buf = torch.zeros(2 * cap, dtype=torch.int64, device="cuda")
-        L.check(lib.odt_debug_nms_timeline(buf.data_ptr(), cap), "timeline")
+    for _ in range(3):
         decode(); nms()
-        torch.cuda.synchronize()
-        L.check(lib.odt_debug_nms_timeline(None, 0), "timeline off")
-        raw = buf.cpu().numpy().view(np.uint64).reshape(-1, 2)
-        raw = raw[raw[:, 0] != 0]
-        ev = (raw[:, 1] >> np.uint64(32)).astype(int)
-        rnd = (raw[:, 1] & np.uint64(0xFFFFFFFF)).astype(int)
-        t0 = int(raw[:, 0].min()) if len(raw) else 0
-        print("-- ODT_NMS_ADAPT=%s: block (0,0), clk since its first stamp (round top / after arg-max barrier / after suppression barrier)" % adapt)
-        rows = {}
-        for (clk, _), e, r in zip(raw, ev, rnd):
-            rows.setdefault((r, e), int(clk) - t0)
-        rounds = sorted({r for r, _ in rows})
-        prev = None
-        for r in rounds:
-            a, b, c = rows.get((r, 0)), rows.get((r, 1)), rows.get((r + 1, 2))
-            line = "round %2d: top %7s  argmax +%5s  suppress +%5s" % (
-                r, a, (b - a) if (a is not None and b is not None) else "-", (c - b) if (b is not None and c is not None) else "-")
-            if prev is not None and a is not None:
-                line += "   (round %d total %d clk)" % (r - 1, a - prev)
-            prev = a
-            print(line)
-        # warm graph timing of the NMS launch alone
-        g = torch.cuda.CUDAGraph()
-        decode()
-        torch.cuda.synchronize()
-        with torch.cuda.graph(g):
-            for _ in range(50):
-                nms()
-        g.replay()
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record(); g.replay(); e1.record()
-        torch.cuda.synchronize()
-        print("   nms (2 memsets + kernel), graph of 50: %.2f us per launch" % (e0.elapsed_time(e1) / 50 * 1e3))
+    torch.cuda.synchronize()
+    buf = torch.zeros(2 * cap, dtype=torch.int64, device="cuda")
+    L.check(lib.odt_debug_nms_timeline(buf.data_ptr(), cap), "timeline")
+    decode(); nms()
+    torch.cuda.synchronize()
+    L.check(lib.odt_debug_nms_timeline(None, 0), "timeline off")
+    raw = buf.cpu().numpy().view(np.uint64).reshape(-1, 2)
+    raw = raw[raw[:, 0] != 0]
+    ev = (raw[:, 1] >> np.uint64(32)).astype(int)
+    rnd = (raw[:, 1] & np.uint64(0xFFFFFFFF)).astype(int)
+    t0 = int(raw[:, 0].min()) if len(raw) else 0
+    print("-- block (0,0), clk since its first stamp (round top / after arg-max barrier / after suppression barrier)")
+    rows = {}
+    for (clk, _), e, r in zip(raw, ev, rnd):
+        rows.setdefault((r, e), int(clk) - t0)
+    rounds = sorted({r for r, _ in rows})
+    prev = None
+    for r in rounds:
+        a, b, c = rows.get((r, 0)), rows.get((r, 1)), rows.get((r + 1, 2))
+        line = "round %2d: top %7s  argmax +%5s  suppress +%5s" % (
+            r, a, (b - a) if (a is not None and b is not None) else "-", (c - b) if (b is not None and c is not None) else "-")
+        if prev is not None and a is not None:
+            line += "   (round %d total %d clk)" % (r - 1, a - prev)
+        prev = a
+        print(line)
+    # warm graph timing of the NMS launch alone
+    g = torch.cuda.CUDAGraph()
+    decode()
+    torch.cuda.synchronize()
+    with torch.cuda.graph(g):
+        for _ in range(50):
+            nms()
+    g.replay()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(); g.replay(); e1.record()
+    torch.cuda.synchronize()
+    print("   nms (2 memsets + kernel), graph of 50: %.2f us per launch" % (e0.elapsed_time(e1) / 50 * 1e3))
 
 
 if __name__ == "__main__":

@@ -10,7 +10,6 @@
 
 namespace odt {
 int pw_mode() { return 2; }
-bool pdl_enabled() { return false; }
 void set_error(const char*, ...) {}
 
 template <int COT>

@@ -31,8 +31,8 @@ CASES = {
     "residual_out1_out2": ((8, 75, 75, 128, 256, 3, 1, 1), {"residual": True, "pre": True, "pre2": True}, {}),
     # thin Cin with K-step skipping (1 of 4 and 1 of 4 / 3 of 4 steps issued)
     "kskip_flat": ((8, 64, 64, 16, 28, 3, 1, 1), {"in_halo": 1, "out_halo": 1},
-                   {"ODT_TC_KSKIP": "1", "ODT_TC_TAPN": "0"}),
-    "kskip_im2col": ((16, 40, 40, 100, 64, 3, 1, 1), {}, {"ODT_TC_KSKIP": "1"}),
+                   {"ODT_TC_TAPN": "0"}),
+    "kskip_im2col": ((16, 40, 40, 100, 64, 3, 1, 1), {}, {}),
 }
 
 

@@ -22,8 +22,8 @@ CASES = {
     "cout512_stride2_conv8_2": ((16, 19, 19, 256, 512, 3, 2, 1), {}, {}),                        # 13 x 2 tiles
     "halo_in_out": ((4, 38, 38, 256, 512, 3, 1, 1), {"in_halo": 1, "out_halo": 1}, {}),
     # thin last 64-channel chunk: 3 of 4 and 1 of 4 K steps issued
-    "kskip_cin100": ((8, 38, 38, 100, 256, 3, 1, 1), {}, {"ODT_TC_KSKIP": "1"}),
-    "kskip_cin16": ((8, 38, 38, 16, 512, 3, 1, 1), {}, {"ODT_TC_KSKIP": "1"}),
+    "kskip_cin100": ((8, 38, 38, 100, 256, 3, 1, 1), {}, {}),
+    "kskip_cin16": ((8, 38, 38, 16, 512, 3, 1, 1), {}, {}),
     # Cout 500 padded to 512: the last 32-column slice is partly padding, the lanes of its upper half hold none
     "ragged_cout": ((8, 38, 38, 128, 500, 3, 1, 1), {}, {}),
     # RetinaNet's pattern: residual added, two consumer pre-activations stored

@@ -397,23 +397,21 @@ def test_decode_grid_runs_several_iterations(name):
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", sorted(GRID_CASES))
 def test_decode_configs_are_bit_identical_and_exact(built, monkeypatch, name):
-    """ODT_DECODE_CFG in {3x2, 2x4} x ODT_DECODE_BLOCKS_PER_SM in {default, 1}: the sorted candidate keys and the
-    records are bit-identical across the four, and equal to the oracle."""
+    """ODT_DECODE_BLOCKS_PER_SM in {default, 1}: the sorted candidate keys and the records are bit-identical across
+    the two grids, and equal to the oracle."""
     net, B = GRID_CASES[name]
     geo = full_size(net)
     thr, mb, iou = THR[geo.kind]
     rows = make_rows(geo.kind, geo.N, batch=B, seed=33)
     h = harness(geo, rows, thr, mb, iou)
     snaps = {}
-    for cfg in ("3x2", "2x4"):
-        for per_sm in (None, "1"):
-            monkeypatch.setenv("ODT_DECODE_CFG", cfg)
-            if per_sm is None:
-                monkeypatch.delenv("ODT_DECODE_BLOCKS_PER_SM", raising=False)
-            else:
-                monkeypatch.setenv("ODT_DECODE_BLOCKS_PER_SM", per_sm)
-            snaps[(cfg, per_sm)] = Snap(h)
-    base = snaps[("3x2", None)]
+    for per_sm in (None, "1"):
+        if per_sm is None:
+            monkeypatch.delenv("ODT_DECODE_BLOCKS_PER_SM", raising=False)
+        else:
+            monkeypatch.setenv("ODT_DECODE_BLOCKS_PER_SM", per_sm)
+        snaps[per_sm] = Snap(h)
+    base = snaps[None]
     for k, s in snaps.items():
         base.assert_same(s, str(k))
     check_all(geo, rows, thr, mb, iou, base)
@@ -537,39 +535,32 @@ def test_select_restatement_edges():
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", sorted(PATH_CASES))
-def test_nms_path_matches_oracle(built, monkeypatch, name):
+def test_nms_path_matches_oracle(built, name):
     """Each case on the GPU: the path predicted from the GPU's keys is the intended one, the pool counter is
-    the summed length of the full-list lists, the records equal the oracle's; ODT_NMS_ADAPT=0 is bit-identical."""
+    the summed length of the full-list lists, the records equal the oracle's."""
     c = PATH_CASES[name]()
     geo, rows = YOLO48, c["rows"]
     h = harness(geo, rows, c["thr"], c["mb"], c["iou"])
     snap = Snap(h)
     check_all(geo, rows, c["thr"], c["mb"], c["iou"], snap, c["expect"])
-    monkeypatch.setenv("ODT_NMS_ADAPT", "0")
-    Snap(h).assert_same(snap, "ODT_NMS_ADAPT=0")
 
 
 @pytest.mark.gpu
-def test_dry_subsets_with_pool_present_partial_exhausted_and_absent(built, monkeypatch):
+def test_dry_subsets_with_pool_present_partial_exhausted_and_absent(built):
     """Six dry lists of 6 912 keys per launch: with the default pool every list caches its boxes; with room for
     2.5 lists some do and some re-decode; with room for less than one list all re-decode; without a pool the
-    counter is untouched.  All records bit-identical (ODT_NMS_ADAPT=0 too) and equal to the oracle."""
+    counter is untouched.  All records bit-identical and equal to the oracle."""
     c = _dry_subsets()
     geo, rows = YOLO48, c["rows"]
     L = geo.N
     snaps = {}
     for pool in (None, 5 * L // 2, L - 1, 0):
-        for adapt in (None, "0"):
-            if adapt is None:
-                monkeypatch.delenv("ODT_NMS_ADAPT", raising=False)
-            else:
-                monkeypatch.setenv("ODT_NMS_ADAPT", adapt)
-            snaps[(pool, adapt)] = Snap(harness(geo, rows, c["thr"], c["mb"], c["iou"], pool_cap=pool))
-    base = snaps[(None, None)]
+        snaps[pool] = Snap(harness(geo, rows, c["thr"], c["mb"], c["iou"], pool_cap=pool))
+    base = snaps[None]
     _, counter = check_all(geo, rows, c["thr"], c["mb"], c["iou"], base, c["expect"])
     assert counter == 6 * L and base.counter == counter and base.pool_entries >= counter
-    for (pool, adapt), s in snaps.items():
-        base.assert_same(s, "pool_cap=%s ODT_NMS_ADAPT=%s" % (pool, adapt))
+    for pool, s in snaps.items():
+        base.assert_same(s, "pool_cap=%s" % pool)
         if pool == 0:
             assert s.pool_entries == 0 and s.counter == 0
         elif pool is not None:
