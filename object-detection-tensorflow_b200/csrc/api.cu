@@ -59,6 +59,9 @@ extern "C" unsigned int odt_crc32c(unsigned int crc, const void* data, unsigned 
 }
 extern "C" const char* odt_last_error(void) { return odt::g_err; }
 
+// Debug only: name of the convolution kernel the last odt_conv2d_* call of this process launched.
+extern "C" const char* odt_debug_last_conv_kernel(void) { return odt::g_last_conv_kernel; }
+
 // TF SAME padding (SURVEY App. A.1): out = ceil(in/stride),
 // pad_total = max((out-1)*stride + (k-1)*dil + 1 - in, 0), before = total/2.
 extern "C" int odt_same_pad(int in, int k, int stride, int dil, int* out, int* pad_before,

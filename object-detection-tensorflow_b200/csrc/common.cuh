@@ -98,4 +98,8 @@ int swap_mode();  // ODT_TC_SWAP: narrow 3x3 halo layers (Cout_pad 64 / 128, fp1
                   // 64-cout x 256-pixel tiles of conv_tc_swap.cu
 int wide_mode();  // ODT_TC_WIDE: conv_tc's 128 x 256 im2col tile (mode 2: wherever Cout_pad % 256 == 0)
 
+// debug: name of the convolution kernel the last odt_conv2d_* call launched (a string literal; see
+// odt_debug_last_conv_kernel), so that tests can name the path a layer took without a profiler.  An inline variable:
+// one instance in the library, and a definition in any program that includes a kernel source on its own.
+inline const char* g_last_conv_kernel = "";
 }  // namespace odt

@@ -211,6 +211,10 @@ static int launch_direct(const void* in, const void* w, int dtype, const odt_con
     conv_direct_kernel<__half, STEM><<<grid, DTHREADS, 0, st>>>(in, (const __half*)w, g, e);
   else
     conv_direct_kernel<float, STEM><<<grid, DTHREADS, 0, st>>>(in, (const float*)w, g, e);
+  if (dtype == ODT_F16)
+    g_last_conv_kernel = STEM ? "conv_direct_kernel<__half,true>" : "conv_direct_kernel<__half,false>";
+  else
+    g_last_conv_kernel = STEM ? "conv_direct_kernel<float,true>" : "conv_direct_kernel<float,false>";
   return ODT_OK;
 }
 

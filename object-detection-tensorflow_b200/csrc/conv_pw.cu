@@ -353,6 +353,7 @@ int conv_pw_try(const void* in, const void* weights, const odt_conv_params* p, v
     ODT_CUDA_OK(launch_pdl(conv_pw_kernel<32>, grid, PW_THREADS, g.smem_bytes, st, inh, wh, g, e));
   ODT_LAUNCH_OK();
   ++g_pw_launches;
+  g_last_conv_kernel = cot == 8 ? "conv_pw_kernel<8>" : cot == 16 ? "conv_pw_kernel<16>" : "conv_pw_kernel<32>";
   return ODT_OK;
 }
 

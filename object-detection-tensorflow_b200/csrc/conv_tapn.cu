@@ -371,6 +371,8 @@ int conv_tapn_try(const void* in, const void* weights, const odt_conv_params* p,
                          (cudaStream_t)stream, tmA, tmB, g, make_epi(*p)));
   ODT_LAUNCH_OK();
   ++g_tapn_launches;
+  g_last_conv_kernel = g.BN == 32 ? (pool ? "conv_tapn_kernel<32,1>" : "conv_tapn_kernel<32,0>")
+                                  : (pool ? "conv_tapn_kernel<64,1>" : "conv_tapn_kernel<64,0>");
   return ODT_OK;
 }
 

@@ -586,14 +586,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
                 float x = apply_act(fmaf(v[i], ps[i], ps[P + i]), e.act);
                 const long long o0 = o0_row + pofs[i];
                 if (e.residual) x += __half2float(reinterpret_cast<const __half*>(e.residual)[o0]);
-                if (e.out0) {
-                  if (e.out0_dtype == ODT_F32) {
-                    reinterpret_cast<float*>(e.out0)[o0] = x;
-                  } else {
-                    const __half hv = __float2half_rn(x);
-                    reinterpret_cast<__half*>(e.out0)[o0] = hv;
-                    x = __half2float(hv);
-                  }
+                if (e.out0 && e.out0_dtype == ODT_F32) {
+                  reinterpret_cast<float*>(e.out0)[o0] = x;
+                } else {
+                  // out1 / out2 take the rounded value, as epi_store_f16 does, whether or not out0 is stored
+                  const __half hv = __float2half_rn(x);
+                  if (e.out0) reinterpret_cast<__half*>(e.out0)[o0] = hv;
+                  x = __half2float(hv);
                 }
                 if (e.out1)
                   reinterpret_cast<__half*>(e.out1)[o1_row + n] =
@@ -980,11 +979,18 @@ extern "C" int odt_conv2d_f16_tc(const void* in, const void* weights, const odt_
         ODT_CUDA_OK(cudaFuncSetAttribute(kerns[t][b], cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_LIMIT));
     smem_set = true;
   }
+  static const char* const names[2][5] = {
+      {"conv_tc_kernel<32,false>", "conv_tc_kernel<64,false>", "conv_tc_kernel<96,false>", "conv_tc_kernel<128,false>",
+       "conv_tc_kernel<256,false>"},
+      {"conv_tc_kernel<32,true>", "conv_tc_kernel<64,true>", "conv_tc_kernel<96,true>", "conv_tc_kernel<128,true>",
+       "conv_tc_kernel<256,true>"}};
+  static_assert(TC_WIDE_BN == 256, "kernel names");
   const Kern kern = kerns[g.tma_out][g.BN > TC_MAX_BN ? 4 : g.BN / 32 - 1];
   const int num_tiles = g.num_m_tiles * g.num_n_tiles;
   ODT_CUDA_OK(launch_pdl(kern, num_tiles < kNumSMs ? num_tiles : kNumSMs, TC_THREADS, smem, st, tmA, tmB, tmO, g,
                          make_epi(*p)));
   ODT_LAUNCH_OK();
+  g_last_conv_kernel = names[g.tma_out][g.BN > TC_MAX_BN ? 4 : g.BN / 32 - 1];
   return ODT_OK;
 }
 

@@ -465,6 +465,7 @@ int conv_swap_try(const void* in, const void* weights, const odt_conv_params* p,
   ODT_CUDA_OK(launch_pdl(conv_tc_swap_kernel, g.num_ptiles < kNumSMs ? g.num_ptiles : kNumSMs, SW_THREADS, smem,
                          (cudaStream_t)stream, tmX, tmW, tmO, g, make_epi(*p)));
   ODT_LAUNCH_OK();
+  g_last_conv_kernel = "conv_tc_swap_kernel";
   return ODT_OK;
 }
 

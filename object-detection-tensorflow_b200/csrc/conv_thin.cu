@@ -131,12 +131,14 @@ __global__ void __launch_bounds__(THIN_THREADS)
 static int g_thin_launches = 0;  // debug: lets a test assert that the layer really took this path
 
 template <int KS, int CI8, int CO8>
-static int launch_thin(const void* in, const void* weights, const ThinGeom& g, const Epi& e, cudaStream_t st) {
+static int launch_thin(const void* in, const void* weights, const ThinGeom& g, const Epi& e, cudaStream_t st,
+                       const char* name) {
   const long long blocks = (g.M + THIN_THREADS - 1) / THIN_THREADS;
   conv_thin_kernel<KS, CI8, CO8><<<(unsigned)blocks, THIN_THREADS, 0, st>>>(
       reinterpret_cast<const __half*>(in), reinterpret_cast<const __half*>(weights), g, e);
   ODT_LAUNCH_OK();
   ++g_thin_launches;
+  g_last_conv_kernel = name;
   return ODT_OK;
 }
 
@@ -196,8 +198,9 @@ int conv_thin_try(const void* in, const void* weights, const odt_conv_params* p,
   if (rc) return rc;
   const Epi e = make_epi(*p);
   cudaStream_t st = (cudaStream_t)stream;
-#define ODT_THIN_CASE(KS_, CI_, CO_) \
-  if (ks == KS_ && ci8r == CI_ && co8r == CO_) return launch_thin<KS_, CI_, CO_>(in, weights, g, e, st);
+#define ODT_THIN_CASE(KS_, CI_, CO_)           \
+  if (ks == KS_ && ci8r == CI_ && co8r == CO_) \
+    return launch_thin<KS_, CI_, CO_>(in, weights, g, e, st, "conv_thin_kernel<" #KS_ "," #CI_ "," #CO_ ">");
   ODT_THIN_DISPATCH(ODT_THIN_CASE)
 #undef ODT_THIN_CASE
   return ODT_ERR_UNSUPPORTED;

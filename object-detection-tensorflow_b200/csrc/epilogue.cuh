@@ -170,7 +170,8 @@ __host__ __device__ __forceinline__ void epi_pre_f16(const uint4* x, const float
 }
 
 // The fused output of the run: v = act(acc*scale + shift) (+ the residual where e.residual is set), rounded to fp16
-// and stored to out0; out1 / out2 are computed from the ROUNDED value, which is what the consumer of out0 sees.
+// and stored to out0; out1 / out2 are computed from the ROUNDED value, which is what the consumer of out0 sees, and
+// stay the same when out0 is not stored (epi_store_one and conv_tc's scalar column path follow the same rule).
 // res(q) yields the residual's sector q of the run: a load issued right there (after the affine step, which keeps
 // the loaded values' live range short) or a value the caller loaded earlier.  o0 / o1 / o2: element offsets of the
 // run in out0 (= residual) / out1 / out2.
@@ -223,14 +224,13 @@ __host__ __device__ __forceinline__ void epi_store_one(const Epi& e, int b, int 
   const long long o0 = (long long)b * e.out0_img_stride + (long long)pix * e.out0_pix_stride +
                        regroup(e, n);
   if (e.residual) v += Elem<T>::ld(reinterpret_cast<const T*>(e.residual) + o0);
-  if (e.out0) {
-    if (e.out0_dtype == ODT_F32) {
-      reinterpret_cast<float*>(e.out0)[o0] = v;
-    } else {
-      reinterpret_cast<__half*>(e.out0)[o0] = __float2half_rn(v);
-      // the consumer of the fp16 tensor sees the rounded value
-      if (sizeof(T) == 2) v = __half2float(__float2half_rn(v));
-    }
+  if (e.out0 && e.out0_dtype == ODT_F32) {
+    reinterpret_cast<float*>(e.out0)[o0] = v;
+  } else {
+    const __half hv = __float2half_rn(v);
+    if (e.out0) reinterpret_cast<__half*>(e.out0)[o0] = hv;
+    // out1 / out2 of an fp16 layer take the rounded value, as the vector step does, whether or not out0 is stored
+    if (sizeof(T) == 2) v = __half2float(hv);
   }
   if (e.out1) {
     float s2 = e.scale2 ? ODT_LDG(e.scale2 + n) : 1.f;

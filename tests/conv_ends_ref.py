@@ -22,6 +22,27 @@ Bound, per element:  |got - ref| <= n_acc * u32 * |scale| * sum|x * w|  +  2 * u
         block then errs by at most 2 * u32 * (b + 2) * (|accumulator| + its products) <= 2 * u32 * (b + 2) * sum|x*w|
         over its prefix, and Kp / b blocks give 2 * (b + 2) / b * Kp <= 3 * Kp for b >= 4, where Kp is the K extent the
         kernel issues (k16 steps of its im2col row, zero padding included: zeros add exactly).
+
+The body convolutions (tests/test_gpu_conv.py's _conv_case, tests/test_gpu_conv_body.py) add, per path and per output:
+  * n_acc of the body kernels:
+      - conv_tc_kernel and conv_tc_swap_kernel: 3 * Kp with Kp = R*S*in_ld (the swap kernel issues the same k16 steps
+        in the same order, pixels on the other wgmma side);
+      - conv_tapn_kernel: three tap partials of Kp/3 each on the tensor core, 3 * Kp/3 * u32 * sum_s|x*w| each, then
+        p0 + p1 + p2 in two fp32 additions, at most 2 * u32 * (1 + Kp * u32) * sum|x*w| more: in all
+        (Kp + 2 + 2 * Kp * u32) * u32 * sum|x*w| <= 3 * Kp * u32 * sum|x*w| since Kp >= 16;
+      - conv_pw_kernel, conv_thin_kernel, conv_direct_kernel: fmaf chains (any order of fp32 additions is within
+        gamma_K too), K + 1 with K = R*S*Cin.
+  * Residual: v = act(acc*s + h) + r with r the fp16 (or fp32) residual: the element bound of a = act(...) above,
+    then one more fp32 rounding of the sum, u32 * (|v| + that bound).
+  * Fused 2x2/2 max-pool: the reference pools the float64 values, the bound is the window maximum of the element
+    bounds.  max is 1-Lipschitz in the infinity norm and fp16 rounding is monotone, so pooling rounded values and
+    rounding pooled values give the same result, within the largest element error of the window.
+  * out1 / out2 = act2(fmaf(v, s2, h2)) when out0 is stored: against act2(out0_got * s2 + h2) from the kernel's own
+    out0, at most one ulp of the output type (the kernel's fmaf is exact up to its one rounding, then fp16 rounds once;
+    leaky's 0.1f * t adds u32).
+  * out1 / out2 when out0 is not stored: v's bound, fp16 rounding included for fp16 layers (the kernels round v
+    before the consumer step either way), times |s2|, plus the fmaf / leaky roundings 2 * u32 * |t| and the output
+    rounding u16 * |t| + 2^-25.
 """
 import numpy as np
 import torch
@@ -58,6 +79,24 @@ def n_acc_stem_tc(k, rgbx):
 def n_acc_conv_tc(R, S, in_ld):
     """conv_tc_kernel: R*S taps of in_ld / 64 channel chunks of 64."""
     return n_acc_wgmma(R * S * in_ld)
+
+
+def n_acc_tapn(R, S, in_ld):
+    """conv_tapn_kernel: three tap partials of R*in_ld each plus two fp32 additions, within 3 * Kp (see the module
+    docstring)."""
+    kp = R * S * in_ld
+    assert kp + 2 <= n_acc_wgmma(kp)
+    return n_acc_wgmma(kp)
+
+
+def n_acc_body(kernel, R, S, Cin, in_ld):
+    """n_acc of the body-convolution kernel named `kernel` (a launched kernel's name)."""
+    if "conv_tapn_kernel" in kernel:
+        return n_acc_tapn(R, S, in_ld)
+    if "conv_tc_kernel" in kernel or "conv_tc_swap_kernel" in kernel:
+        return n_acc_conv_tc(R, S, in_ld)
+    assert any(k in kernel for k in ("conv_pw_kernel", "conv_thin_kernel", "conv_direct_kernel")), kernel
+    return n_acc_cuda_core(R, S, Cin)
 
 
 # ---- operands and reference ------------------------------------------------------------------------------------------
@@ -97,12 +136,56 @@ def reference(x, w, stride, scale, shift, act, dil=1):
     return ref, mag
 
 
-def bound(ref, mag, n_acc, out16):
+def bound(ref, mag, n_acc, out16, res=None):
+    """Element bound of act(acc * scale + shift) (+ res, the residual as the kernel reads it) against ref."""
     acc = n_acc * U32 * mag
-    b = acc + 2 * U32 * ref.abs()
+    if res is None:
+        b = acc + 2 * U32 * ref.abs()
+        e = acc
+    else:
+        b = acc + 2 * U32 * (ref - res.double()).abs()
+        b = b + U32 * (ref.abs() + b)
+        e = b
     if out16:
-        b = b + U16 * (ref.abs() + acc) + F16_HALF_SUB
+        b = b + U16 * (ref.abs() + e) + F16_HALF_SUB
     return b
+
+
+def pool2(t):
+    """2x2 / stride-2 max-pool of NHWC t (even H and W: the fused pool's SAME pads are zero)."""
+    B, H, W, Cc = t.shape
+    return t.reshape(B, H // 2, 2, W // 2, 2, Cc).amax(dim=(2, 4))
+
+
+def consumer(v, s2, h2, act2):
+    """act2(v * s2 + h2) in float64: a consumer pre-activation (out1 / out2) of the value v."""
+    return act64(v.double() * s2.double() + h2.double(), act2)
+
+
+def bound_own(t, out16):
+    """out1 / out2 against consumer() of the kernel's own stored out0: one ulp of the output type, plus leaky's
+    extra rounding."""
+    u = U16 if out16 else U32
+    return 2 * u * t.abs() + 2 * U32 * t.abs() + (2.0 ** -24 if out16 else 2.0 ** -149)
+
+
+def bound_through(t, b0, s2, out16):
+    """out1 / out2 when out0 is not stored: v's bound b0 (its fp16 rounding included) through |s2|, the fmaf and leaky
+    roundings, and the output rounding."""
+    b = b0 * s2.double().abs() + 2 * U32 * t.abs()
+    if out16:
+        b = b + U16 * (t.abs() + b) + F16_HALF_SUB
+    return b
+
+
+def ratio(got, ref, b):
+    """Worst |got - ref| / b (NaN in got counts as infinitely wrong, an exact element as 0 even where b is 0), and the
+    first element at that fraction."""
+    err = (got.double() - ref).abs()
+    r = torch.where(err == 0, torch.zeros_like(err), err / b)
+    r = torch.where(torch.isnan(r), torch.full_like(r, float("inf")), r)
+    i = int(torch.argmax(r.reshape(-1)))
+    return float(r.reshape(-1)[i]), tuple(int(a) for a in np.unravel_index(i, tuple(r.shape)))
 
 
 def worst(got, ref, mag, n_acc, out16):

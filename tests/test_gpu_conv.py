@@ -1,8 +1,7 @@
-"""GPU parity, stage (ii): convolution and glue kernels against plain fp32
-references (torch / the oracle's TF-op restatements) on the same inputs.
-Tolerances: fp16 tensor-core path -- fp16 operands are exact in both, fp32
-accumulation, fp16-rounded output => |err| <= 2e-3 * max|ref|; fp32 CUDA-core
-path => 2e-5 * max|ref| (accumulation order only)."""
+"""GPU parity, stage (ii): convolution and glue kernels on the same inputs as their references.  The body
+convolutions (_conv_case) are checked element by element against the float64 reference and per-path error bound of
+tests/conv_ends_ref.py, inside sentinel-guarded buffers; the glue kernels here against the oracle's TF-op
+restatements in fp32."""
 import ctypes as C
 import os
 
@@ -10,15 +9,58 @@ import numpy as np
 import pytest
 import torch
 
+import conv_ends_ref as R
+from gpu_harness import SENT, Guarded, interior, last_conv_kernel, mask
+
 pytestmark = pytest.mark.gpu
 
 
+class ConvResult:
+    """One _conv_case launch: the interior outputs [B, OH, OW, Cout] as float32 arrays (got, got1, got2; None where
+    the output is absent), the launched kernel's name (kernel) and the worst error over every output as a fraction of
+    its per-element bound (worst, at most 1)."""
+
+    def __init__(self, got, got1, got2, kernel, worst):
+        self.got, self.got1, self.got2, self.kernel, self.worst = got, got1, got2, kernel, worst
+
+
+def _bits(t):
+    return t.view(torch.int16 if t.dtype == torch.float16 else torch.int32)
+
+
+def _guarded_out(shape, dt, halo, off=0):
+    """A sentinel-filled output inside guard bands; a halo layout's zero ring is part of its contract."""
+    init = torch.full(shape, SENT, dtype=dt, device="cuda")
+    if halo:
+        init[mask(shape, 1)] = 0
+    return Guarded(shape, dt, off=off, fill=init)
+
+
+def _assert_write_rules(g, halo, Cout, cpad, what):
+    """Every real interior element written; the halo ring still +0; channels in [Cout, cpad) untouched or +0; channels
+    >= cpad and everything outside the tensor untouched."""
+    g.assert_outside_untouched()
+    t, init = g.t, g.initial()
+    if halo:
+        assert not bool(_bits(t[mask(t.shape, 1)]).ne(0).any()), "%s: halo written" % what
+    inner, was = interior(t, halo), interior(init, halo)
+    assert not bool((inner[..., :Cout] == SENT).any()), "%s: an interior element left unwritten" % what
+    pad = inner[..., Cout:cpad]
+    assert bool(((pad == SENT) | (_bits(pad) == 0)).all()), "%s: channels [Cout, Cout_pad) hold neither +0 nor the " \
+                                                            "initial contents" % what
+    assert torch.equal(inner[..., cpad:], was[..., cpad:]), "%s: channels >= Cout_pad written" % what
+
+
 def _conv_case(B, H, W, Cin, Cout, k, stride, dil, mode, act="relu", residual=False, pre=False,
-               bn=True, f32_out=False, seed=0, in_halo=0, out_halo=0, pool=0, pre2=False, no_out0=False, aux_halo=0):
-    """mode: 'tc' (fp16 wgmma), 'direct16', 'direct32'.  Returns (got, ref, got1, ref1)."""
+               bn=True, f32_out=False, seed=0, in_halo=0, out_halo=0, pool=0, pre2=False, no_out0=False, aux_halo=0,
+               off=0):
+    """One convolution through odt_conv2d_f16_tc (mode 'tc') or odt_conv2d_direct ('direct16', 'direct32'), every
+    output inside a sentinel-filled guarded buffer, checked against the float64 reference of tests/conv_ends_ref.py
+    with the per-element bound of the path that ran (named by the library's launch record) and against the write
+    rules of _assert_write_rules.  out1 = relu(v * s2 + h2), out2 = leaky(v * s3 + h3).  off: every output and the residual
+    start `off` elements past a 16-byte boundary.  Returns a ConvResult."""
     from odt_b200 import lib as L
     from odt_b200.engine import same_pad
-    from oracle import tfops as T
     lib = L.load()
     rng = np.random.default_rng(seed)
     f16 = mode != "direct32"
@@ -55,11 +97,13 @@ def _conv_case(B, H, W, Cin, Cout, k, stride, dil, mode, act="relu", residual=Fa
     cOH, cOW = OH, OW                       # the convolution's own output size
     if pool:                                # out0 is the 2x2/2 max-pooled tensor
         OH, OW = OH // 2, OW // 2
-    yd = torch.zeros((B, OH + 2 * oh, OW + 2 * oh, old), dtype=out_dt, device=dev)
-    rd = None
+    oshape = (B, OH + 2 * oh, OW + 2 * oh, old)
+    yg = _guarded_out(oshape, out_dt, oh, off)
+    rg = None
     if residual:
-        rd = torch.zeros((B, OH + 2 * oh, OW + 2 * oh, old), dtype=tdt, device=dev)
+        rd = torch.zeros(oshape, dtype=tdt, device=dev)
         rd[:, oh:oh + OH, oh:oh + OW, :Cout] = torch.from_numpy(res).to(dev).to(tdt)
+        rg = Guarded(oshape, tdt, off=off, fill=rd)
     p = L.ConvParams()
     p.B, p.H, p.W, p.Cin, p.in_ld = B, H, W, Cin, ld
     p.OH, p.OW, p.Cout = cOH, cOW, Cout
@@ -70,81 +114,80 @@ def _conv_case(B, H, W, Cin, Cout, k, stride, dil, mode, act="relu", residual=Fa
     hd = torch.from_numpy(shift).to(dev)
     p.scale = sd.data_ptr() if sd is not None else None
     p.shift = hd.data_ptr()
-    p.act = {"relu": 1, "leaky": 2, None: 0}[act]
-    p.residual = rd.data_ptr() if rd is not None else None
-    p.out0 = yd.data_ptr()
+    p.act = R.ACTS[act]
+    p.residual = rg.ptr() if rg is not None else None
+    p.out0 = None if no_out0 else yg.ptr()
     p.out0_dtype = L.ODT_F32 if out_dt == torch.float32 else L.ODT_F16
-    p.out0_img_stride, p.out0_pix_stride = (OH + 2 * oh) * (OW + 2 * oh) * old, old
+    p.out0_img_stride, p.out0_pix_stride = oshape[1] * oshape[2] * old, old
     p.in_halo, p.out0_halo = in_halo, out_halo
-    s2 = h2 = y1 = None
+    ah = aux_halo
+    ashape = (B, OH + 2 * ah, OW + 2 * ah, old)
+    extras = []                             # (guarded buffer, scale, shift, activation) of out1 / out2
+    for on, a2 in ((pre, "relu"), (pre2, "leaky")):
+        if not on:
+            continue
+        s2 = torch.from_numpy(rng.uniform(0.5, 1.5, Cout).astype(np.float32)).to(dev)
+        h2 = torch.from_numpy((rng.standard_normal(Cout) * 0.2).astype(np.float32)).to(dev)
+        extras.append((_guarded_out(ashape, tdt, ah, off), s2, h2, a2))
     if pre:
-        s2 = rng.uniform(0.5, 1.5, Cout).astype(np.float32)
-        h2 = (rng.standard_normal(Cout) * 0.2).astype(np.float32)
-        s2d, h2d = torch.from_numpy(s2).to(dev), torch.from_numpy(h2).to(dev)
-        ah = aux_halo
-        y1 = torch.zeros((B, OH + 2 * ah, OW + 2 * ah, old), dtype=tdt, device=dev)
-        p.scale2, p.shift2, p.act2 = s2d.data_ptr(), h2d.data_ptr(), 1
-        p.out1, p.out1_img_stride, p.out1_pix_stride = y1.data_ptr(), (OH + 2 * ah) * (OW + 2 * ah) * old, old
-        p.out1_halo = ah
-    s3 = h3 = y2 = None
-    if pre2:  # third epilogue output (checked in here against the rounded out0 like out1)
-        s3 = rng.uniform(0.5, 1.5, Cout).astype(np.float32)
-        h3 = (rng.standard_normal(Cout) * 0.2).astype(np.float32)
-        s3d, h3d = torch.from_numpy(s3).to(dev), torch.from_numpy(h3).to(dev)
-        ah = aux_halo
-        y2 = torch.zeros((B, OH + 2 * ah, OW + 2 * ah, old), dtype=tdt, device=dev)
-        p.scale3, p.shift3, p.act3 = s3d.data_ptr(), h3d.data_ptr(), 2
-        p.out2, p.out2_img_stride, p.out2_pix_stride = y2.data_ptr(), (OH + 2 * ah) * (OW + 2 * ah) * old, old
-        p.out2_halo = ah
-    if no_out0:
-        p.out0 = None
-    st = torch.cuda.current_stream().cuda_stream
-    if mode == "tc":
-        rc = lib.odt_conv2d_f16_tc(xd.data_ptr(), wd.data_ptr(), C.byref(p), st)
-    else:
-        rc = lib.odt_conv2d_direct(xd.data_ptr(), wd.data_ptr(), L.ODT_F16 if f16 else L.ODT_F32,
-                                   C.byref(p), st)
-    L.check(rc, "conv")
-    torch.cuda.synchronize()
-    ref = T.conv2d_same(x, w, None, stride, dil)
-    ref = ref * (scale if scale is not None else 1.0) + shift
-    if act == "relu":
-        ref = np.maximum(ref, 0)
-    elif act == "leaky":
-        ref = np.maximum(ref, 0.1 * ref)
-    if residual:
-        ref = ref + res
-    if pool:
-        ref = T.max_pool_same(ref, 2, 2)
-    got = yd[:, oh:oh + OH, oh:oh + OW, :Cout].float().cpu().numpy()
-    if oh:  # the zero border must never be dirtied
-        full = yd.float().cpu().numpy()
-        assert np.abs(full[:, 0]).max() == 0 and np.abs(full[:, -1]).max() == 0
-        assert np.abs(full[:, :, 0]).max() == 0 and np.abs(full[:, :, -1]).max() == 0
-    got1 = ref1 = None
-    if pre:
-        base = got if (f16 and not f32_out and not no_out0) else ref
-        ref1 = np.maximum(base * s2 + h2, 0)
-        ah = aux_halo
-        got1 = y1[:, ah:ah + OH, ah:ah + OW, :Cout].float().cpu().numpy()
-        if ah:  # the zero border of a halo output is never dirtied
-            f1 = y1.float().cpu().numpy()
-            assert np.abs(f1[:, 0]).max() == 0 and np.abs(f1[:, -1]).max() == 0
-            assert np.abs(f1[:, :, 0]).max() == 0 and np.abs(f1[:, :, -1]).max() == 0
+        g1, s2, h2, a2 = extras[0]
+        p.scale2, p.shift2, p.act2 = s2.data_ptr(), h2.data_ptr(), R.ACTS[a2]
+        p.out1, p.out1_img_stride, p.out1_pix_stride, p.out1_halo = g1.ptr(), ashape[1] * ashape[2] * old, old, ah
     if pre2:
-        base = got if (f16 and not f32_out and not no_out0) else ref
-        t = base * s3 + h3
-        ref2 = np.maximum(t, 0.1 * t)
-        ah = aux_halo
-        got2 = y2[:, ah:ah + OH, ah:ah + OW, :Cout].float().cpu().numpy()
-        if ah:
-            f2 = y2.float().cpu().numpy()
-            assert np.abs(f2[:, 0]).max() == 0 and np.abs(f2[:, :, -1]).max() == 0
-        tol2 = (6e-3 if f16 else 4e-5) * max(np.abs(ref2).max(), 1.0)
-        assert np.abs(got2 - ref2).max() <= tol2, ("out2", float(np.abs(got2 - ref2).max()))
-    if mode == "tc" and old > Cout and not f32_out:
-        assert float(yd[..., Cout:].abs().max()) == 0.0, "pad channels must stay zero"
-    return got, ref.astype(np.float32), got1, ref1
+        g2, s3, h3, a3 = extras[-1]
+        p.scale3, p.shift3, p.act3 = s3.data_ptr(), h3.data_ptr(), R.ACTS[a3]
+        p.out2, p.out2_img_stride, p.out2_pix_stride, p.out2_halo = g2.ptr(), ashape[1] * ashape[2] * old, old, ah
+    st = torch.cuda.current_stream().cuda_stream
+
+    def launch():
+        if mode == "tc":
+            return lib.odt_conv2d_f16_tc(xd.data_ptr(), wd.data_ptr(), C.byref(p), st)
+        return lib.odt_conv2d_direct(xd.data_ptr(), wd.data_ptr(), L.ODT_F16 if f16 else L.ODT_F32, C.byref(p), st)
+
+    L.check(launch(), "conv")
+    kernel = last_conv_kernel()
+    if rg is not None:
+        rg.assert_outside_untouched()
+        rg.assert_untouched(torch.ones(oshape, dtype=torch.bool, device=dev), "residual")
+    # float64 reference of exactly the operands the kernel multiplies
+    xt, wt = torch.from_numpy(x).to(dev), torch.from_numpy(np.ascontiguousarray(ohwi)).to(dev)
+    ref, mag = R.reference(xt, wt, stride, sd, hd, act, dil)
+    rt = torch.from_numpy(res).to(dev) if residual else None
+    n_acc = R.n_acc_body(kernel, k, k, Cin, ld)
+    out16 = out_dt == torch.float16
+    v = ref + rt.double() if residual else ref
+    b0 = R.bound(v, mag, n_acc, f16 and not f32_out, rt)
+    worst = {}
+    got0 = interior(yg.t, oh)[..., :Cout]
+    if no_out0:
+        yg.assert_untouched(torch.ones(oshape, dtype=torch.bool, device=dev), "out0 (not stored)")
+    else:
+        _assert_write_rules(yg, oh, Cout, cpad if out16 else Cout, "out0")
+        if pool:
+            worst["out0"] = R.ratio(got0, R.pool2(v), R.pool2(b0))
+        else:
+            worst["out0"] = R.ratio(got0, v, b0)
+    gots = []
+    for i, (g, s2, h2, a2) in enumerate(extras):
+        name = "out%d" % (i + 1 if pre else 2)
+        _assert_write_rules(g, ah, Cout, cpad, name)
+        got = interior(g.t, ah)[..., :Cout]
+        if no_out0:
+            t = R.consumer(v, s2, h2, a2)
+            worst[name] = R.ratio(got, t, R.bound_through(t, b0, s2, f16))
+        else:
+            t = R.consumer(got0, s2, h2, a2)
+            worst[name] = R.ratio(got, t, R.bound_own(t, f16))
+        gots.append(got.float().cpu().numpy())
+    top = max(worst.values(), key=lambda r: r[0])[0]
+    print("%s B=%d %dx%d %d->%d k%d s%d d%d %s: worst %s" % (
+        kernel, B, H, W, Cin, Cout, k, stride, dil, mode,
+        ", ".join("%s %.3g at %s" % (n, r, at) for n, (r, at) in worst.items())))
+    for n, (r, at) in worst.items():
+        assert r <= 1.0, (kernel, n, r, at)
+    got1 = gots[0] if pre else None
+    got2 = gots[-1] if pre2 else None
+    return ConvResult(got0.float().cpu().numpy(), got1, got2, kernel, top)
 
 
 TC_SHAPES = [
@@ -167,43 +210,33 @@ TC_SHAPES = [
 
 @pytest.mark.parametrize("shape", TC_SHAPES)
 def test_conv_tc_vs_fp32_reference(built, shape):
-    got, ref, _, _ = _conv_case(*shape, mode="tc", seed=hash(shape) % 1000)
-    err = np.abs(got - ref).max()
-    assert err <= 2e-3 * max(np.abs(ref).max(), 1.0), (shape, float(err), float(np.abs(ref).max()))
+    _conv_case(*shape, mode="tc", seed=hash(shape) % 1000)
 
 
 def test_conv_tc_epilogue_variants(built):
     base = (2, 19, 19, 256, 256, 3, 1, 1)
     for kw in (dict(act="leaky", residual=True), dict(act=None, bn=False, pre=True),
                dict(act=None, residual=True, pre=True), dict(act="relu", f32_out=True)):
-        got, ref, got1, ref1 = _conv_case(*base, mode="tc", **kw)
-        tol = 2e-3 * max(np.abs(ref).max(), 1.0)
-        assert np.abs(got - ref).max() <= tol, kw
-        if got1 is not None:
-            assert np.abs(got1 - ref1).max() <= 4e-3 * max(np.abs(ref1).max(), 1.0), kw
+        _conv_case(*base, mode="tc", **kw)
     # fp32 head scatter out of the halo-flat mode (RetinaNet regression head fed by a halo'd pre-activation)
     for cout in (36, 20):
-        got, ref, _, _ = _conv_case(2, 24, 24, 256, cout, 3, 1, 1, mode="tc", act=None, f32_out=True, in_halo=1)
-        assert np.abs(got - ref).max() <= 2e-3 * max(np.abs(ref).max(), 1.0), ("flat head", cout)
+        _conv_case(2, 24, 24, 256, cout, 3, 1, 1, mode="tc", act=None, f32_out=True, in_halo=1)
     # head-style output: ragged Cout (100, 150), fp32, through the generic store path
     for cout in (100, 150, 75, 36, 189, 20, 4, 1):
-        got, ref, _, _ = _conv_case(1, 10, 10, 256, cout, 3, 1, 1, mode="tc", act=None, f32_out=True)
-        assert np.abs(got - ref).max() <= 2e-3 * max(np.abs(ref).max(), 1.0), cout
+        _conv_case(1, 10, 10, 256, cout, 3, 1, 1, mode="tc", act=None, f32_out=True)
 
 
-@pytest.mark.parametrize("mode,tol", [("direct32", 2e-5), ("direct16", 2e-3)])
-def test_conv_direct_vs_fp32_reference(built, mode, tol):
+@pytest.mark.parametrize("mode", ["direct32", "direct16"], ids=["direct32-2e-05", "direct16-0.002"])  # former ids
+def test_conv_direct_vs_fp32_reference(built, mode):
     for shape in [(2, 19, 19, 64, 96, 3, 1, 2), (2, 20, 20, 3, 16, 7, 2, 1), (1, 10, 10, 7, 28, 3, 2, 1),
                   (2, 13, 13, 100, 75, 1, 1, 1), (1, 38, 38, 32, 64, 3, 1, 1)]:
-        got, ref, got1, ref1 = _conv_case(*shape, mode=mode, act="leaky", residual=True, pre=True)
-        assert np.abs(got - ref).max() <= tol * max(np.abs(ref).max(), 1.0), (mode, shape)
-        assert np.abs(got1 - ref1).max() <= 2 * tol * max(np.abs(ref1).max(), 1.0), (mode, shape)
+        _conv_case(*shape, mode=mode, act="leaky", residual=True, pre=True)
 
 
 def test_conv_tc_matches_direct_on_device(built):
     """The two independent device implementations agree (cross-check of im2col TMA)."""
-    a, _, _, _ = _conv_case(2, 38, 38, 128, 128, 3, 1, 1, mode="tc")
-    b, _, _, _ = _conv_case(2, 38, 38, 128, 128, 3, 1, 1, mode="direct16")
+    a = _conv_case(2, 38, 38, 128, 128, 3, 1, 1, mode="tc").got
+    b = _conv_case(2, 38, 38, 128, 128, 3, 1, 1, mode="direct16").got
     assert np.abs(a - b).max() <= 4e-3 * max(np.abs(b).max(), 1.0)
 
 
@@ -410,8 +443,7 @@ FLAT_SHAPES = [
 @pytest.mark.parametrize("tapn", ["0", "1"])   # 0: conv_tc's own flat modes; 1: the default planner (taps-as-N where it pays)
 def test_conv_tc_flat_halo_vs_fp32_reference(built, monkeypatch, shape, out_halo, tapn):
     monkeypatch.setenv("ODT_TC_TAPN", tapn)
-    got, ref, _, _ = _conv_case(*shape, mode="tc", in_halo=1, out_halo=out_halo, seed=sum(shape))
-    assert np.abs(got - ref).max() <= 2e-3 * max(np.abs(ref).max(), 1.0), (shape, out_halo)
+    _conv_case(*shape, mode="tc", in_halo=1, out_halo=out_halo, seed=sum(shape))
 
 
 POOL_SHAPES = [
@@ -432,9 +464,8 @@ def test_conv_tc_fused_maxpool(built, monkeypatch, shape, out_halo, tapn):
     same conv followed by the stand-alone pooling kernel (max commutes with fp16 rounding)."""
     from odt_b200 import lib as L
     monkeypatch.setenv("ODT_TC_TAPN", tapn)
-    got, ref, _, _ = _conv_case(*shape, mode="tc", in_halo=1, out_halo=out_halo, pool=2, seed=sum(shape))
-    assert np.abs(got - ref).max() <= 2e-3 * max(np.abs(ref).max(), 1.0), (shape, out_halo)
-    full, _, _, _ = _conv_case(*shape, mode="tc", in_halo=1, out_halo=0, seed=sum(shape))
+    got = _conv_case(*shape, mode="tc", in_halo=1, out_halo=out_halo, pool=2, seed=sum(shape)).got
+    full = _conv_case(*shape, mode="tc", in_halo=1, out_halo=0, seed=sum(shape)).got
     B, H, W, _, Cout = shape[:5]
     ld = (Cout + 63) // 64 * 64
     xd = torch.zeros((B, H, W, ld), dtype=torch.float16, device="cuda")
@@ -456,11 +487,10 @@ def test_conv_tc_fused_maxpool_rejects_bad_shapes(built):
 @pytest.mark.parametrize("shape,pool", [((2, 38, 38, 64, 64, 3, 1, 1), 0), ((3, 75, 75, 64, 128, 3, 1, 1), 0),
                                         ((2, 300, 300, 64, 64, 3, 1, 1), 2), ((1, 40, 40, 128, 64, 3, 1, 1), 2)])
 def test_conv_tc_resident_filter_bank_is_bit_identical(built, shape, pool):
-    """Layers whose filter bank stays resident in shared memory, against the fp32 reference, and two launches
+    """Layers whose filter bank stays resident in shared memory, against the float64 bound, and two launches
     bit-identical."""
-    a, ref, _, _ = _conv_case(*shape, mode="tc", in_halo=1, out_halo=1, pool=pool)
-    b, _, _, _ = _conv_case(*shape, mode="tc", in_halo=1, out_halo=1, pool=pool)
-    assert np.abs(a - ref).max() <= 2e-3 * max(np.abs(ref).max(), 1.0)
+    a = _conv_case(*shape, mode="tc", in_halo=1, out_halo=1, pool=pool).got
+    b = _conv_case(*shape, mode="tc", in_halo=1, out_halo=1, pool=pool).got
     np.testing.assert_array_equal(a, b)
 
 
@@ -477,22 +507,18 @@ LARGE_SHAPES = [
 @pytest.mark.parametrize("shape", LARGE_SHAPES)
 def test_conv_tc_large_tile_counts(built, shape):
     """Layers of hundreds of tiles (odd tile counts, ragged last tiles, several N tiles, stride, dilation) against the
-    fp32 reference, and two launches bit-identical (static tile schedule, fixed K order)."""
-    a, ref, a1, r1 = _conv_case(*shape, mode="tc", act="leaky", residual=True, pre=True, seed=sum(shape))
-    tol = 2e-3 * max(np.abs(ref).max(), 1.0)
-    assert np.abs(a - ref).max() <= tol and np.abs(a1 - r1).max() <= 2 * tol
-    b, _, b1, _ = _conv_case(*shape, mode="tc", act="leaky", residual=True, pre=True, seed=sum(shape))
-    np.testing.assert_array_equal(a, b)
-    np.testing.assert_array_equal(a1, b1)
+    float64 bound, and two launches bit-identical (static tile schedule, fixed K order)."""
+    a = _conv_case(*shape, mode="tc", act="leaky", residual=True, pre=True, seed=sum(shape))
+    b = _conv_case(*shape, mode="tc", act="leaky", residual=True, pre=True, seed=sum(shape))
+    np.testing.assert_array_equal(a.got, b.got)
+    np.testing.assert_array_equal(a.got1, b.got1)
 
 
 def test_conv_tc_large_head_scatter_and_halo(built):
     # fp32 head rows (RetinaNet cls head shape class) and halo in/out layouts at large tile counts
-    g, ref, _, _ = _conv_case(4, 100, 100, 256, 189, 3, 1, 1, mode="tc", act=None, f32_out=True)
-    assert np.abs(g - ref).max() <= 2e-3 * max(np.abs(ref).max(), 1.0)
-    h, ref2, _, _ = _conv_case(4, 100, 100, 128, 256, 3, 1, 1, mode="tc", in_halo=1, out_halo=1)
-    assert np.abs(h - ref2).max() <= 2e-3 * max(np.abs(ref2).max(), 1.0)
-    h0, _, _, _ = _conv_case(4, 100, 100, 128, 256, 3, 1, 1, mode="tc", in_halo=1, out_halo=1)
+    _conv_case(4, 100, 100, 256, 189, 3, 1, 1, mode="tc", act=None, f32_out=True)
+    h = _conv_case(4, 100, 100, 128, 256, 3, 1, 1, mode="tc", in_halo=1, out_halo=1).got
+    h0 = _conv_case(4, 100, 100, 128, 256, 3, 1, 1, mode="tc", in_halo=1, out_halo=1).got
     np.testing.assert_array_equal(h, h0)
 
 
@@ -500,10 +526,9 @@ def test_conv_tc_large_head_scatter_and_halo(built):
                                         ((2, 300, 300, 64, 64, 3, 1, 1), 2), ((2, 150, 150, 128, 128, 3, 1, 1), 2),
                                         ((1, 150, 150, 128, 128, 3, 1, 1), 0), ((1, 17, 23, 64, 28, 3, 1, 1), 0)])
 def test_conv_tc_flat_modes_bit_identical(built, shape, pool):
-    """Halo-flat / row-block modes against the fp32 reference, and two launches bit-identical."""
-    a, ref, _, _ = _conv_case(*shape, mode="tc", in_halo=1, out_halo=1, pool=pool)
-    assert np.abs(a - ref).max() <= 2e-3 * max(np.abs(ref).max(), 1.0)
-    b, _, _, _ = _conv_case(*shape, mode="tc", in_halo=1, out_halo=1, pool=pool)
+    """Halo-flat / row-block modes against the float64 bound, and two launches bit-identical."""
+    a = _conv_case(*shape, mode="tc", in_halo=1, out_halo=1, pool=pool).got
+    b = _conv_case(*shape, mode="tc", in_halo=1, out_halo=1, pool=pool).got
     np.testing.assert_array_equal(a, b)
 
 
@@ -515,11 +540,7 @@ def test_conv_tc_flat_modes_bit_identical(built, shape, pool):
 ])
 def test_conv_tc_two_preactivation_outputs(built, shape, kw):
     """out1 and out2 (two consumer BN+activation variants of the same conv output)."""
-    got, ref, g1, r1 = _conv_case(*shape, mode="tc", pre=True, pre2=True, **kw)
-    tol = 2e-3 * max(np.abs(ref).max(), 1.0)
-    if not kw.get("no_out0"):
-        assert np.abs(got - ref).max() <= tol
-    assert np.abs(g1 - r1).max() <= 3 * tol
+    _conv_case(*shape, mode="tc", pre=True, pre2=True, **kw)
 
 
 @pytest.mark.parametrize("shape,kw,env", [
@@ -534,15 +555,11 @@ def test_conv_extra_outputs_in_halo_layout(built, monkeypatch, shape, kw, env):
     every kernel behind odt_conv2d_f16_tc: the 3x3 convolutions that read them then take the halo modes."""
     for k, v in env.items():
         monkeypatch.setenv(k, v)
-    got, ref, g1, r1 = _conv_case(*shape, mode="tc", seed=sum(shape), pre=True, pre2=True, aux_halo=1, **kw)
-    tol = 2e-3 * max(np.abs(ref).max(), 1.0)
-    assert np.abs(got - ref).max() <= tol, shape
-    assert np.abs(g1 - r1).max() <= 3 * tol
+    _conv_case(*shape, mode="tc", seed=sum(shape), pre=True, pre2=True, aux_halo=1, **kw)
 
 
 def test_conv_direct_two_preactivation_outputs(built):
-    got, ref, g1, r1 = _conv_case(2, 20, 20, 24, 40, 3, 1, 1, mode="direct32", pre=True, pre2=True)
-    assert np.abs(got - ref).max() <= 2e-5 * max(np.abs(ref).max(), 1.0)
+    _conv_case(2, 20, 20, 24, 40, 3, 1, 1, mode="direct32", pre=True, pre2=True)
 
 
 @pytest.mark.parametrize("shape,kw", [
@@ -555,21 +572,17 @@ def test_conv_direct_two_preactivation_outputs(built):
 def test_conv_tc_thin_input_channels(built, shape, kw):
     """Cin that does not fill its 64-channel chunk (RetinaNet's 7*2^i widths, zero-padded operands) in every
     tensor-core mode; the all-zero 16-deep K steps are not issued."""
-    got, ref, _, _ = _conv_case(*shape, mode="tc", seed=sum(shape), **kw)
-    assert np.abs(got - ref).max() <= 2e-3 * max(np.abs(ref).max(), 1.0), shape
+    _conv_case(*shape, mode="tc", seed=sum(shape), **kw)
 
 
 def test_conv_tc_flat_equals_im2col_path(built):
     """The same operands through both tensor-core paths: stored with a halo (halo-flat mode) and densely (im2col
     mode; _conv_case draws the same values whatever the layout)."""
     shape = (2, 38, 38, 128, 128, 3, 1, 1)
-    a, ref, a1, r1 = _conv_case(*shape, mode="tc", in_halo=1, out_halo=1, act="leaky", residual=True, pre=True)
-    b, _, b1, _ = _conv_case(*shape, mode="tc", in_halo=0, out_halo=0, act="leaky", residual=True, pre=True)
-    tol = 2e-3 * max(np.abs(ref).max(), 1.0)
-    assert np.abs(a - ref).max() <= tol and np.abs(b - ref).max() <= tol
-    assert np.abs(a1 - r1).max() <= 2 * tol and np.abs(b1 - r1).max() <= 2 * tol
+    a = _conv_case(*shape, mode="tc", in_halo=1, out_halo=1, act="leaky", residual=True, pre=True).got
+    b = _conv_case(*shape, mode="tc", in_halo=0, out_halo=0, act="leaky", residual=True, pre=True).got
     # identical operand values and accumulation order per tap chunk -> (near) identical results
-    assert np.abs(a - b).max() <= 1e-3 * max(np.abs(ref).max(), 1.0)
+    assert np.abs(a - b).max() <= 1e-3 * max(np.abs(b).max(), 1.0)
 
 
 @pytest.mark.parametrize("shape", [
@@ -578,8 +591,7 @@ def test_conv_tc_flat_equals_im2col_path(built):
     (2, 26, 26, 128, 64, 1, 1, 1),    # 1x1 writing a halo output
 ])
 def test_conv_tc_im2col_with_halo_layouts(built, shape):
-    got, ref, _, _ = _conv_case(*shape, mode="tc", in_halo=1, out_halo=1)
-    assert np.abs(got - ref).max() <= 2e-3 * max(np.abs(ref).max(), 1.0), shape
+    _conv_case(*shape, mode="tc", in_halo=1, out_halo=1)
 
 
 def test_maxpool_halo_layouts(built):
@@ -642,12 +654,9 @@ def test_conv_tapn_matches_reference(built, monkeypatch, shape, kw):
     from odt_b200 import lib as L
     monkeypatch.setenv("ODT_TC_TAPN", "2")   # 2 = wherever the layer qualifies (1 also asks the cost model)
     before = L.load().odt_debug_tapn_launches()
-    got, ref, g1, r1 = _conv_case(*shape, mode="tc", seed=sum(shape), **kw)
-    assert L.load().odt_debug_tapn_launches() == before + 1, "the layer did not take the taps-as-N path"
-    tol = 2e-3 * max(np.abs(ref).max(), 1.0)
-    assert np.abs(got - ref).max() <= tol, shape
-    if g1 is not None:
-        assert np.abs(g1 - r1).max() <= 3 * tol
+    r = _conv_case(*shape, mode="tc", seed=sum(shape), **kw)
+    assert L.load().odt_debug_tapn_launches() == before + 1 and r.kernel.startswith("conv_tapn_kernel<"), \
+        "the layer did not take the taps-as-N path"
 
 
 def _tc_raw(x, w, pool=0, in_halo=1, out_halo=1):
@@ -698,13 +707,9 @@ def test_conv_pw_matches_reference(built, monkeypatch, shape, kw):
     from odt_b200 import lib as L
     monkeypatch.setenv("ODT_TC_PW", "2")
     before = L.load().odt_debug_pw_launches()
-    got, ref, g1, r1 = _conv_case(*shape, mode="tc", seed=sum(shape), **kw)
-    assert L.load().odt_debug_pw_launches() == before + 1, "the layer did not take the pointwise path"
-    tol = 2e-3 * max(np.abs(ref).max(), 1.0)
-    if not kw.get("no_out0"):
-        assert np.abs(got - ref).max() <= tol, shape
-    if g1 is not None:
-        assert np.abs(g1 - r1).max() <= 3 * tol
+    r = _conv_case(*shape, mode="tc", seed=sum(shape), **kw)
+    assert L.load().odt_debug_pw_launches() == before + 1 and r.kernel.startswith("conv_pw_kernel<"), \
+        "the layer did not take the pointwise path"
 
 
 def test_conv_pw_is_bit_identical_to_the_tensor_core_path_on_exact_inputs(built, monkeypatch):
@@ -791,10 +796,6 @@ def test_conv_thin_matches_reference(built, monkeypatch, shape, kw):
     monkeypatch.setenv("ODT_TC_THIN", "2")
     monkeypatch.setenv("ODT_TC_PW", "0")  # the staged pointwise kernel would take the 1x1 cases first
     before = L.load().odt_debug_thin_launches()
-    got, ref, g1, r1 = _conv_case(*shape, mode="tc", seed=sum(shape), **kw)
-    assert L.load().odt_debug_thin_launches() == before + 1, "the layer did not take the thin path"
-    tol = 2e-3 * max(np.abs(ref).max(), 1.0)
-    if not kw.get("no_out0"):
-        assert np.abs(got - ref).max() <= tol, shape
-    if g1 is not None:
-        assert np.abs(g1 - r1).max() <= 3 * tol
+    r = _conv_case(*shape, mode="tc", seed=sum(shape), **kw)
+    assert L.load().odt_debug_thin_launches() == before + 1 and r.kernel.startswith("conv_thin_kernel<"), \
+        "the layer did not take the thin path"

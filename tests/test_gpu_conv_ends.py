@@ -12,15 +12,17 @@
   d. every network's stem and head convolutions in situ at full size, and the candidate rows of pipeline slot 1.
 """
 import ctypes as C
-import re
 
 import numpy as np
 import pytest
 import torch
 
 import conv_ends_ref as R
+from gpu_harness import Guarded, kernels_launched
+from gpu_harness import interior as _interior
+from gpu_harness import mask as _mask
+from gpu_harness import model as _model
 
-SENT = -12345.0  # exactly representable in fp16 and fp32
 ERR_INVALID = -1
 
 
@@ -31,64 +33,6 @@ def _lib():
 
 def _st():
     return torch.cuda.current_stream().cuda_stream
-
-
-class Guarded:
-    """A tensor of `shape` placed `off` elements into a buffer of `fill` with `guard` elements on either side."""
-
-    def __init__(self, shape, dt, off=0, guard=2048, fill=SENT):
-        n = int(np.prod(shape))
-        self.buf = torch.full((n + 2 * guard + off,), fill, dtype=dt, device="cuda")
-        self.lo, self.n = guard + off, n
-        self.t = self.buf[self.lo:self.lo + n].view(shape)
-        self.before = self.buf.clone()
-
-    def ptr(self):
-        return self.t.data_ptr()
-
-    def assert_outside_untouched(self):
-        b, a = self.buf, self.before
-        assert torch.equal(b[:self.lo], a[:self.lo]), "write before the tensor"
-        assert torch.equal(b[self.lo + self.n:], a[self.lo + self.n:]), "write past the tensor"
-
-    def assert_untouched(self, region, what):
-        now, was = self.t[region], self.before[self.lo:self.lo + self.n].view(self.t.shape)[region]
-        assert torch.equal(now, was), "%s written" % what
-
-
-def _mask(shape, halo=0, c=None):
-    """True at the positions a kernel must not write: the 1-pixel halo and the channels >= c."""
-    m = torch.zeros(shape, dtype=torch.bool, device="cuda")
-    if halo:
-        m[:, 0], m[:, -1], m[:, :, 0], m[:, :, -1] = True, True, True, True
-    if c is not None:
-        m[..., c:] = True
-    return m
-
-
-def _interior(t, halo):
-    return t[:, halo:t.shape[1] - halo, halo:t.shape[2] - halo] if halo else t
-
-
-def kernels_launched(fn, tries=3):
-    """(fn(), names with whitespace removed of the library's kernels fn launches), from a torch.profiler trace.  A short
-    trace can come back without some of its device activity, so fn runs between two torch marker kernels and the trace
-    counts only when both markers are in it (fn is re-run otherwise: every call here is idempotent)."""
-    from torch.profiler import ProfilerActivity, profile
-    marker = torch.zeros(1, device="cuda")
-    for _ in range(tries):
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-            marker.add_(1)
-            out = fn()
-            marker.add_(1)
-            torch.cuda.synchronize()
-        names = [re.sub(r"\s+", "", e.name) for e in prof.events()
-                 if e.device_type == torch.autograd.DeviceType.CUDA and "Memcpy" not in e.name
-                 and "Memset" not in e.name]
-        if len([n for n in names if "odt::" not in n]) == 2:
-            return out, [n for n in names if "odt::" in n]
-    raise AssertionError("%d profiler traces in a row lost device activity" % tries)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -547,24 +491,6 @@ def test_head_scatter(built, mode, name):
 # ---------------------------------------------------------------------------------------------------------------------
 # d. in situ at full size
 # ---------------------------------------------------------------------------------------------------------------------
-def _model(kind, precision, **over):
-    from helpers import model_cfg
-    import FCOS
-    import RetinaNet
-    import SSD300
-    import SSD512
-    import YOLOv3
-    if kind == "ssd300":
-        return SSD300.SSD300(model_cfg("ssd", precision=precision, bn_init="trained", **over), None)
-    if kind == "ssd512":
-        return SSD512.SSD512(model_cfg("ssd", precision=precision, bn_init="trained", **over), None)
-    if kind == "retinanet":
-        return RetinaNet.RetinaNet(model_cfg("retinanet", precision=precision, bn_init="trained", **over), None)
-    if kind == "yolov3":
-        return YOLOv3.YOLOv3(model_cfg("yolov3", precision=precision, bn_init="trained", **over), None)
-    return FCOS.FCOS(model_cfg("fcos", precision=precision, bn_init="trained", **over), None)
-
-
 def _op_operands(op, net):
     """(weights [Cout,R,S,Cin], scale or None, shift) the kernel multiplies, cut to the real channels."""
     cin = 3 if op.is_image else op.x.C

@@ -1,7 +1,7 @@
 """conv_tc_kernel's ping-pong schedule: the two consumer warpgroups take alternate tiles of a CTA's static tile list
 (grid = min(tiles, 132)).  Cases at the schedule's edges -- one, exactly two and an odd number of tiles per CTA, the
 two warpgroups on different N tiles, every A-feeding mode, the head scatter, residual + out1 + out2, K-step
-skipping -- against the fp32 reference at the tolerances of test_gpu_conv.py, and two launches bit-identical."""
+skipping -- against the float64 bound of _conv_case, and two launches bit-identical."""
 import numpy as np
 import pytest
 
@@ -41,12 +41,9 @@ def test_conv_tc_pingpong_schedule(built, monkeypatch, case):
     shape, kw, env = CASES[case]
     for k, v in env.items():
         monkeypatch.setenv(k, v)
-    a, ref, a1, r1 = _conv_case(*shape, mode="tc", seed=sum(shape), **kw)
-    tol = 2e-3 * max(np.abs(ref).max(), 1.0)
-    assert np.abs(a - ref).max() <= tol, (case, float(np.abs(a - ref).max()), tol)
-    if a1 is not None:
-        assert np.abs(a1 - r1).max() <= 3 * tol, case
-    b, _, b1, _ = _conv_case(*shape, mode="tc", seed=sum(shape), **kw)
-    np.testing.assert_array_equal(a, b)
-    if a1 is not None:
-        np.testing.assert_array_equal(a1, b1)
+    a = _conv_case(*shape, mode="tc", seed=sum(shape), **kw)
+    assert a.kernel.startswith("conv_tc_kernel<"), a.kernel
+    b = _conv_case(*shape, mode="tc", seed=sum(shape), **kw)
+    np.testing.assert_array_equal(a.got, b.got)
+    if a.got1 is not None:
+        np.testing.assert_array_equal(a.got1, b.got1)

@@ -19,11 +19,15 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from gpu_harness import Guarded
+from gpu_harness import interior as _interior
+from gpu_harness import mask as _mask
+from gpu_harness import model as _model
+
 pytestmark = pytest.mark.gpu
 
 U32 = 2.0 ** -24   # unit roundoff of fp32
 U16 = 2.0 ** -11   # unit roundoff of fp16
-SENT16 = -12345.0  # exactly representable in fp16 and fp32
 GN_EPS = 1e-6
 DTYPES = {"f16": torch.float16, "f32": torch.float32}
 
@@ -46,46 +50,6 @@ def _st():
 def _check(rc, what=""):
     from odt_b200 import lib as L
     L.check(rc, what)
-
-
-class Guarded:
-    """A tensor of `shape` placed `off` elements into a sentinel-filled buffer with `guard` elements on either side."""
-
-    def __init__(self, shape, dt, off=0, guard=1024, fill=None):
-        n = int(np.prod(shape))
-        self.buf = torch.full((n + 2 * guard + off,), SENT16, dtype=dt, device="cuda")
-        self.lo, self.n = guard + off, n
-        self.t = self.buf[self.lo:self.lo + n].view(shape)
-        if fill is not None:
-            self.t.copy_(fill)
-        self.before = self.buf.clone()
-
-    def ptr(self):
-        return self.t.data_ptr()
-
-    def assert_outside_untouched(self):
-        b, a = self.buf, self.before
-        assert torch.equal(b[:self.lo], a[:self.lo]), "write before the tensor"
-        assert torch.equal(b[self.lo + self.n:], a[self.lo + self.n:]), "write past the tensor"
-
-    def assert_untouched(self, region, what):
-        """`region` (a boolean mask over the tensor) kept its initial contents."""
-        now, was = self.t[region], self.before[self.lo:self.lo + self.n].view(self.t.shape)[region]
-        assert torch.equal(now, was), "%s written" % what
-
-
-def _mask(shape, halo=0, c=None):
-    """True at the positions a kernel must not write: the 1-pixel halo and the channels >= c."""
-    m = torch.zeros(shape, dtype=torch.bool, device="cuda")
-    if halo:
-        m[:, 0], m[:, -1], m[:, :, 0], m[:, :, -1] = True, True, True, True
-    if c is not None:
-        m[..., c:] = True
-    return m
-
-
-def _interior(t, halo):
-    return t[:, halo:t.shape[1] - halo, halo:t.shape[2] - halo] if halo else t
 
 
 def _ulps(got, ref):
@@ -655,24 +619,6 @@ def test_groupnorm_batch_invariant_and_reproducible(lib, dtype, shape):
 # ---------------------------------------------------------------------------------------------------------------------
 # c. in situ at full size
 # ---------------------------------------------------------------------------------------------------------------------
-def _model(kind, precision, **over):
-    from helpers import model_cfg
-    import FCOS
-    import RetinaNet
-    import SSD300
-    import SSD512
-    import YOLOv3
-    if kind == "ssd300":
-        return SSD300.SSD300(model_cfg("ssd", precision=precision, bn_init="trained", **over), None)
-    if kind == "ssd512":
-        return SSD512.SSD512(model_cfg("ssd", precision=precision, bn_init="trained", **over), None)
-    if kind == "retinanet":
-        return RetinaNet.RetinaNet(model_cfg("retinanet", precision=precision, bn_init="trained", **over), None)
-    if kind == "yolov3":
-        return YOLOv3.YOLOv3(model_cfg("yolov3", precision=precision, bn_init="trained", **over), None)
-    return FCOS.FCOS(model_cfg("fcos", precision=precision, bn_init="trained", **over), None)
-
-
 def _check_pad_lanes(buf, C, what):
     if buf.shape[-1] > C:
         assert not bool(buf[..., C:].ne(0).any()), "%s: channel >= C written" % what
