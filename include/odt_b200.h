@@ -309,7 +309,9 @@ int odt_fcos_loss_fwd(const float* head, const odt_tail_params* p, int B, const 
  * without a GT centre): replaces the loss section of `_build_graph` YOLOv3.py:115-318 on the candidate
  * rows [20 cls, y, x, h, w, obj].  The four scales are config['coord_scale' | 'noobj_scale' |
  * 'obj_scale' | 'class_scale'].  loss_out [B] is pos_loss + neg_loss per image (the graph then takes
- * 0.5 x the batch mean). */
+ * 0.5 x the batch mean).  Every level holds the same number of priors A (1..ODT_MAX_PRIORS), its rows
+ * cell after cell with the A priors of a cell consecutive: level.offset = rows of the levels before it,
+ * N = sum of H*W*A; anything else is rejected before any launch.  The scratch holds one byte per cell. */
 long long odt_yolo_loss_scratch_bytes(const odt_tail_params* p, int B);
 int odt_yolo_loss_fwd(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
                       float coord_scale, float noobj_scale, float obj_scale, float class_scale,

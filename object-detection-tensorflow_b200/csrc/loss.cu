@@ -595,6 +595,14 @@ __device__ __forceinline__ YoloGt yolo_gt(const float* gb, int g, int k) {
   return n;
 }
 
+// Cells (H * W) of the levels before `lvl`: where that level starts in the per-image occupancy array.  Every level
+// holds the same number of priors A (odt_yolo_loss_fwd checks it), and a cell's A rows are consecutive.
+__device__ __forceinline__ int yolo_cell_base(const odt_tail_params& p, int lvl) {
+  int c = 0;
+  for (int i = 0; i < lvl; ++i) c += p.level[i].H * p.level[i].W;
+  return c;
+}
+
 // K1: one block per image, one thread per GT: level / prior assignment, positive terms, cell occupancy.
 // NFG = 20: the 25-float rows, class loop fixed at compile time; NFG = 0: num_fg from the parameters.
 template <int NFG>
@@ -609,7 +617,7 @@ __global__ void __launch_bounds__(kMaxGT)
   const float* gb = gt + (long long)b * G * 5;
   __shared__ float s_red[3][kMaxGT];
   const int cnt = block_gt_count(gb, G);
-  const long long cells = p.N / 3;
+  const long long cells = yolo_cell_base(p, kYoloLevels);
   float coord = 0.f, cls = 0.f, obj = 0.f;
   if (g < cnt) {
     float mx[kYoloLevels];
@@ -620,11 +628,12 @@ __global__ void __launch_bounds__(kMaxGT)
       const YoloGt n = yolo_gt(gb, g, k);
       cy[k] = min(max((int)floorf(n.y), 0), L.H - 1);
       cx[k] = min(max((int)floorf(n.x), 0), L.W - 1);
-      occ[(long long)b * cells + L.offset / 3 + cy[k] * L.W + cx[k]] = 1;  // every GT marks its cell on every level
+      // every GT marks its cell on every level
+      occ[(long long)b * cells + yolo_cell_base(p, k) + cy[k] * L.W + cx[k]] = 1;
       const float ay = (float)cy[k] + 0.5f, ax = (float)cx[k] + 0.5f;
       float bv = 0.f;
       int bi = 0;
-      for (int a = 0; a < 3; ++a) {
+      for (int a = 0; a < L.A; ++a) {  // the level's priors; the first maximum wins
         const float hh = __fdiv_rn(L.prior_h[a], 2.f), hw = __fdiv_rn(L.prior_w[a], 2.f);
         const float v = iou_unclamped(n.y1, n.x1, n.y2, n.x2, __fsub_rn(ay, hh), __fsub_rn(ax, hw), __fadd_rn(ay, hh),
                                       __fadd_rn(ax, hw), __fmul_rn(L.prior_h[a], L.prior_w[a]));
@@ -641,7 +650,7 @@ __global__ void __launch_bounds__(kMaxGT)
     else if (mx[1] > mx[0] && mx[1] > mx[2]) k = 1;
     const odt_level& L = p.level[k];
     const YoloGt n = yolo_gt(gb, g, k);
-    const float* r = head + ((long long)b * p.N + L.offset + (long long)(cy[k] * L.W + cx[k]) * 3 + arg[k]) * row;
+    const float* r = head + ((long long)b * p.N + L.offset + (long long)(cy[k] * L.W + cx[k]) * L.A + arg[k]) * row;
     const float ty = __fsub_rn(n.y, floorf(n.y)), tx = __fsub_rn(n.x, floorf(n.x));
     const float th = logf(__fdiv_rn(n.h, L.prior_h[arg[k]])), tw = logf(__fdiv_rn(n.w, L.prior_w[arg[k]]));
     const float* t = r + nfg;  // y, x, h, w, obj behind the class scores
@@ -680,7 +689,7 @@ __global__ void __launch_bounds__(kLossThreads)
     }
   }
   __syncthreads();
-  const long long cells = p.N / 3;
+  const long long cells = yolo_cell_base(p, kYoloLevels);
   const int row = row_floats(p.num_fg);
   const float* hb = head + (long long)b * p.N * row;
   float acc = 0.f;
@@ -689,7 +698,7 @@ __global__ void __launch_bounds__(kLossThreads)
   for (int n = n_begin + threadIdx.x; n < n_end; n += blockDim.x) {
     const Cell c = locate(p, n);
     const odt_level& L = p.level[c.lvl];
-    if (occ[(long long)b * cells + L.offset / 3 + c.y * L.W + c.x]) continue;
+    if (occ[(long long)b * cells + yolo_cell_base(p, c.lvl) + c.y * L.W + c.x]) continue;
     const float ay = (float)c.y + 0.5f, ax = (float)c.x + 0.5f;
     const float ph = L.prior_h[c.a], pw = L.prior_w[c.a];
     const float cyy = __fsub_rn(ay, __fdiv_rn(ph, 2.f)), cxx = __fsub_rn(ax, __fdiv_rn(pw, 2.f));  // "centre" = y1x1
@@ -771,13 +780,18 @@ static FcosScratch fcos_scratch(const odt_tail_params&, int B, void* base) {
 struct YoloScratch {
   float* pos;          // (coord, class, obj, #GT) per image
   float* partial;      // no-object sum per (image, anchor block)
-  unsigned char* occ;  // 1 for a cell that holds a GT, [B][N / 3]
+  unsigned char* occ;  // 1 for a cell that holds a GT, [B][sum of H * W over the levels]
   long long bytes;
 };
+static long long yolo_cells(const odt_tail_params& p) {
+  long long c = 0;
+  for (int i = 0; i < kYoloLevels; ++i) c += (long long)p.level[i].H * p.level[i].W;
+  return c;
+}
 static YoloScratch yolo_scratch(const odt_tail_params& p, int B, void* base) {
   Carve c{(uintptr_t)base, 0};
   return {c.take<float>((long long)B * 4), c.take<float>((long long)B * kLossBlocks),
-          c.take<unsigned char>((long long)B * (p.N / 3)), c.bytes};
+          c.take<unsigned char>((long long)B * yolo_cells(p)), c.bytes};
 }
 
 template <class Layout>
@@ -870,12 +884,23 @@ extern "C" int odt_yolo_loss_fwd(const float* head, const odt_tail_params* p, in
   ODT_CHECK_ARG(head && p && gt && scratch && loss_out, "null pointer");
   ODT_CHECK_ARG(p->kind == ODT_DECODE_YOLO3 && p->num_levels == kYoloLevels && p->num_fg >= 1 && p->num_fg <= kMaxFg,
                 "YOLOv3 head with 3 levels and 1..128 classes expected");
-  for (int i = 0; i < kYoloLevels; ++i) ODT_CHECK_ARG(p->level[i].A == 3, "3 priors per level expected");
+  // One prior count on every level (the config's num_priors), and rows laid out level after level, cell after cell:
+  // the kernels find a level's rows at its offset and its cells in the occupancy array by these sums.
+  const int A = p->level[0].A;
+  ODT_CHECK_ARG(A >= 1 && A <= ODT_MAX_PRIORS, "1..9 priors per level expected");
+  long long rows = 0;
+  for (int i = 0; i < kYoloLevels; ++i) {
+    const odt_level& L = p->level[i];
+    ODT_CHECK_ARG(L.A == A, "the same number of priors on every level expected");
+    ODT_CHECK_ARG(L.H >= 1 && L.W >= 1 && L.offset == rows, "level geometry: H, W >= 1, offset = rows before it");
+    rows += (long long)L.H * L.W * A;
+  }
+  ODT_CHECK_ARG(rows == p->N, "N must be the sum of H * W * A over the levels");
   ODT_CHECK_ARG(B > 0 && G > 0 && G <= kMaxGT, "B/G (G <= 128)");
   ODT_CHECK_ARG(((uintptr_t)scratch & 7) == 0, "scratch must be 8-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
   const YoloScratch s = yolo_scratch(*p, B, scratch);
-  ODT_CUDA_OK(cudaMemsetAsync(s.occ, 0, (size_t)B * (p->N / 3), st));
+  ODT_CUDA_OK(cudaMemsetAsync(s.occ, 0, (size_t)B * yolo_cells(*p), st));
   TailP tp;
   tp.p = *p;
   if (p->num_fg == 20)

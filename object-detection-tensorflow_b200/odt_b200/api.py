@@ -633,6 +633,7 @@ class YOLOv3(_Detector):
     def __init__(self, config, data_provider):
         assert len(config["data_shape"]) == 3
         nets.check_sigmoid_num_classes(config)
+        nets.check_yolo_priors(config)
         self._common_init(config, data_provider)
         self.data_shape = config["data_shape"]
         self.num_classes = config["num_classes"]

@@ -45,6 +45,29 @@ def check_sigmoid_num_classes(cfg):
                          % (nc, MAX_SIGMOID_CLASSES))
 
 
+MAX_PRIORS = 9  # ODT_MAX_PRIORS: the prior sizes a level carries in odt_tail_params
+
+
+def check_yolo_priors(cfg):
+    """YOLOv3's anchors: `num_priors` from 1 to 9 and `priors` as three levels of exactly `num_priors` (h, w) pairs of
+    positive finite numbers.  The reference reshapes each level with [1, 1, -1, 2] and lets TF broadcast a level of
+    one pair over every prior; that is rejected here (DESIGN.md section 1)."""
+    npri = cfg["num_priors"]
+    if isinstance(npri, bool) or not isinstance(npri, (int, np.integer)) or not 1 <= npri <= MAX_PRIORS:
+        raise ValueError("num_priors = %r: YOLOv3 supports 1 to %d priors per level" % (npri, MAX_PRIORS))
+    priors = cfg["priors"]
+    if not isinstance(priors, (list, tuple, np.ndarray)) or len(priors) != 3:
+        raise ValueError("priors = %r: YOLOv3 takes 3 levels of num_priors = %d (h, w) pairs" % (priors, npri))
+    for k, level in enumerate(priors):
+        try:
+            arr = np.asarray(level, dtype=np.float64)
+        except (TypeError, ValueError):
+            arr = None
+        if arr is None or arr.shape != (npri, 2) or not (np.isfinite(arr).all() and (arr > 0).all()):
+            raise ValueError("priors[%d] = %r: YOLOv3 takes num_priors = %d positive finite (h, w) pairs per level"
+                             % (k, level, npri))
+
+
 # ------------------------------------------------------------------- SSD ----
 def ssd_scales(size):
     """ref SSD300.py:112-113, SSD512.py:116-118 (Python doubles like the reference)."""
@@ -257,8 +280,8 @@ def build_yolov3(batch, cfg, precision="fp16", device="cuda", allow_tc=True):
     """ref YOLOv3.py:81-113,387-417,485-507."""
     H, W, _ = cfg["data_shape"]
     check_sigmoid_num_classes(cfg)
+    check_yolo_priors(cfg)
     nc, npri = cfg["num_classes"], cfg["num_priors"]
-    assert npri == 3, "3 priors per level"
     net = Net(batch, H, W, precision, device, allow_tc)
 
     def cl(x, f, k, s, act=True, residual=None, head=None):  # conv -> BN -> leaky (:494-507)
@@ -315,7 +338,7 @@ def yolo_tail(cfg):
         lv.cmul_y = lv.cmul_x = lv.cdiv_y = lv.cdiv_x = 1.0
         lv.out_mul = mult[i]
         pr = (np.array(priors[i], dtype=F32) / F32(stride[i])).astype(F32)
-        for a in range(3):
+        for a in range(cfg["num_priors"]):
             lv.prior_h[a], lv.prior_w[a] = float(pr[a][0]), float(pr[a][1])
 
     return Tail(L.DECODE_YOLO3, nc, nc, cfg["nms_score_threshold"], cfg["nms_iou_threshold"],

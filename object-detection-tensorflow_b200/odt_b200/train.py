@@ -503,15 +503,15 @@ class GraphTrainer:
                     + 0.5 * ((rws[:, nc + 2:nc + 4] - thw) ** 2).sum()
                 cls_l = cls_l + bce(rws[:, :nc], F.one_hot(L_["lab"][gi], nc).to(self.dtype), reduction="sum")
                 obj_l = obj_l + bce(rws[:, nc + 4], torch.ones_like(rws[:, nc + 4]), reduction="sum")
-            h, w = L_["h"], L_["w"]
+            h, w, a = L_["h"], L_["w"], pri.shape[0]
             with torch.no_grad():
                 occ = torch.zeros((h, w), dtype=torch.bool, device=self.device)
                 occ[L_["fl"][:, 0], L_["fl"][:, 1]] = True
-                cy = (torch.arange(h, device=self.device, dtype=self.dtype) + 0.5).view(h, 1, 1, 1).expand(h, w, 3, 1)
-                cx = (torch.arange(w, device=self.device, dtype=self.dtype) + 0.5).view(1, w, 1, 1).expand(h, w, 3, 1)
+                cy = (torch.arange(h, device=self.device, dtype=self.dtype) + 0.5).view(h, 1, 1, 1).expand(h, w, a, 1)
+                cx = (torch.arange(w, device=self.device, dtype=self.dtype) + 0.5).view(1, w, 1, 1).expand(h, w, a, 1)
                 ayx = torch.cat([cy, cx], dim=-1)
-                yx_nb = ayx - pri.view(1, 1, 3, 2) / 2.0        # really y1x1, re-used as a centre (:249-262)
-                hw_nb = ayx + pri.view(1, 1, 3, 2) / 2.0        # really y2x2, re-used as a size
+                yx_nb = ayx - pri.view(1, 1, a, 2) / 2.0        # really y1x1, re-used as a centre (:249-262)
+                hw_nb = ayx + pri.view(1, 1, a, 2) / 2.0        # really y2x2, re-used as a size
                 b1 = (yx_nb - hw_nb / 2.0)[..., None, :]
                 b2 = (yx_nb + hw_nb / 2.0)[..., None, :]
                 gg1, gg2 = L_["g1"].view(1, 1, 1, -1, 2), L_["g2"].view(1, 1, 1, -1, 2)
