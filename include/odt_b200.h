@@ -317,6 +317,28 @@ int odt_yolo_loss_fwd(const float* head, const odt_tail_params* p, int B, const 
                       float coord_scale, float noobj_scale, float obj_scale, float class_scale,
                       void* scratch, float* loss_out, void* stream);
 
+/* Training-loss gradients, one per family: the family's loss forward (same kernels, same arguments, same
+ * checks, loss_out / info_out bit-identical to the _fwd call) followed by its gradient kernel.
+ *   grad_out: f32 [B,N,num_fg+5], every element written: d loss_out[b] / d head[b], zero where a row has no
+ *   gradient.  It restates the gradient of the training step's autograd loss (odt_b200/train.py):
+ *   RetinaNet: focal (through clamp(p, 1e-8, 1), zero outside) and smooth-L1, / #positives, ignored anchors 0;
+ *   SSD: (softmax - one-hot) / #positives on positives, smooth-L1 / #positives on their boxes,
+ *   (softmax - one-hot(background)) / #mined on the mined negatives only;
+ *   FCOS: per level with GT, IoU loss through exp(), centre-ness BCE, sigmoid focal, / its positive class cells;
+ *   YOLOv3: sigmoid-BCE and squared log-size terms of the assigned (cell, prior) rows, the no-object term on
+ *   the objectness column under its mask, / #GT.
+ * GTs sharing a row add up in GT order; no floating-point atomics: the gradient is bit-identical from run to
+ * run and an image's gradient does not depend on its batch.  scratch: odt_<family>_loss_scratch_bytes. */
+int odt_retina_loss_grad(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
+                         float alpha, float gamma, void* scratch, float* loss_out, float* grad_out, void* stream);
+int odt_ssd_loss_grad(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
+                      void* scratch, float* loss_out, int* info_out, float* grad_out, void* stream);
+int odt_fcos_loss_grad(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
+                       void* scratch, float* loss_out, float* grad_out, void* stream);
+int odt_yolo_loss_grad(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
+                       float coord_scale, float noobj_scale, float obj_scale, float class_scale,
+                       void* scratch, float* loss_out, float* grad_out, void* stream);
+
 /* ------------------------------------------------- classification tail --- */
 /* Global mean pool + arg-max (+ sparse softmax cross-entropy) of RetinaNet's ImageNet-pretraining mode.
  *   feat: activation `dtype` [B][H+2*halo][W+2*halo][ld], real channels [0, C) (C <= 4096, ld >= C); the halo

@@ -910,22 +910,28 @@ class Tail:
         self.level_fn, self.cap = level_fn, cap
         self.pool_cap = 8 << 20  # box-pool entries (16 B each) for lists beyond the shared-memory window
 
-    def prepare(self, net, head_buf=None):
-        dev = net.device
-        B, N = net.batch, net.N
-        self.head_buf = net.head_buf if head_buf is None else head_buf  # the candidate rows this tail reads
+    def params(self, levels):
+        """odt_tail_params of this tail over the (H, W, A) level table, candidate order: what `prepare` hands the
+        decode / NMS / loss kernels, and what the training step hands the loss kernels for the same network."""
+        N = sum(h * w * a for h, w, a in levels)
         p = L.TailParams()
-        p.kind, p.num_levels, p.N = self.kind, len(net.levels), N
+        p.kind, p.num_levels, p.N = self.kind, len(levels), N
         p.num_fg, p.nms_classes = self.num_fg, self.nms_classes
         p.score_thr, p.iou_thr, p.max_boxes = self.score_thr, self.iou_thr, self.max_boxes
         p.cap = self.cap or N
         off = 0
-        for i, (h, w, a) in enumerate(net.levels):
+        for i, (h, w, a) in enumerate(levels):
             lv = p.level[i]
             lv.H, lv.W, lv.A, lv.offset = h, w, a, off
             self.level_fn(i, h, w, lv)
             off += h * w * a
-        self.p = p
+        return p
+
+    def prepare(self, net, head_buf=None):
+        dev = net.device
+        B = net.batch
+        self.head_buf = net.head_buf if head_buf is None else head_buf  # the candidate rows this tail reads
+        self.p = p = self.params(net.levels)
         self.cand_keys = torch.zeros((B, self.num_fg, p.cap), dtype=torch.int64, device=dev)
         self.cand_count = torch.zeros((B, self.num_fg), dtype=torch.int32, device=dev)
         D = self.nms_classes * self.max_boxes
@@ -975,6 +981,14 @@ class Tail:
         the family's scalars (LOSS_SCALARS) as keywords.  ground_truth [B,G,5] (y,x,h,w,id) padded with -1.
         Returns float32 [B]; for 'ssd' with return_info=True also int32 [B,3] = (#positives, #negatives,
         #mined negatives) per image."""
+        return self._loss_call(net, kind, ground_truth, return_info, False, kw)
+
+    def loss_grad(self, net, kind, ground_truth, return_info=False, **kw):
+        """odt_<kind>_loss_grad on the rows this tail reads (arguments as `loss`): (loss float32 [B], gradient
+        d loss[b] / d rows[b] float32 [B,N,row]), and for 'ssd' with return_info=True the info as a third item."""
+        return self._loss_call(net, kind, ground_truth, return_info, True, kw)
+
+    def _loss_call(self, net, kind, ground_truth, return_info, with_grad, kw):
         if kind not in self.LOSS_SCALARS:
             raise ValueError(kind)
         if return_info and kind != "ssd":
@@ -987,14 +1001,21 @@ class Tail:
         scratch = torch.zeros((nbytes + 7) // 8, dtype=torch.int64, device=net.device)
         out = torch.zeros(B, dtype=torch.float32, device=net.device)
         info = torch.zeros((B, 3), dtype=torch.int32, device=net.device) if return_info else None
+        grad = torch.empty_like(self.head_buf) if with_grad else None
         args = [float(kw.get(k, d)) for k, d in self.LOSS_SCALARS[kind]] + [scratch.data_ptr(), out.data_ptr()]
         if kind == "ssd":
             args.append(None if info is None else info.data_ptr())
-        L.check(getattr(net.lib, "odt_%s_loss_fwd" % kind)(self.head_buf.data_ptr(), p, B, gt.data_ptr(), G, *args,
-                                                          torch.cuda.current_stream().cuda_stream), kind + "_loss")
+        if with_grad:
+            args.append(grad.data_ptr())
+        fn = "odt_%s_loss_%s" % (kind, "grad" if with_grad else "fwd")
+        L.check(getattr(net.lib, fn)(self.head_buf.data_ptr(), p, B, gt.data_ptr(), G, *args,
+                                     torch.cuda.current_stream().cuda_stream), kind + ("_loss_grad" if with_grad else "_loss"))
+        res = [out.cpu().numpy()]
+        if with_grad:
+            res.append(grad.cpu().numpy())
         if return_info:
-            return out.cpu().numpy(), info.cpu().numpy()
-        return out.cpu().numpy()
+            res.append(info.cpu().numpy())
+        return res[0] if len(res) == 1 else tuple(res)
 
     def num_launches(self):
         return 2  # decode + NMS kernels (plus 3 memset nodes)
@@ -1003,6 +1024,30 @@ class Tail:
         """ONE D2H read of the packed records -> per-image [scores f32[K], bbox f32[K,4] (y1,x1,y2,x2),
         class_id i32[K]] (ref SSD300.py:190)."""
         return unpack_records(self.rec.cpu().numpy(), self.p.cap)
+
+
+MAX_LOSS_GT = 128  # GT rows per image the loss kernels hold (kMaxGT in csrc/loss.cu)
+
+
+def loss_ground_truth(ground_truth):
+    """Ground truth [B,G,5] (y,x,h,w,id) padded with -1 -> float32 ndarray the loss kernels take.  An image's box
+    count is the index of its first minimum in column 0 (the reference's argmin).  When G exceeds the kernels' 128
+    rows, the array is cut to the rows the counts reach (max count + 1 rows keep every count: no earlier row holds the
+    minimum), computed here in numpy; an image whose count needs more than 128 rows (128 boxes or more ahead of its
+    first padding row) is a ValueError."""
+    gt = np.ascontiguousarray(ground_truth, dtype=np.float32)
+    if gt.ndim != 3 or gt.shape[2] != 5 or gt.shape[1] < 1:
+        raise ValueError("ground truth: expected shape [B, G, 5] with G >= 1, got %s" % (gt.shape,))
+    if gt.shape[1] <= MAX_LOSS_GT:
+        return gt
+    cnt = np.argmin(gt[:, :, 0], axis=1)
+    need = int(cnt.max()) + 1
+    if need > MAX_LOSS_GT:
+        b = int(np.argmax(cnt))
+        raise ValueError("ground truth: image %d has %d boxes ahead of its first padding row; the loss kernels hold %d "
+                         "GT rows per image, so at most %d boxes when the rows are padded beyond %d"
+                         % (b, int(cnt[b]), MAX_LOSS_GT, MAX_LOSS_GT - 1, MAX_LOSS_GT))
+    return np.ascontiguousarray(gt[:, :need])
 
 
 def check_class_labels(labels, batch, num_classes):
@@ -1125,6 +1170,10 @@ class RowsHarness:
     def loss(self, kind, ground_truth, return_info=False, **kw):
         """Training-loss forward kernels on the same rows (Tail.loss)."""
         return self.tail.loss(self, kind, ground_truth, return_info, **kw)
+
+    def loss_grad(self, kind, ground_truth, return_info=False, **kw):
+        """Training-loss gradient kernels on the same rows (Tail.loss_grad): (loss [B], gradient [B,N,row])."""
+        return self.tail.loss_grad(self, kind, ground_truth, return_info, **kw)
 
 
 # ------------------------------------------------------------------ weights --

@@ -95,6 +95,10 @@ SYMBOLS = {
     "odt_yolo_loss_fwd": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _F, _F, _F, _F, _P, _P, _P]),
     "odt_fcos_loss_scratch_bytes": (_L, [C.POINTER(TailParams), _I]),
     "odt_fcos_loss_fwd": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _P, _P, _P]),
+    "odt_retina_loss_grad": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _F, _F, _P, _P, _P, _P]),
+    "odt_ssd_loss_grad": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _P, _P, _P, _P, _P]),
+    "odt_yolo_loss_grad": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _F, _F, _F, _F, _P, _P, _P, _P]),
+    "odt_fcos_loss_grad": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _P, _P, _P, _P]),
     "odt_pool_classify": (_I, [_P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
     "odt_ctx_unique_id": (_I, [_P]),
     "odt_ctx_create": (_I, [C.POINTER(_P), _I, _I, _P]),

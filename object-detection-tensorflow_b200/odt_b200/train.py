@@ -271,6 +271,11 @@ class GraphTrainer:
                 self.slots[name] = torch.zeros_like(t)
         self.global_step = int(getattr(model, "global_step", 0))
         self._anchor_cache = None
+        # CUDA, fp32 rows: the data term is the family's loss-gradient kernel (csrc/loss.cu) behind one autograd
+        # Function; the CPU (and float64) keep the restatement below, which the kernels are tested against
+        self._loss_kernels = None
+        if self.kind in ("ssd", "retina", "yolo", "fcos") and self.device.type == "cuda" and dtype == torch.float32:
+            self._loss_kernels = LossKernels(self)
         if self.kind == "ssd":
             self._ssd = SSDTrainer.__new__(SSDTrainer)   # borrows the SSD loss / anchors
             self._ssd.device, self._ssd.dtype, self._ssd.size, self._ssd._anchors = self.device, dtype, model.input_size, None
@@ -528,8 +533,12 @@ class GraphTrainer:
         return {"retina": self.retina_image_loss, "fcos": self.fcos_image_loss, "yolo": self.yolo_image_loss}[self.kind](row, gt)
 
     def total_loss(self, rows, ground_truth):
-        per = [self.image_loss(rows[b], ground_truth[b]) for b in range(rows.shape[0])]
-        data = torch.stack([torch.as_tensor(p, device=self.device, dtype=self.dtype) for p in per]).sum() / rows.shape[0]
+        if self._loss_kernels is not None:
+            data = self._loss_kernels(rows, ground_truth).sum() / rows.shape[0]
+        else:
+            per = [self.image_loss(rows[b], ground_truth[b]) for b in range(rows.shape[0])]
+            data = torch.stack([torch.as_tensor(p, device=self.device, dtype=self.dtype) for p in per]).sum() \
+                / rows.shape[0]
         if self.kind == "yolo":
             data = 0.5 * data                                   # YOLOv3.py:313
         l2 = sum((p * p).sum() for p in self.params.values()) * 0.5
@@ -574,6 +583,71 @@ class GraphTrainer:
         return float(loss.detach())
 
     export = SSDTrainer.export
+
+
+class _RowsLoss(torch.autograd.Function):
+    """Per-image losses [B] of the candidate rows [B, N, row] by one odt_<family>_loss_grad launch; the backward
+    scales the gradient the same launch wrote by the incoming per-image weights."""
+
+    @staticmethod
+    def forward(ctx, rows, kernels, gt):
+        loss, grad = kernels.launch(rows, gt)
+        ctx.grad = grad         # the trainer's buffer: read by this step's backward, rewritten by the next launch
+        return loss.clone()
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        return ctx.grad * grad_output.view(-1, 1, 1), None, None
+
+
+class LossKernels:
+    """The training step's data term on the GPU: the family's loss and its gradient with respect to the candidate
+    rows, from the CUDA kernels (odt_<family>_loss_grad), on the tail parameters the inference engine builds for the
+    same network.  Scratch, loss and gradient buffers are allocated once per batch size.  Ground truth goes through
+    engine.loss_ground_truth (at most 128 GT rows per image)."""
+
+    def __init__(self, trainer):
+        from . import lib as L
+        self.E, self.L, self.lib = trainer.E, L, L.load()
+        self.kind, self.device, self.row = trainer.kind, trainer.device, trainer.row
+        self.p = trainer.net.tail.params(trainer.net.levels)
+        self.N = self.p.N
+        cfg = trainer.cfg
+        self.scalars = [float(cfg.get(k, d)) for k, d in trainer.E.Tail.LOSS_SCALARS[self.kind]]
+        self.fn = getattr(self.lib, "odt_%s_loss_grad" % self.kind)
+        self._bufs = {}
+
+    def _buffers(self, B):
+        if B not in self._bufs:
+            import ctypes as C
+            nbytes = getattr(self.lib, "odt_%s_loss_scratch_bytes" % self.kind)(C.byref(self.p), B)
+            self._bufs[B] = (torch.zeros((nbytes + 7) // 8, dtype=torch.int64, device=self.device),
+                             torch.zeros((B,), dtype=torch.float32, device=self.device),
+                             torch.empty((B, self.N, self.row), dtype=torch.float32, device=self.device))
+        return self._bufs[B]
+
+    def launch(self, rows, gt):
+        """rows fp32 [B, N, row] on the device, gt a float32 ndarray from loss_ground_truth -> (loss [B], gradient
+        [B, N, row]); both are views of this object's buffers, valid until the next launch with the same B."""
+        import ctypes as C
+        B = rows.shape[0]
+        assert rows.shape[1:] == (self.N, self.row) and rows.dtype == torch.float32
+        rows = rows.contiguous()
+        scratch, loss, grad = self._buffers(B)
+        g = torch.from_numpy(gt).to(self.device)
+        args = self.scalars + [scratch.data_ptr(), loss.data_ptr()]
+        if self.kind == "ssd":
+            args.append(None)
+        self.L.check(self.fn(rows.data_ptr(), C.byref(self.p), B, g.data_ptr(), g.shape[1], *args, grad.data_ptr(),
+                             torch.cuda.current_stream().cuda_stream), "%s_loss_grad" % self.kind)
+        return loss, grad
+
+    def __call__(self, rows, ground_truth):
+        """Per-image losses [B] with the kernels' gradient attached to `rows`."""
+        gt = self.E.loss_ground_truth(ground_truth)
+        if gt.shape[0] != rows.shape[0]:
+            raise ValueError("ground truth for %d images, rows for %d" % (gt.shape[0], rows.shape[0]))
+        return _RowsLoss.apply(rows, self, gt)
 
 
 def pooled_xent(features, labels):
