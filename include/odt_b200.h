@@ -339,6 +339,55 @@ int odt_yolo_loss_grad(const float* head, const odt_tail_params* p, int B, const
                        float coord_scale, float noobj_scale, float obj_scale, float class_scale,
                        void* scratch, float* loss_out, float* grad_out, void* stream);
 
+/* ------------------------------------------------ training augmentation --- */
+/* image_augmentor's pixel work (utils/image_augmentor.py:7-264, as odt_b200/tfrecord.py's augment_pixels restates
+ * it) for a batch of uint8 RGB sources of any sizes; the random draws, box arithmetic and the float32 scalars
+ * derived from the draws (tfrecord.plan_augment) stay on the host.  Per output pixel (y, x) of an oh x ow image:
+ *   flips (y -> oh-1-y, x -> ow-1-x), + crop -> canvas pixel (zy, zx) of a zh x zw canvas; inside the inner
+ *   rh x rw rectangle at its top-left the resize mode's sample, elsewhere cval:
+ *     BILINEAR / NEAREST / BICUBIC: align_corners resize of h x w to rh x rw (TF 1.13's kernels; bicubic
+ *       table-driven, A = -0.75, taps clamped);  PAD: the source pixel itself (CONSTANT fill, rh, rw = min(h, zh),
+ *       min(w, zw));  LEGACY: gt_checker_helper's fallback, TF1 bilinear (no align_corners) of the whole source to
+ *       oh x ow, no canvas, crop, flip, jitter or rotation;
+ *   then brightness (+ delta), contrast ((v - mean) * factor + mean, the per-channel mean of the image so far,
+ *   summed in fp64 in a fixed order and rounded once), hue (hue6 = float32(delta) * 6), each where it fired, and
+ *   the rotation: bilinear gather at (c x - s y + x_off, s x + c y + y_off), neighbours outside read 0.
+ * Every operation is numpy's, rounded as numpy rounds it (fp32 without FMA; fp64 where numpy promotes).
+ *   src: uint8 HWC RGB sources, image b at byte src_offset;  out: f32 [B,oh,ow,3] (NHWC) or [B,3,oh,ow] (NCHW);
+ *   means_out: f32 [B,3] or NULL: the contrast means (NaN rows where contrast did not fire);
+ *   scratch: odt_augment_scratch_bytes(params_host, B) bytes (-1 for parameters odt_augment_batch rejects).
+ * All images share oh, ow and the layout.  Deterministic; an image's output does not depend on its batch. */
+#define ODT_AUG_BILINEAR 0
+#define ODT_AUG_NEAREST 1
+#define ODT_AUG_BICUBIC 2
+#define ODT_AUG_PAD 3
+#define ODT_AUG_LEGACY 4
+#define ODT_AUG_NHWC 0
+#define ODT_AUG_NCHW 1
+typedef struct {
+  long long src_offset;
+  int h, w;                 /* source size */
+  int mode;                 /* ODT_AUG_* resize mode */
+  int zh, zw;               /* canvas (zoom) size */
+  int rh, rw;               /* inner rectangle of the resized source */
+  float cval;               /* canvas value outside it */
+  int crop_y, crop_x;       /* window of oh x ow on the canvas */
+  int flip_y, flip_x;
+  int brightness_on;
+  float brightness;         /* float32(delta) */
+  int contrast_on;
+  float contrast;           /* float32(factor) */
+  int hue_on;
+  float hue6;               /* float32(delta) * 6 */
+  int rotate_on;
+  float rot_c, rot_s, rot_x_off, rot_y_off;
+  int oh, ow;               /* output size */
+  int layout;               /* ODT_AUG_NHWC / ODT_AUG_NCHW */
+} odt_augment_params;
+long long odt_augment_scratch_bytes(const odt_augment_params* params_host, int B);
+int odt_augment_batch(const uint8_t* src, const odt_augment_params* params_host, int B, float* out,
+                      float* means_out, void* scratch, void* stream);
+
 /* ------------------------------------------------- classification tail --- */
 /* Global mean pool + arg-max (+ sparse softmax cross-entropy) of RetinaNet's ImageNet-pretraining mode.
  *   feat: activation `dtype` [B][H+2*halo][W+2*halo][ld], real channels [0, C) (C <= 4096, ld >= C); the halo

@@ -37,6 +37,22 @@ def _as_host_tensor(images):
     return torch.from_numpy(np.ascontiguousarray(images, dtype=np.float32))
 
 
+def _next_batch(iterator, tr, data_format):
+    """The next training batch, NHWC.  A tfrecord BatchIterator feeding a CUDA trainer augments on the trainer's
+    device (get_next(device): the same batch, made by the augmentation kernels); any other iterator, and a CPU
+    trainer, take the numpy batch."""
+    from .tfrecord import BatchIterator
+    if isinstance(iterator, BatchIterator) and tr.device.type == "cuda":
+        images, truth = iterator.get_next(tr.device)
+        if data_format == "channels_first":
+            images = images.permute(0, 2, 3, 1)
+        return images, truth
+    images, truth = iterator.get_next()
+    if data_format == "channels_first":
+        images = np.transpose(np.asarray(images), (0, 2, 3, 1))
+    return images, truth
+
+
 def _precision(config):
     return config.get("precision", os.environ.get("ODT_PRECISION", "fp16"))
 
@@ -385,9 +401,7 @@ class _Detector:
         num_iters = self.num_train // self.batch_size
         mean_loss = []
         for i in range(num_iters):
-            images, gt = self.train_iterator.get_next()
-            if self.data_format == "channels_first":
-                images = np.transpose(np.asarray(images), (0, 2, 3, 1))
+            images, gt = _next_batch(self.train_iterator, tr, self.data_format)
             loss = tr.step(images, gt, lr)
             sys.stdout.write("\r>> iters %d/%d loss %s" % (i, num_iters, loss))
             sys.stdout.flush()
@@ -552,9 +566,7 @@ class RetinaNet(_Detector):
         num_iters = self.num_train // self.batch_size
         losses, accs = [], []
         for i in range(num_iters):
-            images, labels = self.train_iterator.get_next()
-            if self.data_format == "channels_first":
-                images = np.transpose(np.asarray(images), (0, 2, 3, 1))
+            images, labels = _next_batch(self.train_iterator, tr, self.data_format)
             loss, acc = tr.step(images, labels, lr)
             losses.append(loss)
             accs.append(acc)

@@ -59,6 +59,23 @@ class TailParams(C.Structure):
     ]
 
 
+AUG_BILINEAR, AUG_NEAREST, AUG_BICUBIC, AUG_PAD, AUG_LEGACY = 0, 1, 2, 3, 4
+AUG_NHWC, AUG_NCHW = 0, 1
+
+
+class AugmentParams(C.Structure):
+    """Mirror of odt_augment_params."""
+    _fields_ = [
+        ("src_offset", C.c_longlong), ("h", C.c_int), ("w", C.c_int), ("mode", C.c_int),
+        ("zh", C.c_int), ("zw", C.c_int), ("rh", C.c_int), ("rw", C.c_int), ("cval", C.c_float),
+        ("crop_y", C.c_int), ("crop_x", C.c_int), ("flip_y", C.c_int), ("flip_x", C.c_int),
+        ("brightness_on", C.c_int), ("brightness", C.c_float), ("contrast_on", C.c_int), ("contrast", C.c_float),
+        ("hue_on", C.c_int), ("hue6", C.c_float),
+        ("rotate_on", C.c_int), ("rot_c", C.c_float), ("rot_s", C.c_float), ("rot_x_off", C.c_float),
+        ("rot_y_off", C.c_float), ("oh", C.c_int), ("ow", C.c_int), ("layout", C.c_int),
+    ]
+
+
 # every symbol include/odt_b200.h declares: name -> (restype, argtypes)
 _P, _I, _L, _F = C.c_void_p, C.c_int, C.c_longlong, C.c_float
 SYMBOLS = {
@@ -99,6 +116,8 @@ SYMBOLS = {
     "odt_ssd_loss_grad": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _P, _P, _P, _P, _P]),
     "odt_yolo_loss_grad": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _F, _F, _F, _F, _P, _P, _P, _P]),
     "odt_fcos_loss_grad": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _P, _P, _P, _P]),
+    "odt_augment_scratch_bytes": (_L, [C.POINTER(AugmentParams), _I]),
+    "odt_augment_batch": (_I, [_P, C.POINTER(AugmentParams), _I, _P, _P, _P, _P]),
     "odt_pool_classify": (_I, [_P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
     "odt_ctx_unique_id": (_I, [_P]),
     "odt_ctx_create": (_I, [C.POINTER(_P), _I, _I, _P]),

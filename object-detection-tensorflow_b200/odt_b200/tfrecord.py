@@ -1,6 +1,7 @@
 """TFRecord + tf.train.Example reader / writer and the VOC record schema of the reference's
 input pipeline (utils/tfrecord_voc_utils.py:30-113), without TensorFlow.  Host-side IO for
-SURVEY section 8(f) row 3; not on the accelerated hot path.
+SURVEY section 8(f) row 3.  The augmentation's pixel step also runs as CUDA kernels (odt_b200/augment.py,
+`BatchIterator.get_next(device)`); everything else here is host-side.
 
 * TFRecord framing: u64 length | u32 masked crc32c(length) | payload | u32 masked crc32c(payload).
 * tf.train.Example: Example{1: Features{1: map<string, Feature>}}, Feature = oneof
@@ -324,9 +325,13 @@ def adjust_brightness(img, delta):
     return (img + np.float32(delta)).astype(np.float32)
 
 
-def adjust_contrast(img, factor):
-    """tf.image.adjust_contrast: (x - mean) * factor + mean with the mean of each channel over H, W."""
-    mean = img.mean(axis=(0, 1), keepdims=True, dtype=np.float32)
+def adjust_contrast(img, factor, mean=None):
+    """tf.image.adjust_contrast: (x - mean) * factor + mean with the mean of each channel over H, W.  `mean` (3
+    float32) replaces numpy's own float32 mean, so that a mean computed elsewhere can be applied bit for bit."""
+    if mean is None:
+        mean = img.mean(axis=(0, 1), keepdims=True, dtype=np.float32)
+    else:
+        mean = np.asarray(mean, np.float32).reshape(1, 1, -1)
     return ((img - mean) * np.float32(factor) + mean).astype(np.float32)
 
 
@@ -356,14 +361,20 @@ def adjust_hue(img, delta):
     return np.stack([r2, g2, b2], -1).astype(np.float32)
 
 
+def rotation_coefficients(angle, h, w):
+    """(cos, sin, x_off, y_off) of `rotate_bilinear` on an h x w image, float32 as numpy computes them."""
+    c, s = np.float32(np.cos(angle)), np.float32(np.sin(angle))
+    x_off = np.float32(((w - 1) - (c * (w - 1) - s * (h - 1))) / 2.0)
+    y_off = np.float32(((h - 1) - (s * (w - 1) + c * (h - 1))) / 2.0)
+    return c, s, x_off, y_off
+
+
 def rotate_bilinear(img, angle):
     """tf.contrib.image.rotate(img, angle, 'BILINEAR'): counter-clockwise by `angle` (radians) about the
     image centre; output pixel (x, y) samples input (cos*x - sin*y + x_off, sin*x + cos*y + y_off) with the
     offsets of angles_to_projective_transforms; neighbours outside the image read 0."""
     h, w = img.shape[:2]
-    c, s = np.float32(np.cos(angle)), np.float32(np.sin(angle))
-    x_off = np.float32(((w - 1) - (c * (w - 1) - s * (h - 1))) / 2.0)
-    y_off = np.float32(((h - 1) - (s * (w - 1) + c * (h - 1))) / 2.0)
+    c, s, x_off, y_off = rotation_coefficients(angle, h, w)
     xs, ys = np.meshgrid(np.arange(w, dtype=np.float32), np.arange(h, dtype=np.float32))
     sx = c * xs - s * ys + x_off
     sy = s * xs + c * ys + y_off
@@ -395,13 +406,42 @@ def rotate_boxes(angle, ymin, xmin, ymax, xmax, oh, ow):
             np.maximum.reduce(py).astype(np.float32), np.maximum.reduce(px).astype(np.float32))
 
 
-def preprocess(img, gt, config, rng=None):
-    """image_augmentor (utils/image_augmentor.py:7-233): resize (or aspect-preserving resize + constant padding) to
-    `zoom_size` / `output_shape`, centre or random crop, top-down / left-right flips, colour jitter, rotation, box
-    clamping and the centre-inside filter, conversion to (y_c, x_c, h, w, id), `pad_truth_to`.  Randomness comes
-    from the seeded numpy generator `rng` (TF's generator is not reproducible outside TF); without one the
-    random steps are skipped.  gt=None (`image_augmentor(ground_truth=None)`, the ImageNet path) returns the
-    image alone."""
+class AugmentPlan:
+    """Everything `preprocess` decides for one image without touching its pixels: the resize mode and geometry, the
+    crop, the flips and the drawn jitter / rotation values (the raw draws for the numpy step, and the float32
+    scalars numpy derives from them for the CUDA kernels of odt_b200/augment.py).
+
+      mode       'bilinear' | 'nearest' | 'bicubic': resize the source to the inner rh x rw rectangle at the
+                 top-left of a zh x zw canvas of `cval` (rh, rw = zh, zw unless the aspect ratio is kept);
+                 'pad': the CONSTANT fill mode, the source copied into that corner as it is, rh, rw = min(h, zh),
+                 min(w, zw); 'legacy': the `gt_checker_helper` fallback, the original image through TF1's
+                 half-pixel-free bilinear resize to oh x ow, nothing else applied.
+      crop       (ch, cw) window of oh x ow on the canvas, or None without `zoom_size` (the canvas is oh x ow)
+      brightness, contrast, hue, angle: the drawn value, or None where the step did not fire."""
+    __slots__ = ("h", "w", "mode", "zh", "zw", "rh", "rw", "cval", "crop", "oh", "ow", "flip_y", "flip_x",
+                 "brightness", "contrast", "hue", "angle", "channels_first")
+
+    def __init__(self, **kw):
+        for k in self.__slots__:
+            setattr(self, k, kw.pop(k, None))
+        assert not kw, kw
+
+    def __repr__(self):
+        return "AugmentPlan(%s)" % ", ".join("%s=%r" % (k, getattr(self, k)) for k in self.__slots__)
+
+    @property
+    def rotation(self):
+        """(cos, sin, x_off, y_off) float32 of the rotation, or None."""
+        return None if self.angle is None else rotation_coefficients(self.angle, self.oh, self.ow)
+
+
+_RESIZE = {"NEAREST_NEIGHBOR": "nearest", "BICUBIC": "bicubic"}
+
+
+def plan_augment(h, w, gt, config, rng=None):
+    """The pixel-free half of `preprocess` for an h x w source: argument checks, every random draw (same order, same
+    conditions), the box arithmetic, the fallback decision and `pad_truth_to`.  -> (AugmentPlan, boxes), boxes None
+    when gt is None.  `augment_pixels(img, plan)` then gives preprocess's image bit for bit."""
     no_boxes = gt is None
     if no_boxes:
         gt = np.zeros((0, 5), np.float32)
@@ -415,27 +455,22 @@ def preprocess(img, gt, config, rng=None):
     cj = config.get("color_jitter_prob")
     if cj is not None and not 0.0 <= cj <= 1.0:
         raise ValueError("color_jitter_prob can't be less than 0.0 or greater than 1.0")
-    img_copy, gt_copy = img, gt
+    gt_copy = gt
     zoom = config.get("zoom_size")
     zh, zw = (zoom if zoom is not None else (oh, ow))
-    h, w = img.shape[:2]
     ymin, ymax, xmin, xmax = [gt[:, i].astype(np.float32) for i in range(4)]
     fill = config.get("fill_mode", "BILINEAR")
     keep = bool(config.get("keep_aspect_ratios")) or fill == "CONSTANT"
-    resize = {"NEAREST_NEIGHBOR": _resize_nearest_aligned, "BICUBIC": _resize_bicubic_aligned}.get(
-        fill, _resize_bilinear_aligned)
-    cval = np.float32(config.get("constant_values") or 0.0)
+    p = AugmentPlan(h=h, w=w, mode=_RESIZE.get(fill, "bilinear"), zh=zh, zw=zw, rh=zh, rw=zw, oh=oh, ow=ow,
+                    cval=np.float32(config.get("constant_values") or 0.0), flip_y=False, flip_x=False,
+                    channels_first=config.get("data_format") == "channels_first")
     if keep and fill != "CONSTANT":           # :93-114
         ratio = np.float32(min(zh / h, zw / w))
-        rh, rw = (zh, int(np.float32(w) * ratio)) if zh / h < zw / w else (int(np.float32(h) * ratio), zw)
-        out = np.full((zh, zw, img.shape[2]), cval, np.float32)
-        out[:rh, :rw] = resize(img, rh, rw)
+        p.rh, p.rw = (zh, int(np.float32(w) * ratio)) if zh / h < zw / w else (int(np.float32(h) * ratio), zw)
         ymin, ymax, xmin, xmax = ymin * ratio, ymax * ratio, xmin * ratio, xmax * ratio
     elif keep:                                # CONSTANT: pad only (:115-119)
-        out = np.full((zh, zw, img.shape[2]), cval, np.float32)
-        out[:min(h, zh), :min(w, zw)] = img[:zh, :zw]
+        p.mode, p.rh, p.rw = "pad", min(h, zh), min(w, zw)
     else:                                     # :121-131
-        out = resize(img, zh, zw)
         ry, rx = np.float32(zh / h), np.float32(zw / w)
         ymin, ymax, xmin, xmax = ymin * ry, ymax * ry, xmin * rx, xmax * rx
     if zoom is not None:                      # :133-147
@@ -444,29 +479,28 @@ def preprocess(img, gt, config, rng=None):
             cw = int(rng.integers(0, zw - ow)) if zw > ow else 0
         else:
             ch, cw = (zh - oh) // 2, (zw - ow) // 2
-        out = out[ch:ch + oh, cw:cw + ow]
+        p.crop = (ch, cw)
         ymin, ymax, xmin, xmax = ymin - ch, ymax - ch, xmin - cw, xmax - cw
     flip = config.get("flip_prob")
     if flip is not None and rng is not None:  # :149-173 (note the reference's "- 1." offsets)
         if rng.random() < flip[0]:
-            out = out[::-1]
+            p.flip_y = True
             ymax, ymin = oh - ymin - 1.0, oh - ymax - 1.0
         if rng.random() < flip[1]:
-            out = out[:, ::-1]
+            p.flip_x = True
             xmax, xmin = ow - xmin - 1.0, ow - xmax - 1.0
     if cj is not None and rng is not None:    # :174-187 (deltas drawn only when the step fires, like tf.cond)
         bcs = rng.random(3)
         if bcs[0] < cj:
-            out = adjust_brightness(out, rng.uniform(0.0, 0.3))
+            p.brightness = rng.uniform(0.0, 0.3)
         if bcs[1] < cj:
-            out = adjust_contrast(out, rng.uniform(0.8, 1.2))
+            p.contrast = rng.uniform(0.8, 1.2)
         if bcs[2] < cj:
-            out = adjust_hue(out, rng.uniform(-0.1, 0.1))
+            p.hue = rng.uniform(-0.1, 0.1)
     if rot is not None and rng is not None:   # :189-196
         if rng.random() < rot[0]:
-            ang = np.float32(rng.uniform(rot[1], rot[2]) * 3.1415926 / 180.0)
-            out = rotate_bilinear(out, ang)
-            ymin, xmin, ymax, xmax = rotate_boxes(ang, ymin, xmin, ymax, xmax, float(oh), float(ow))
+            p.angle = np.float32(rng.uniform(rot[1], rot[2]) * 3.1415926 / 180.0)
+            ymin, xmin, ymax, xmax = rotate_boxes(p.angle, ymin, xmin, ymax, xmax, float(oh), float(ow))
     lim_y, lim_x = np.float32(oh - 1), np.float32(ow - 1)   # :199-218
     ymin, ymax = np.clip(ymin, 0, lim_y), np.clip(ymax, 0, lim_y)
     xmin, xmax = np.clip(xmin, 0, lim_x), np.clip(xmax, 0, lim_x)
@@ -474,7 +508,8 @@ def preprocess(img, gt, config, rng=None):
     m = (yc > 0) & (yc < lim_y) & (xc > 0) & (xc < lim_x)
     box = np.stack([yc[m], xc[m], (ymax - ymin)[m], (xmax - xmin)[m], gt[:, 4][m]], -1).astype(np.float32)
     if len(box) == 0 and len(gt_copy):        # gt_checker_helper (:220-225,:259-264): plain resize of the original
-        out = _resize_bilinear_legacy(img_copy, oh, ow)
+        p.mode, p.zh, p.zw, p.rh, p.rw, p.crop, p.flip_y, p.flip_x = "legacy", oh, ow, oh, ow, None, False, False
+        p.brightness = p.contrast = p.hue = p.angle = None
         fy, fx = np.float32(oh) / np.float32(h), np.float32(ow) / np.float32(w)
         g = gt_copy.astype(np.float32)
         box = np.stack([(g[:, 0] / 2 + g[:, 1] / 2) * fy, (g[:, 2] / 2 + g[:, 3] / 2) * fx,
@@ -485,56 +520,127 @@ def preprocess(img, gt, config, rng=None):
         n = min(len(box), int(pad))
         full[:n] = box[:n]
         box = full
-    if config.get("data_format") == "channels_first":
+    return p, (None if no_boxes else box)
+
+
+_RESIZE_FN = {"bilinear": _resize_bilinear_aligned, "nearest": _resize_nearest_aligned,
+              "bicubic": _resize_bicubic_aligned}
+
+
+def augment_pixels(img, plan, means=None):
+    """The pixel half of `preprocess`: `img` (uint8 or float [h, w, c]) through `plan`.  `means` (3 float32) stands
+    in for numpy's own channel means in the contrast step, e.g. the means the CUDA kernels computed."""
+    p = plan
+    if p.mode == "legacy":
+        out = _resize_bilinear_legacy(img, p.oh, p.ow)
+    else:
+        if p.mode == "pad":
+            out = np.full((p.zh, p.zw, img.shape[2]), p.cval, np.float32)
+            out[:p.rh, :p.rw] = img[:p.zh, :p.zw]
+        elif (p.rh, p.rw) == (p.zh, p.zw):
+            out = _RESIZE_FN[p.mode](img, p.zh, p.zw)
+        else:
+            out = np.full((p.zh, p.zw, img.shape[2]), p.cval, np.float32)
+            out[:p.rh, :p.rw] = _RESIZE_FN[p.mode](img, p.rh, p.rw)
+        if p.crop is not None:
+            ch, cw = p.crop
+            out = out[ch:ch + p.oh, cw:cw + p.ow]
+        if p.flip_y:
+            out = out[::-1]
+        if p.flip_x:
+            out = out[:, ::-1]
+        if p.brightness is not None:
+            out = adjust_brightness(out, p.brightness)
+        if p.contrast is not None:
+            out = adjust_contrast(out, p.contrast, means)
+        if p.hue is not None:
+            out = adjust_hue(out, p.hue)
+        if p.angle is not None:
+            out = rotate_bilinear(out, p.angle)
+    if p.channels_first:
         out = np.transpose(out, (2, 0, 1))
-    if no_boxes:
-        return np.ascontiguousarray(out, np.float32)
-    return np.ascontiguousarray(out, np.float32), box
+    return np.ascontiguousarray(out, np.float32)
+
+
+def preprocess(img, gt, config, rng=None):
+    """image_augmentor (utils/image_augmentor.py:7-233): resize (or aspect-preserving resize + constant padding) to
+    `zoom_size` / `output_shape`, centre or random crop, top-down / left-right flips, colour jitter, rotation, box
+    clamping and the centre-inside filter, conversion to (y_c, x_c, h, w, id), `pad_truth_to`.  Randomness comes
+    from the seeded numpy generator `rng` (TF's generator is not reproducible outside TF); without one the
+    random steps are skipped.  gt=None (`image_augmentor(ground_truth=None)`, the ImageNet path) returns the
+    image alone.  = `plan_augment` (no pixels) + `augment_pixels`."""
+    plan, box = plan_augment(img.shape[0], img.shape[1], gt, config, rng)
+    out = augment_pixels(img, plan)
+    return out if gt is None else (out, box)
 
 
 preprocess._warned = {}
 
 
+DECODE_THREADS = 4   # JPEG decoding ahead of the consumer (cv2.imdecode releases the GIL)
+DECODE_AHEAD = 16    # records in flight
+
+
 class BatchIterator:
     """`iterator.get_next()` of `get_generator` (utils/tfrecord_voc_utils.py:115-120): endless batches
-    (images float32 [B,...], ground_truth float32 [B,pad,5]); drop_remainder, shuffle buffer, repeat."""
+    (images float32 [B,...], ground_truth float32 [B,pad,5]); drop_remainder, shuffle buffer, repeat.
+
+    Records are decoded ahead on DECODE_THREADS threads and consumed in record order; the random draws (plan_augment
+    per example, then the shuffle buffer's pick) happen in the consumer, in the order `preprocess` made them.  The
+    shuffle buffer holds (uint8 source, AugmentPlan, boxes); the pixels are made when a batch is taken:
+    `get_next()` with numpy, `get_next(device)` with the CUDA kernels of odt_b200/augment.py (the same batch, the
+    images a float32 CUDA tensor in the configured layout).  The decoding threads end with the iterator (`close()`,
+    a new `initialize()`, or garbage collection)."""
 
     def __init__(self, tfrecords, batch_size, buffer_size, config, seed=0):
         self.files = [tfrecords] if isinstance(tfrecords, str) else list(tfrecords)
         self.batch_size, self.buffer_size, self.config = int(batch_size), max(int(buffer_size), 1), dict(config)
         self.rng = np.random.default_rng(seed)
         self._it = None
+        self._gpu = None
 
     def initialize(self):
+        self.close()
         self._it = self._batches()
 
-    def _examples(self):
-        while True:  # .repeat()
-            n = 0
-            for path in self.files:
-                for rec in read_records(path):
-                    n += 1
-                    yield preprocess(*decode_voc_example(rec), self.config, self.rng)
-            if n == 0:
-                raise RecordError("no records in %r" % (self.files,))
+    def close(self):
+        """Stop the decoding threads (the next get_next() starts a fresh stream, like initialize())."""
+        if self._it is not None:
+            self._it.close()
+            self._it = None
 
-    def _shuffled(self):
-        buf = []
-        for ex in self._examples():
-            buf.append(ex)
-            if len(buf) >= self.buffer_size:
-                yield buf.pop(int(self.rng.integers(len(buf))))
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    # The stream is a chain of module-level generators that hold the files, config and generator but not the
+    # iterator itself, so that dropping the iterator closes the chain (and its decoding threads) at once.
+    def _examples(self):
+        return _voc_examples(self.files, self.config, self.rng)
 
     def _batches(self):
-        src = self._shuffled()
-        while True:
-            items = [next(src) for _ in range(self.batch_size)]
-            yield np.stack([i[0] for i in items]), np.stack([i[1] for i in items])
+        return _batches(_shuffled(self._examples(), self.buffer_size, self.rng), self.batch_size)
 
-    def get_next(self):
+    def _next_items(self):
         if self._it is None:
             self.initialize()
         return next(self._it)
+
+    def _images(self, items, device):
+        if device is None:
+            return np.stack([augment_pixels(i[0], i[1]) for i in items])
+        if self._gpu is None:
+            from .augment import GpuAugmentor
+            self._gpu = GpuAugmentor()
+        return self._gpu(items, device)
+
+    def get_next(self, device=None):
+        """The next batch.  device=None: numpy images; a CUDA device: the same images as a float32 tensor there,
+        made by the augmentation kernels on that device's current stream (the truth stays numpy)."""
+        items = self._next_items()
+        return self._images(items, device), np.stack([i[2] for i in items])
 
 
 class ImageNetBatchIterator(BatchIterator):
@@ -542,12 +648,67 @@ class ImageNetBatchIterator(BatchIterator):
     labels int64 [B]) of ImageNet records, each image through `preprocess` without boxes."""
 
     def _examples(self):
+        return _imagenet_examples(self.files, self.config, self.rng)
+
+
+def _records(files):
+    while True:  # .repeat()
+        n = 0
+        for path in files:
+            for rec in read_records(path):
+                n += 1
+                yield rec
+        if n == 0:
+            raise RecordError("no records in %r" % (files,))
+
+
+def _decoded(files, decode):
+    """decode(record) of every record in order, DECODE_AHEAD records ahead on a small thread pool.  An error of the
+    record stream or of a decode is raised where that record's example would have been."""
+    import collections
+    from concurrent.futures import ThreadPoolExecutor
+    from sys import is_finalizing     # a local: module globals may be gone when the generator is finalised at exit
+    src = _records(files)
+    window = collections.deque()
+    pool = ThreadPoolExecutor(DECODE_THREADS, thread_name_prefix="odt-decode")
+    failed = False
+    try:
         while True:
-            n = 0
-            for path in self.files:
-                for rec in read_records(path):
-                    n += 1
-                    img, label = decode_imagenet_example(rec)
-                    yield preprocess(img, None, self.config, self.rng), label
-            if n == 0:
-                raise RecordError("no records in %r" % (self.files,))
+            while not failed and len(window) < DECODE_AHEAD:
+                try:
+                    rec = next(src)
+                except Exception as e:          # framing error / no records: at its place in the stream
+                    window.append(e)
+                    failed = True
+                    break
+                window.append(pool.submit(decode, rec))
+            item = window.popleft()
+            if isinstance(item, BaseException):
+                raise item
+            yield item.result()
+    finally:
+        if not is_finalizing():     # at interpreter exit concurrent.futures has joined its workers already
+            pool.shutdown(wait=True, cancel_futures=True)
+
+
+def _voc_examples(files, config, rng):
+    for img, gt in _decoded(files, decode_voc_example):
+        yield (img,) + plan_augment(img.shape[0], img.shape[1], gt, config, rng)
+
+
+def _imagenet_examples(files, config, rng):
+    for img, label in _decoded(files, decode_imagenet_example):
+        yield img, plan_augment(img.shape[0], img.shape[1], None, config, rng)[0], label
+
+
+def _shuffled(examples, buffer_size, rng):
+    buf = []
+    for ex in examples:
+        buf.append(ex)
+        if len(buf) >= buffer_size:
+            yield buf.pop(int(rng.integers(len(buf))))
+
+
+def _batches(src, batch_size):
+    while True:
+        yield [next(src) for _ in range(batch_size)]

@@ -558,7 +558,7 @@ class GraphTrainer:
         stats = []
         accuracy = None
         if self.kind == "classify":
-            lab = self.E.check_class_labels(ground_truth, np.asarray(images).shape[0], self.features.C)
+            lab = self.E.check_class_labels(ground_truth, len(images), self.features.C)
             lab = torch.from_numpy(lab).to(self.device)
             loss, _, logits = self.classify_loss(self.forward_features(images, True, stats), lab)
             accuracy = float((torch.argmax(logits, dim=1) == lab).to(torch.float32).mean())
