@@ -3,7 +3,7 @@
  *
  * This is the drop-in boundary underneath the reference's Python surface
  * (SSD300.SSD300 / RetinaNet.RetinaNet / YOLOv3.YOLOv3 / FCOS.FCOS /
- * SSD512.SSD512 .test_one_image()).  The reference has no FFI of its own: all
+ * SSD512.SSD512 / YOLOv2.YOLOv2 .test_one_image()).  The reference has no FFI of its own: all
  * of its arithmetic is executed by TensorFlow 1.13 ops called from Python.
  * Each entry point below replaces one class of TF op *call sites* on the
  * inference path; the call site it stands in for is cited as
@@ -316,6 +316,17 @@ long long odt_yolo_loss_scratch_bytes(const odt_tail_params* p, int B);
 int odt_yolo_loss_fwd(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
                       float coord_scale, float noobj_scale, float obj_scale, float class_scale,
                       void* scratch, float* loss_out, void* stream);
+/* YOLOv2 training-loss forward: the YOLOv3 loss of one level, run by the same kernels (YOLOv2.py:105-173).  The
+ * head is ODT_DECODE_YOLO3 with num_levels == 1 (the 32-pixel grid; the GT is divided by 32), A = 1..ODT_MAX_PRIORS,
+ * num_fg = 1..128, G <= 128; the best prior at the GT's cell by unclamped IoU (first maximum), the no-object term
+ * where the best IoU <= 0.6 (not 0.5) and the cell holds no GT.  loss_out [B] = coord_scale * coord + class_scale *
+ * class + obj_scale * obj + noobj_scale * noobj per image, NOT divided by the GT count (the graph takes the plain
+ * batch mean, no 0.5); an image without boxes gets the no-object term of every row.  Geometry as odt_yolo_loss_fwd,
+ * checked before any launch. */
+long long odt_yolo2_loss_scratch_bytes(const odt_tail_params* p, int B);
+int odt_yolo2_loss_fwd(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
+                       float coord_scale, float noobj_scale, float obj_scale, float class_scale,
+                       void* scratch, float* loss_out, void* stream);
 
 /* Training-loss gradients, one per family: the family's loss forward (same kernels, same arguments, same
  * checks, loss_out / info_out bit-identical to the _fwd call) followed by its gradient kernel.
@@ -326,7 +337,7 @@ int odt_yolo_loss_fwd(const float* head, const odt_tail_params* p, int B, const 
  *   (softmax - one-hot(background)) / #mined on the mined negatives only;
  *   FCOS: per level with GT, IoU loss through exp(), centre-ness BCE, sigmoid focal, / its positive class cells;
  *   YOLOv3: sigmoid-BCE and squared log-size terms of the assigned (cell, prior) rows, the no-object term on
- *   the objectness column under its mask, / #GT.
+ *   the objectness column under its mask, / #GT;  YOLOv2: the same terms on its one level, not divided.
  * GTs sharing a row add up in GT order; no floating-point atomics: the gradient is bit-identical from run to
  * run and an image's gradient does not depend on its batch.  scratch: odt_<family>_loss_scratch_bytes. */
 int odt_retina_loss_grad(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
@@ -338,6 +349,9 @@ int odt_fcos_loss_grad(const float* head, const odt_tail_params* p, int B, const
 int odt_yolo_loss_grad(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
                        float coord_scale, float noobj_scale, float obj_scale, float class_scale,
                        void* scratch, float* loss_out, float* grad_out, void* stream);
+int odt_yolo2_loss_grad(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
+                        float coord_scale, float noobj_scale, float obj_scale, float class_scale,
+                        void* scratch, float* loss_out, float* grad_out, void* stream);
 
 /* ------------------------------------------------ training augmentation --- */
 /* image_augmentor's pixel work (utils/image_augmentor.py:7-264, as odt_b200/tfrecord.py's augment_pixels restates

@@ -1,4 +1,4 @@
-// Training-loss forwards of the four families (RetinaNet, SSD, FCOS, YOLOv3), forward only.
+// Training-loss forwards of the five families (RetinaNet, SSD, FCOS, YOLOv3, YOLOv2), forward only.
 // RetinaNet (BASELINE config 3 "focal-loss + decode + NMS"): anchor/GT matching, softmax focal loss and
 // smooth-L1 box loss.  Restates RetinaNet.py:357-474 (never copied):
 //   * GT rows (y,x,h,w,id) padded with -1; valid count = index of first -1 in col 0
@@ -598,7 +598,7 @@ __global__ void fcos_loss_final_kernel(const float* __restrict__ partial, const 
   out[b] = total;
 }
 
-// ============================ YOLOv3 loss forward ===========================
+// ======================== YOLOv3 / YOLOv2 loss forward ======================
 // Restates YOLOv3.py:115-318 (+ :37-41 priors, :419-433 anchors, :435-442 GT normalisation), never copied.
 // Quirks kept: level k divides the GT by 32 / 16 / 8 while its priors are priors[k] / (8, 16, 32)[k];
 // the GT x anchor intersections are products of UNCLAMPED differences; the no-object anchors are built
@@ -613,7 +613,24 @@ __device__ __forceinline__ float iou_unclamped(float gy1, float gx1, float gy2, 
   const float garea = __fmul_rn(__fsub_rn(gy2, gy1), __fsub_rn(gx2, gx1));
   return __fdiv_rn(inter, __fsub_rn(__fadd_rn(aarea, garea), inter));
 }
-constexpr int kYoloLevels = 3;
+// The two YOLO losses share these kernels; a variant fixes what differs between them at compile time:
+//   YOLOv3 (YOLOv3.py:115-318): three levels, no-object where the best IoU <= 0.5, the image loss divided by its GT
+//     count;
+//   YOLOv2 (YOLOv2.py:105-173): the YOLOv3 loss of level 0 alone (GT divided by 32), no-object where the best
+//     IoU <= 0.6, the image loss NOT divided by its GT count -- an image without boxes is all no-object terms.
+// Every other operation, and its order, is the same in both.
+struct Yolo3Loss {
+  static constexpr int kLevels = 3;
+  static constexpr float kNoobjIou = 0.5f;
+  static constexpr bool kPerGt = true;
+  static constexpr const char* kHead = "YOLOv3 head with 3 levels and 1..128 classes expected";
+};
+struct Yolo2Loss {
+  static constexpr int kLevels = 1;
+  static constexpr float kNoobjIou = 0.6f;
+  static constexpr bool kPerGt = false;
+  static constexpr const char* kHead = "YOLOv2 head with 1 level and 1..128 classes expected";
+};
 
 // GT row g normalised for level k (divided by 32 / 16 / 8): centre, size and corners
 struct YoloGt {
@@ -634,7 +651,7 @@ __device__ __forceinline__ YoloGt yolo_gt(const float* gb, int g, int k) {
 }
 
 // Cells (H * W) of the levels before `lvl`: where that level starts in the per-image occupancy array.  Every level
-// holds the same number of priors A (odt_yolo_loss_fwd checks it), and a cell's A rows are consecutive.
+// holds the same number of priors A (yolo_forward checks it), and a cell's A rows are consecutive.
 __device__ __forceinline__ int yolo_cell_base(const odt_tail_params& p, int lvl) {
   int c = 0;
   for (int i = 0; i < lvl; ++i) c += p.level[i].H * p.level[i].W;
@@ -643,16 +660,18 @@ __device__ __forceinline__ int yolo_cell_base(const odt_tail_params& p, int lvl)
 
 // Level / prior assignment of GT row g (YOLOv3.py:160-200): on every level its cell (clamped to the grid) and the
 // first maximum of its IoU with the level's priors centred there; the level of the largest of the three (ties go to
-// level 2).  occ_img (or nullptr): the image's cell occupancy, where every GT marks its cell on every level.
+// level 2).  YOLOv2 has level 0 only (YOLOv2.py:106-128).  occ_img (or nullptr): the image's cell occupancy, where
+// every GT marks its cell on every level.
 struct YoloAssign {
   int k, row;  // level, row of (cell, prior) in the image
 };
+template <class V>
 __device__ __forceinline__ YoloAssign yolo_assign(const odt_tail_params& p, const float* gb, int g,
                                                   unsigned char* occ_img) {
-  float mx[kYoloLevels];
-  int arg[kYoloLevels], cy[kYoloLevels], cx[kYoloLevels];
+  float mx[V::kLevels];
+  int arg[V::kLevels], cy[V::kLevels], cx[V::kLevels];
 #pragma unroll
-  for (int k = 0; k < kYoloLevels; ++k) {
+  for (int k = 0; k < V::kLevels; ++k) {
     const odt_level& L = p.level[k];
     const YoloGt n = yolo_gt(gb, g, k);
     cy[k] = min(max((int)floorf(n.y), 0), L.H - 1);
@@ -672,6 +691,9 @@ __device__ __forceinline__ YoloAssign yolo_assign(const odt_tail_params& p, cons
     }
     mx[k] = bv;
     arg[k] = bi;
+  }
+  if constexpr (V::kLevels == 1) {
+    return {0, p.level[0].offset + (cy[0] * p.level[0].W + cx[0]) * p.level[0].A + arg[0]};
   }
   int k = 2;
   if (mx[0] > mx[1] && mx[0] > mx[2]) k = 0;
@@ -694,7 +716,7 @@ __device__ __forceinline__ float4 yolo_targets(const odt_tail_params& p, const f
 
 // K1: one block per image, one thread per GT: level / prior assignment, positive terms, cell occupancy.
 // NFG = 20: the 25-float rows, class loop fixed at compile time; NFG = 0: num_fg from the parameters.
-template <int NFG>
+template <class V, int NFG>
 __global__ void __launch_bounds__(kMaxGT)
     yolo_loss_pos_kernel(const float* __restrict__ head, const __grid_constant__ TailP tp,
                          const float* __restrict__ gt, int G, unsigned char* __restrict__ occ,
@@ -706,10 +728,10 @@ __global__ void __launch_bounds__(kMaxGT)
   const float* gb = gt + (long long)b * G * 5;
   __shared__ float s_red[3][kMaxGT];
   const int cnt = block_gt_count(gb, G);
-  const long long cells = yolo_cell_base(p, kYoloLevels);
+  const long long cells = yolo_cell_base(p, V::kLevels);
   float coord = 0.f, cls = 0.f, obj = 0.f;
   if (g < cnt) {
-    const YoloAssign as = yolo_assign(p, gb, g, occ + (long long)b * cells);
+    const YoloAssign as = yolo_assign<V>(p, gb, g, occ + (long long)b * cells);
     const float* r = head + ((long long)b * p.N + as.row) * row;
     const float4 tg = yolo_targets(p, gb, g, as);
     const float ty = tg.x, tx = tg.y, th = tg.z, tw = tg.w;
@@ -728,10 +750,11 @@ __global__ void __launch_bounds__(kMaxGT)
 
 // GT corners of every level for the no-object test, staged in shared memory by the block's threads (the caller
 // synchronises)
-__device__ __forceinline__ void yolo_stage_gt(const float* gb, int cnt, float (*s_g)[kYoloLevels][4]) {
+template <int NL>
+__device__ __forceinline__ void yolo_stage_gt(const float* gb, int cnt, float (*s_g)[NL][4]) {
   for (int g = threadIdx.x; g < cnt; g += blockDim.x) {
 #pragma unroll
-    for (int k = 0; k < kYoloLevels; ++k) {
+    for (int k = 0; k < NL; ++k) {
       const YoloGt n = yolo_gt(gb, g, k);
       s_g[g][k][0] = n.y1;
       s_g[g][k][1] = n.x1;
@@ -760,12 +783,14 @@ __device__ __forceinline__ YoloNoobjBox yolo_noobj_box(const odt_tail_params& p,
   o.area = __fmul_rn(__fsub_rn(o.y2, o.y1), __fsub_rn(o.x2, o.x1));
   return o;
 }
-__device__ __forceinline__ float yolo_noobj_iou(const float (*s_g)[kYoloLevels][4], int g, int lvl,
+template <int NL>
+__device__ __forceinline__ float yolo_noobj_iou(const float (*s_g)[NL][4], int g, int lvl,
                                                 const YoloNoobjBox& o) {
   return iou_unclamped(s_g[g][lvl][0], s_g[g][lvl][1], s_g[g][lvl][2], s_g[g][lvl][3], o.y1, o.x1, o.y2, o.x2, o.area);
 }
 
 // K2: no-object term over every (cell, prior) whose cell holds no GT centre
+template <class V>
 __global__ void __launch_bounds__(kLossThreads)
     yolo_loss_noobj_kernel(const float* __restrict__ head, const __grid_constant__ TailP tp,
                            const float* __restrict__ gt, int G, const unsigned char* __restrict__ occ,
@@ -774,12 +799,12 @@ __global__ void __launch_bounds__(kLossThreads)
   const odt_tail_params& p = tp.p;
   const int b = blockIdx.y, blk = blockIdx.x;
   const float* gb = gt + (long long)b * G * 5;
-  __shared__ float s_g[kMaxGT][kYoloLevels][4];
+  __shared__ float s_g[kMaxGT][V::kLevels][4];
   __shared__ float s_red[1][kLossThreads];
   const int cnt = block_gt_count(gb, G);
   yolo_stage_gt(gb, cnt, s_g);
   __syncthreads();
-  const long long cells = yolo_cell_base(p, kYoloLevels);
+  const long long cells = yolo_cell_base(p, V::kLevels);
   const int row = row_floats(p.num_fg);
   const float* hb = head + (long long)b * p.N * row;
   float acc = 0.f;
@@ -792,12 +817,13 @@ __global__ void __launch_bounds__(kLossThreads)
     const YoloNoobjBox o = yolo_noobj_box(p, c);
     float best = -3.0e38f;
     for (int g = 0; g < cnt; ++g) best = fmaxf(best, yolo_noobj_iou(s_g, g, c.lvl, o));
-    if (best <= 0.5f) acc += sig_xent(0.f, hb[(long long)n * row + p.num_fg + 4]);  // objectness
+    if (best <= V::kNoobjIou) acc += sig_xent(0.f, hb[(long long)n * row + p.num_fg + 4]);  // objectness
   }
   block_sum(s_red, {acc});
   if (threadIdx.x == 0) partial[(long long)b * kLossBlocks + blk] = s_red[0][0];
 }
 
+template <class V>
 __global__ void yolo_loss_final_kernel(const float* __restrict__ pos, const float* __restrict__ partial, int B,
                                        float cs, float ns, float os, float ks, float* __restrict__ out) {
   pdl_launch_dependents();
@@ -805,8 +831,12 @@ __global__ void yolo_loss_final_kernel(const float* __restrict__ pos, const floa
   if (b >= B) return;
   double noobj = 0.0;
   for (int i = 0; i < kLossBlocks; ++i) noobj += (double)partial[(long long)b * kLossBlocks + i];
-  const float ng = pos[b * 4 + 3];
-  out[b] = (cs * pos[b * 4 + 0] + ks * pos[b * 4 + 1] + os * pos[b * 4 + 2]) / ng + ns * (float)noobj / ng;
+  if constexpr (V::kPerGt) {
+    const float ng = pos[b * 4 + 3];
+    out[b] = (cs * pos[b * 4 + 0] + ks * pos[b * 4 + 1] + os * pos[b * 4 + 2]) / ng + ns * (float)noobj / ng;
+  } else {
+    out[b] = cs * pos[b * 4 + 0] + ks * pos[b * 4 + 1] + os * pos[b * 4 + 2] + ns * (float)noobj;
+  }
 }
 
 // ============================ loss gradients ================================
@@ -995,12 +1025,13 @@ __global__ void __launch_bounds__(kLossThreads)
   }
 }
 
-// YOLOv3, all / #GT: the objectness column of a no-object row (a cell without GT, best IoU <= 0.5, as the forward
-// decides it) gets noobj_scale * sigmoid(x); an assigned row gets, once per GT assigned to it, class_scale *
-// (sigmoid - one-hot) on the classes, coord_scale * (sigmoid - target) on y, x, coord_scale * (x - target) on h, w
-// (the 0.5 of the squared term cancels), obj_scale * (sigmoid - 1) on the objectness; every other element is zero.
-// The block re-derives its image's assignments with the forward's yolo_assign and reads the forward's occupancy.
-template <int NFG>
+// YOLOv3, all / #GT (YOLOv2: not divided): the objectness column of a no-object row (a cell without GT, best IoU
+// <= the variant's threshold, as the forward decides it) gets noobj_scale * sigmoid(x); an assigned row gets, once
+// per GT assigned to it, class_scale * (sigmoid - one-hot) on the classes, coord_scale * (sigmoid - target) on y, x,
+// coord_scale * (x - target) on h, w (the 0.5 of the squared term cancels), obj_scale * (sigmoid - 1) on the
+// objectness; every other element is zero.  The block re-derives its image's assignments with the forward's
+// yolo_assign and reads the forward's occupancy.
+template <class V, int NFG>
 __global__ void __launch_bounds__(kLossThreads, 4)
     yolo_loss_grad_kernel(const float* __restrict__ head, const __grid_constant__ TailP tp,
                           const float* __restrict__ gt, int G, const unsigned char* __restrict__ occ, float cs,
@@ -1010,20 +1041,20 @@ __global__ void __launch_bounds__(kLossThreads, 4)
   const int nfg = NFG ? NFG : p.num_fg, row = row_floats(nfg);
   const int b = blockIdx.y, lane = threadIdx.x & 31;
   const float* gb = gt + (long long)b * G * 5;
-  __shared__ float s_g[kMaxGT][kYoloLevels][4];
+  __shared__ float s_g[kMaxGT][V::kLevels][4];
   __shared__ int s_row[kMaxGT], s_lab[kMaxGT];
   __shared__ float4 s_t[kMaxGT];
   const int cnt = block_gt_count(gb, G);
   yolo_stage_gt(gb, cnt, s_g);
   for (int g = threadIdx.x; g < cnt; g += blockDim.x) {
-    const YoloAssign as = yolo_assign(p, gb, g, nullptr);
+    const YoloAssign as = yolo_assign<V>(p, gb, g, nullptr);
     s_row[g] = as.row;
     s_t[g] = yolo_targets(p, gb, g, as);
     s_lab[g] = (int)gb[g * 5 + 4];
   }
   __syncthreads();
-  const long long cells = yolo_cell_base(p, kYoloLevels);
-  const float inv = __fdiv_rn(1.f, (float)cnt);
+  const long long cells = yolo_cell_base(p, V::kLevels);
+  const float inv = V::kPerGt ? __fdiv_rn(1.f, (float)cnt) : 1.f;
   for (int n = blockIdx.x * kGradWarps + (threadIdx.x >> 5); n < p.N; n += gridDim.x * kGradWarps) {
     const Cell c = locate(p, n);
     const odt_level& L = p.level[c.lvl];
@@ -1033,7 +1064,7 @@ __global__ void __launch_bounds__(kLossThreads, 4)
       const YoloNoobjBox o = yolo_noobj_box(p, c);
       float best = -3.0e38f;
       for (int g = lane; g < cnt; g += 32) best = fmaxf(best, yolo_noobj_iou(s_g, g, c.lvl, o));
-      noobj = warp_max(best) <= 0.5f;
+      noobj = warp_max(best) <= V::kNoobjIou;
     }
     float* go = grad + ((long long)b * p.N + n) * row;
     const float* r = head + ((long long)b * p.N + n) * row;
@@ -1119,15 +1150,17 @@ struct YoloScratch {
   unsigned char* occ;  // 1 for a cell that holds a GT, [B][sum of H * W over the levels]
   long long bytes;
 };
+template <class V>
 static long long yolo_cells(const odt_tail_params& p) {
   long long c = 0;
-  for (int i = 0; i < kYoloLevels; ++i) c += (long long)p.level[i].H * p.level[i].W;
+  for (int i = 0; i < V::kLevels; ++i) c += (long long)p.level[i].H * p.level[i].W;
   return c;
 }
+template <class V>
 static YoloScratch yolo_scratch(const odt_tail_params& p, int B, void* base) {
   Carve c{(uintptr_t)base, 0};
   return {c.take<float>((long long)B * 4), c.take<float>((long long)B * kLossBlocks),
-          c.take<unsigned char>((long long)B * yolo_cells(p)), c.bytes};
+          c.take<unsigned char>((long long)B * yolo_cells<V>(p)), c.bytes};
 }
 
 template <class Layout>
@@ -1201,18 +1234,19 @@ static int fcos_forward(const float* head, const odt_tail_params* p, int B, cons
   return ODT_OK;
 }
 
+template <class V>
 static int yolo_forward(const float* head, const odt_tail_params* p, int B, const float* gt, int G, float coord_scale,
                         float noobj_scale, float obj_scale, float class_scale, void* scratch, float* loss_out,
                         cudaStream_t st, YoloScratch& s) {
   ODT_CHECK_ARG(head && p && gt && scratch && loss_out, "null pointer");
-  ODT_CHECK_ARG(p->kind == ODT_DECODE_YOLO3 && p->num_levels == kYoloLevels && p->num_fg >= 1 && p->num_fg <= kMaxFg,
-                "YOLOv3 head with 3 levels and 1..128 classes expected");
+  ODT_CHECK_ARG(p->kind == ODT_DECODE_YOLO3 && p->num_levels == V::kLevels && p->num_fg >= 1 && p->num_fg <= kMaxFg,
+                V::kHead);
   // One prior count on every level (the config's num_priors), and rows laid out level after level, cell after cell:
   // the kernels find a level's rows at its offset and its cells in the occupancy array by these sums.
   const int A = p->level[0].A;
   ODT_CHECK_ARG(A >= 1 && A <= ODT_MAX_PRIORS, "1..9 priors per level expected");
   long long rows = 0;
-  for (int i = 0; i < kYoloLevels; ++i) {
+  for (int i = 0; i < V::kLevels; ++i) {
     const odt_level& L = p->level[i];
     ODT_CHECK_ARG(L.A == A, "the same number of priors on every level expected");
     ODT_CHECK_ARG(L.H >= 1 && L.W >= 1 && L.offset == rows, "level geometry: H, W >= 1, offset = rows before it");
@@ -1221,19 +1255,40 @@ static int yolo_forward(const float* head, const odt_tail_params* p, int B, cons
   ODT_CHECK_ARG(rows == p->N, "N must be the sum of H * W * A over the levels");
   ODT_CHECK_ARG(B > 0 && G > 0 && G <= kMaxGT, "B/G (G <= 128)");
   ODT_CHECK_ARG(((uintptr_t)scratch & 7) == 0, "scratch must be 8-byte aligned");
-  s = yolo_scratch(*p, B, scratch);
-  ODT_CUDA_OK(cudaMemsetAsync(s.occ, 0, (size_t)B * yolo_cells(*p), st));
+  s = yolo_scratch<V>(*p, B, scratch);
+  ODT_CUDA_OK(cudaMemsetAsync(s.occ, 0, (size_t)B * yolo_cells<V>(*p), st));
   TailP tp;
   tp.p = *p;
   if (p->num_fg == 20)
-    yolo_loss_pos_kernel<20><<<B, kMaxGT, 0, st>>>(head, tp, gt, G, s.occ, s.pos);
+    yolo_loss_pos_kernel<V, 20><<<B, kMaxGT, 0, st>>>(head, tp, gt, G, s.occ, s.pos);
   else
-    yolo_loss_pos_kernel<0><<<B, kMaxGT, 0, st>>>(head, tp, gt, G, s.occ, s.pos);
+    yolo_loss_pos_kernel<V, 0><<<B, kMaxGT, 0, st>>>(head, tp, gt, G, s.occ, s.pos);
   ODT_LAUNCH_OK();
-  yolo_loss_noobj_kernel<<<dim3(kLossBlocks, B), kLossThreads, 0, st>>>(head, tp, gt, G, s.occ, s.partial);
+  yolo_loss_noobj_kernel<V><<<dim3(kLossBlocks, B), kLossThreads, 0, st>>>(head, tp, gt, G, s.occ, s.partial);
   ODT_LAUNCH_OK();
-  yolo_loss_final_kernel<<<(B + 63) / 64, 64, 0, st>>>(s.pos, s.partial, B, coord_scale, noobj_scale, obj_scale,
-                                                       class_scale, loss_out);
+  yolo_loss_final_kernel<V><<<(B + 63) / 64, 64, 0, st>>>(s.pos, s.partial, B, coord_scale, noobj_scale, obj_scale,
+                                                          class_scale, loss_out);
+  ODT_LAUNCH_OK();
+  return ODT_OK;
+}
+
+// forward, then the gradient kernel on the matching the forward left in scratch
+template <class V>
+static int yolo_forward_grad(const float* head, const odt_tail_params* p, int B, const float* gt, int G, float cs,
+                             float ns, float os, float ks, void* scratch, float* loss_out, float* grad_out,
+                             cudaStream_t st) {
+  ODT_CHECK_ARG(grad_out, "null pointer");
+  YoloScratch s;
+  const int rc = yolo_forward<V>(head, p, B, gt, G, cs, ns, os, ks, scratch, loss_out, st, s);
+  if (rc != ODT_OK) return rc;
+  TailP tp;
+  tp.p = *p;
+  if (p->num_fg == 20)
+    yolo_loss_grad_kernel<V, 20><<<grad_grid(B), kLossThreads, 0, st>>>(head, tp, gt, G, s.occ, cs, ns, os, ks,
+                                                                        grad_out);
+  else
+    yolo_loss_grad_kernel<V, 0><<<grad_grid(B), kLossThreads, 0, st>>>(head, tp, gt, G, s.occ, cs, ns, os, ks,
+                                                                       grad_out);
   ODT_LAUNCH_OK();
   return ODT_OK;
 }
@@ -1252,7 +1307,10 @@ extern "C" long long odt_fcos_loss_scratch_bytes(const odt_tail_params* p, int B
   return scratch_bytes(p, B, fcos_scratch);
 }
 extern "C" long long odt_yolo_loss_scratch_bytes(const odt_tail_params* p, int B) {
-  return scratch_bytes(p, B, yolo_scratch);
+  return scratch_bytes(p, B, yolo_scratch<Yolo3Loss>);
+}
+extern "C" long long odt_yolo2_loss_scratch_bytes(const odt_tail_params* p, int B) {
+  return scratch_bytes(p, B, yolo_scratch<Yolo2Loss>);
 }
 
 extern "C" int odt_retina_loss_fwd(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
@@ -1277,8 +1335,16 @@ extern "C" int odt_yolo_loss_fwd(const float* head, const odt_tail_params* p, in
                                  float coord_scale, float noobj_scale, float obj_scale, float class_scale,
                                  void* scratch, float* loss_out, void* stream) {
   YoloScratch s;
-  return yolo_forward(head, p, B, gt, G, coord_scale, noobj_scale, obj_scale, class_scale, scratch, loss_out,
-                      (cudaStream_t)stream, s);
+  return yolo_forward<Yolo3Loss>(head, p, B, gt, G, coord_scale, noobj_scale, obj_scale, class_scale, scratch,
+                                 loss_out, (cudaStream_t)stream, s);
+}
+
+extern "C" int odt_yolo2_loss_fwd(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
+                                  float coord_scale, float noobj_scale, float obj_scale, float class_scale,
+                                  void* scratch, float* loss_out, void* stream) {
+  YoloScratch s;
+  return yolo_forward<Yolo2Loss>(head, p, B, gt, G, coord_scale, noobj_scale, obj_scale, class_scale, scratch,
+                                 loss_out, (cudaStream_t)stream, s);
 }
 
 extern "C" int odt_retina_loss_grad(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
@@ -1334,22 +1400,13 @@ extern "C" int odt_fcos_loss_grad(const float* head, const odt_tail_params* p, i
 extern "C" int odt_yolo_loss_grad(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
                                   float coord_scale, float noobj_scale, float obj_scale, float class_scale,
                                   void* scratch, float* loss_out, float* grad_out, void* stream) {
-  ODT_CHECK_ARG(grad_out, "null pointer");
-  cudaStream_t st = (cudaStream_t)stream;
-  YoloScratch s;
-  const int rc = yolo_forward(head, p, B, gt, G, coord_scale, noobj_scale, obj_scale, class_scale, scratch, loss_out,
-                              st, s);
-  if (rc != ODT_OK) return rc;
-  TailP tp;
-  tp.p = *p;
-  if (p->num_fg == 20)
-    yolo_loss_grad_kernel<20><<<grad_grid(B), kLossThreads, 0, st>>>(head, tp, gt, G, s.occ,
-                                                                     coord_scale, noobj_scale, obj_scale, class_scale,
-                                                                     grad_out);
-  else
-    yolo_loss_grad_kernel<0><<<grad_grid(B), kLossThreads, 0, st>>>(head, tp, gt, G, s.occ,
-                                                                    coord_scale, noobj_scale, obj_scale, class_scale,
-                                                                    grad_out);
-  ODT_LAUNCH_OK();
-  return ODT_OK;
+  return yolo_forward_grad<Yolo3Loss>(head, p, B, gt, G, coord_scale, noobj_scale, obj_scale, class_scale, scratch,
+                                      loss_out, grad_out, (cudaStream_t)stream);
+}
+
+extern "C" int odt_yolo2_loss_grad(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
+                                   float coord_scale, float noobj_scale, float obj_scale, float class_scale,
+                                   void* scratch, float* loss_out, float* grad_out, void* stream) {
+  return yolo_forward_grad<Yolo2Loss>(head, p, B, gt, G, coord_scale, noobj_scale, obj_scale, class_scale, scratch,
+                                      loss_out, grad_out, (cudaStream_t)stream);
 }

@@ -1,4 +1,4 @@
-// Inference tail of the five detectors on sm_90a: score activation, analytic
+// Inference tail of the six detectors on sm_90a: score activation, analytic
 // anchor/prior generation, box decode, thresholding, candidate compaction and
 // exact per-class TF NonMaxSuppressionV3 (iterative arg-max + IoU suppress).
 //

@@ -4,7 +4,7 @@ Same class names, constructor signature `(config, data_provider)`, config keys,
 asserts and method names as the reference model scripts, so its test*.py
 drivers run unchanged (SURVEY.md section 8b):
     SSD300.py:11-50,473-504   SSD512.py   RetinaNet.py:11-79,505-539
-    YOLOv3.py:11-60,444-483   FCOS.py:11-49,401-436
+    YOLOv3.py:11-60,444-483   YOLOv2.py:11-54,305-343   FCOS.py:11-49,401-436
 Inference (`test_one_image`) runs entirely on the hand-written GPU kernels; there is no CPU
 fallback.  `train_one_epoch` runs the training step of odt_b200/train.py (PyTorch autograd over the
 engine's layer list + the reference's losses + Momentum: the first stage of SURVEY 8f row 2; RetinaNet's
@@ -367,7 +367,7 @@ class _Detector:
         return self.detect_stream(batches_local, precision, sharded=True, consumer=consumer)
 
     # ---- training / checkpoints (API surface; SURVEY 8f) --------------------
-    loss_kind = None  # the family's training loss: 'ssd' | 'retina' | 'yolo' | 'fcos' (engine.Tail.loss)
+    loss_kind = None  # the family's training loss: 'ssd' | 'retina' | 'yolo' | 'yolo2' | 'fcos' (engine.Tail.loss)
 
     def _loss_scalars(self):
         """The family's loss scalars from config, as keywords of engine.Tail.loss."""
@@ -657,6 +657,33 @@ class YOLOv3(_Detector):
 
     def _build(self, batch, precision, allow_tc=True):
         return nets.build_yolov3(batch, self.config, precision, self.device, allow_tc)
+
+    def _loss_scalars(self):
+        return {"coord_scale": self.coord_sacle, "noobj_scale": self.noobj_scale, "obj_scale": self.obj_scale,
+                "class_scale": self.class_scale}
+
+
+class YOLOv2(_Detector):
+    name = "YOLOv2"
+    backbone_scope = "backone"  # sic: the reference's scope name (YOLOv2.py:76,220)
+    # YOLOv3's loss on one level, no-object IoU <= 0.6, not divided by the GT count: ref YOLOv2.py:103-181
+    loss_kind = "yolo2"
+
+    def __init__(self, config, data_provider):
+        assert len(config["data_shape"]) == 3
+        nets.check_yolo2_config(config)
+        self._common_init(config, data_provider)
+        self.data_shape = config["data_shape"]
+        self.num_classes = config["num_classes"]
+        self.coord_sacle = config["coord_scale"]
+        self.noobj_scale = config["noobj_scale"]
+        self.obj_scale = config["obj_scale"]
+        self.class_scale = config["class_scale"]
+        self.rescore_confidence = config["rescore_confidence"]  # read and unused, as in the reference
+        self.num_priors = len(config["priors"])
+
+    def _build(self, batch, precision, allow_tc=True):
+        return nets.build_yolov2(batch, self.config, precision, self.device, allow_tc)
 
     def _loss_scalars(self):
         return {"coord_scale": self.coord_sacle, "noobj_scale": self.noobj_scale, "obj_scale": self.obj_scale,

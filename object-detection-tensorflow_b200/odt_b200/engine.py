@@ -74,6 +74,8 @@ class Act:
         self.buf = None
         self.needed = True  # False when only a fused second output is consumed
         self.halo = 0       # 1: stored as [B, H+2, W+2, ld] with a zero border (halo-flat 3x3 convs)
+        self.base, self.c0 = None, 0  # a channel slice [c0, c0 + C) of the tensor `base` (Net.concat)
+        self.parts = ()               # Net.concat: the slices that make up this tensor
 
     @property
     def img_stride(self):
@@ -107,7 +109,8 @@ class ConvOp(Op):
         self.pre = None     # fused consumer pre-activation: (bn_scope, act, Act)
         self.pre2 = None    # a second one (tensor-core path): RetinaNet block inputs feed two BNs
         self.pool = 0       # 2: the 2x2/2 max-pool that follows is done in the epilogue (y is the pooled tensor)
-        self.reads = tuple(t for t in (x, residual) if t is not None)
+        # a concatenated input is read through its slices: their producers are what the op waits for
+        self.reads = tuple(t for t in (x, residual) if t is not None) + (x.parts if x is not None else ())
         self.writes = (y,) if y is not None else ()
         self.flops = 0
 
@@ -543,6 +546,23 @@ class Net:
         self.ops.append(NearestConcatOp(a, b, y))
         return y
 
+    def concat(self, parts):
+        """tf.concat(parts, axis=channels) with no copy (YOLOv2.py:90): one tensor whose channel slices are stored by the
+        producers of the parts, each as an extra epilogue output of its convolution (an identity pre-activation that
+        fuse() folds in).  A part whose producer cannot take it is an error at finalize, not a copy."""
+        y = self.new_act(parts[0].name + "/concat", parts[0].H, parts[0].W, sum(t.C for t in parts))
+        c0, views = 0, []
+        for t in parts:
+            assert (t.B, t.H, t.W) == (y.B, y.H, y.W), (t.name, y.name)
+            v = Act(t.name + "/slice", t.B, t.H, t.W, t.C, y.ld, t.dtype)
+            v.base, v.c0 = y, c0
+            self.acts.append(v)
+            self.ops.append(AffineActOp(t, v, None, None))
+            views.append(v)
+            c0 += t.C
+        y.parts = tuple(views)
+        return y
+
     def add_level(self, H, W, A):
         off = sum(h * w * a for h, w, a in self.levels)
         self.levels.append((H, W, A))
@@ -582,6 +602,8 @@ class Net:
                     if not consumers[id(op.x)] and isinstance(q, (ConvOp, PoolOp)):
                         op.x.needed = False
                     continue
+            if isinstance(op, AffineActOp) and op.y.base is not None:
+                raise ValueError("concat: the producer of %s cannot store its channel slice" % op.x.name)
             kept.append(op)
         self.ops = kept
 
@@ -683,9 +705,13 @@ class Net:
         for t in self.acts:
             if getattr(t, "fused_away", False):
                 continue  # the pre-pool tensor of a conv with a fused max-pool is never materialised
-            if not t.needed:
-                continue  # raw output nobody reads (only its fused pre-activations are consumed)
+            if not t.needed or t.base is not None:
+                continue  # raw output nobody reads (only its fused pre-activations are consumed); slices below
             t.buf = torch.zeros((t.B, t.H + 2 * t.halo, t.W + 2 * t.halo, t.ld), dtype=self.tdtype, device=dev)
+        for t in self.acts:
+            if t.base is not None:
+                assert t.halo == 0 and t.base.halo == 0
+                t.buf = t.base.buf[..., t.c0:t.c0 + t.C]
         self.N = sum(h * w * a for h, w, a in self.levels)
         # candidate rows of a detection tail (a classification tail has no head levels and no rows)
         self.head_buf = torch.zeros((self.batch, self.N, getattr(tail, "row", 0)), dtype=torch.float32, device=dev)
@@ -974,10 +1000,11 @@ class Tail:
 
     # training-loss kind -> the family's scalars of odt_<kind>_loss_fwd, in argument order, with their defaults
     LOSS_SCALARS = {"retina": (("alpha", 0.25), ("gamma", 2.0)), "ssd": (), "fcos": (),
-                    "yolo": (("coord_scale", 1.0), ("noobj_scale", 1.0), ("obj_scale", 5.0), ("class_scale", 1.0))}
+                    "yolo": (("coord_scale", 1.0), ("noobj_scale", 1.0), ("obj_scale", 5.0), ("class_scale", 1.0)),
+                    "yolo2": (("coord_scale", 1.0), ("noobj_scale", 1.0), ("obj_scale", 5.0), ("class_scale", 1.0))}
 
     def loss(self, net, kind, ground_truth, return_info=False, **kw):
-        """Training-loss forward kernels on the rows this tail reads: kind in 'retina' | 'ssd' | 'fcos' | 'yolo',
+        """Training-loss forward kernels on the rows this tail reads: kind in 'retina' | 'ssd' | 'fcos' | 'yolo' | 'yolo2',
         the family's scalars (LOSS_SCALARS) as keywords.  ground_truth [B,G,5] (y,x,h,w,id) padded with -1.
         Returns float32 [B]; for 'ssd' with return_info=True also int32 [B,3] = (#positives, #negatives,
         #mined negatives) per image."""

@@ -116,6 +116,9 @@ SYMBOLS = {
     "odt_ssd_loss_grad": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _P, _P, _P, _P, _P]),
     "odt_yolo_loss_grad": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _F, _F, _F, _F, _P, _P, _P, _P]),
     "odt_fcos_loss_grad": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _P, _P, _P, _P]),
+    "odt_yolo2_loss_scratch_bytes": (_L, [C.POINTER(TailParams), _I]),
+    "odt_yolo2_loss_fwd": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _F, _F, _F, _F, _P, _P, _P]),
+    "odt_yolo2_loss_grad": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _F, _F, _F, _F, _P, _P, _P, _P]),
     "odt_augment_scratch_bytes": (_L, [C.POINTER(AugmentParams), _I]),
     "odt_augment_batch": (_I, [_P, C.POINTER(AugmentParams), _I, _P, _P, _P, _P]),
     "odt_pool_classify": (_I, [_P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P]),

@@ -1,4 +1,4 @@
-"""Layer graphs of SSD300 / SSD512 / RetinaNet / YOLOv3 / FCOS expressed on the
+"""Layer graphs of SSD300 / SSD512 / RetinaNet / YOLOv3 / YOLOv2 / FCOS expressed on the
 H100 engine (engine.Net).  Each builder mirrors the reference's layer creation
 order so variables get the same TF1 names as in the reference checkpoints
 (SURVEY.md App. D); citations give the reference lines each block stands for.
@@ -340,6 +340,80 @@ def yolo_tail(cfg):
         pr = (np.array(priors[i], dtype=F32) / F32(stride[i])).astype(F32)
         for a in range(cfg["num_priors"]):
             lv.prior_h[a], lv.prior_w[a] = float(pr[a][0]), float(pr[a][1])
+
+    return Tail(L.DECODE_YOLO3, nc, nc, cfg["nms_score_threshold"], cfg["nms_iou_threshold"],
+                cfg["nms_max_boxes"], level_fn)
+
+
+# ---------------------------------------------------------------- YOLOv2 ----
+def check_yolo2_config(cfg):
+    """YOLOv2's classes and anchors: num_classes from 1 to 128 (the sigmoid rows of YOLOv3, see
+    check_sigmoid_num_classes) and `priors` as 1 to 9 (h, w) pairs of positive finite numbers in grid cells; the prior
+    count is len(priors) (YOLOv2.py:33), there is no num_priors key."""
+    nc = cfg["num_classes"]
+    if isinstance(nc, bool) or not isinstance(nc, (int, np.integer)) or not 1 <= nc <= MAX_SIGMOID_CLASSES:
+        raise ValueError("num_classes = %r: YOLOv2 supports 1 to %d classes" % (nc, MAX_SIGMOID_CLASSES))
+    priors = cfg["priors"]
+    try:
+        arr = np.asarray(priors, dtype=np.float64)
+    except (TypeError, ValueError):
+        arr = None
+    if arr is None or arr.ndim != 2 or arr.shape[1] != 2 or not 1 <= arr.shape[0] <= MAX_PRIORS:
+        raise ValueError("priors = %r: YOLOv2 takes 1 to %d (h, w) pairs" % (priors, MAX_PRIORS))
+    if not (np.isfinite(arr).all() and (arr > 0).all()):
+        raise ValueError("priors = %r: YOLOv2 takes positive finite (h, w) pairs" % (priors,))
+
+
+# Darknet-19 of YOLOv2.py:255-303: (name, filters, kernel) of conv1 .. conv18, "pool" for a 2x2/2 SAME max-pool
+_DARKNET19 = [("conv1", 32, 3), "pool", ("conv2", 64, 3), "pool",
+              ("conv3", 128, 3), ("conv4", 64, 1), ("conv5", 128, 3), "pool",
+              ("conv6", 256, 3), ("conv7", 128, 1), ("conv8", 256, 3), "pool",
+              ("conv9", 512, 3), ("conv10", 256, 1), ("conv11", 512, 3), ("conv12", 256, 1), ("conv13", 512, 3), "pool",
+              ("conv14", 1024, 3), ("conv15", 512, 1), ("conv16", 1024, 3), ("conv17", 512, 1), ("conv18", 1024, 3)]
+
+
+def build_yolov2(batch, cfg, precision="fp16", device="cuda", allow_tc=True):
+    """ref YOLOv2.py:75-100,255-303.  Every `_conv_layer` is conv + bias -> BN; the caller's leaky_relu(0.1) follows
+    all of them but `predictions`.  The passthrough is conv17's output on the same 32-pixel grid, concatenated
+    before the head's conv5 output (no space-to-depth reorg: the reference has none)."""
+    check_yolo2_config(cfg)
+    H, W, _ = cfg["data_shape"]
+    nc, npri = cfg["num_classes"], len(cfg["priors"])
+    net = Net(batch, H, W, precision, device, allow_tc)
+
+    def cl(x, f, k, name, act=True, head=None):
+        return net.conv(x, f, k, 1, name=name, bn=True, act="leaky" if act else None, head=head)
+
+    with net.scope("backone"):
+        y = None
+        for item in _DARKNET19:
+            if item == "pool":
+                y = net.maxpool(y, 2, 2)
+                continue
+            y = cl(y, item[1], item[2], item[0])
+            if item[0] == "conv17":
+                passthrough = y
+    with net.scope("head"):
+        for i, (f, k) in enumerate([(1024, 3), (512, 1), (1024, 3), (512, 1), (1024, 3)]):
+            y = cl(y, f, k, "conv%d" % (i + 1))
+        y = net.concat([passthrough, y])
+        off = net.add_level(y.H, y.W, npri)
+        cl(y, (nc + 5) * npri, 1, "predictions", act=False, head=(off, 0, 0, 0, npri))
+    return net, yolo2_tail(cfg)
+
+
+def yolo2_tail(cfg):
+    """decode/NMS tail of YOLOv2 (ref YOLOv2.py:183-210,230-244): YOLOv3's decode on one level -- centre = cell + 0.5 +
+    sigmoid, size = prior + exp (additive), corners x 32 -- with the priors as given, in grid cells; per-class NMS over
+    every class."""
+    nc = cfg["num_classes"]
+    priors = np.asarray(cfg["priors"], dtype=F32)
+
+    def level_fn(i, h, w, lv):
+        lv.cmul_y = lv.cmul_x = lv.cdiv_y = lv.cdiv_x = 1.0
+        lv.out_mul = 32.0
+        for a in range(len(priors)):
+            lv.prior_h[a], lv.prior_w[a] = float(priors[a][0]), float(priors[a][1])
 
     return Tail(L.DECODE_YOLO3, nc, nc, cfg["nms_score_threshold"], cfg["nms_iou_threshold"],
                 cfg["nms_max_boxes"], level_fn)

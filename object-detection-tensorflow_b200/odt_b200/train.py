@@ -245,13 +245,14 @@ def _act(x, act):
 
 
 class GraphTrainer:
-    """Training state + step of SSD300 / SSD512 / RetinaNet / YOLOv3 / FCOS (reference: SSD300.py:129-155,
-    RetinaNet.py:193-222, YOLOv3.py:115-318, FCOS.py:153-195).  Same interface as SSDTrainer."""
+    """Training state + step of SSD300 / SSD512 / RetinaNet / YOLOv3 / YOLOv2 / FCOS (reference: SSD300.py:129-155,
+    RetinaNet.py:193-222, YOLOv3.py:115-318, YOLOv2.py:103-181, FCOS.py:153-195).  Same interface as SSDTrainer."""
 
     def __init__(self, model, device=None, dtype=torch.float32):
         from . import engine as E
         self.model, self.cfg, self.E = model, model.config, E
-        self.kind = {"SSD300": "ssd", "SSD512": "ssd", "RetinaNet": "retina", "YOLOv3": "yolo", "FCOS": "fcos"}[model.name]
+        self.kind = {"SSD300": "ssd", "SSD512": "ssd", "RetinaNet": "retina", "YOLOv3": "yolo", "YOLOv2": "yolo2",
+                     "FCOS": "fcos"}[model.name]
         if getattr(model, "is_pretraining", False):
             self.kind = "classify"                # RetinaNet's ImageNet-pretraining mode
         self.weight_decay = float(model.weight_decay)
@@ -274,7 +275,7 @@ class GraphTrainer:
         # CUDA, fp32 rows: the data term is the family's loss-gradient kernel (csrc/loss.cu) behind one autograd
         # Function; the CPU (and float64) keep the restatement below, which the kernels are tested against
         self._loss_kernels = None
-        if self.kind in ("ssd", "retina", "yolo", "fcos") and self.device.type == "cuda" and dtype == torch.float32:
+        if self.kind in ("ssd", "retina", "yolo", "yolo2", "fcos") and self.device.type == "cuda" and dtype == torch.float32:
             self._loss_kernels = LossKernels(self)
         if self.kind == "ssd":
             self._ssd = SSDTrainer.__new__(SSDTrainer)   # borrows the SSD loss / anchors
@@ -318,7 +319,12 @@ class GraphTrainer:
         val = {}
         for op in self.net.ops:
             if isinstance(op, E.ConvOp):
-                x = x0 if op.is_image else val[id(op.x)]
+                if op.is_image:
+                    x = x0
+                elif op.x.parts:                    # engine.Net.concat: the slices in channel order
+                    x = torch.cat([val[id(v)] for v in op.x.parts], dim=1)
+                else:
+                    x = val[id(op.x)]
                 y = conv_same(x, P[op.kernel], P[op.bias] if op.bias else None, op.stride, op.dil)
                 if op.bn:
                     y = self._bn(y, op.bn, training, stats)
@@ -338,7 +344,8 @@ class GraphTrainer:
             elif isinstance(op, E.PoolOp):
                 val[id(op.y)] = max_pool_same(val[id(op.x)], op.k, op.stride)
             elif isinstance(op, E.AffineActOp):
-                val[id(op.y)] = _act(self._bn(val[id(op.x)], op.bn, training, stats), op.act)
+                x = val[id(op.x)]
+                val[id(op.y)] = _act(x if op.bn is None else self._bn(x, op.bn, training, stats), op.act)
             elif isinstance(op, E.GroupNormActOp):
                 x = val[id(op.x)]
                 y = F.group_norm(x, op.groups, P[op.gn + "/gamma"], P[op.gn + "/beta"], eps=E.GN_EPS)
@@ -467,11 +474,66 @@ class GraphTrainer:
             total = total + (iou_loss + pos + neg + center) / hgt.sum()
         return total
 
+    def _yolo_level(self, r, pri, g, norm, clamp=False):
+        """One YOLO level's matching of the image's GT g: the GT divided by `norm`, its cell (clamped to the grid for
+        YOLOv2, as the kernels do), the first-maximum prior by unclamped IoU at that cell (YOLOv3.py:160-200)."""
+        h, w = r.shape[0], r.shape[1]
+        with torch.no_grad():
+            gn = g / torch.tensor([norm] * 4 + [1.0], device=self.device, dtype=self.dtype)
+            gyx, ghw, lab = gn[:, :2], gn[:, 2:4], gn[:, 4].long()
+            fl = torch.floor(gyx).long()
+            if clamp:
+                fl = torch.stack([fl[:, 0].clamp(0, h - 1), fl[:, 1].clamp(0, w - 1)], dim=1)
+            ayx = (fl.to(self.dtype) + 0.5)[:, None, :]
+            a1, a2 = ayx - pri[None] / 2, ayx + pri[None] / 2
+            g1, g2 = (gyx - ghw / 2.0)[:, None, :], (gyx + ghw / 2.0)[:, None, :]
+            inter = (torch.minimum(g2, a2) - torch.maximum(g1, a1)).prod(-1)        # not clamped (:171-173)
+            iou = inter / (pri.prod(-1)[None] + (g2 - g1).prod(-1) - inter)
+            mx, idx = iou.max(dim=-1)
+        return dict(r=r, pri=pri, gyx=gyx, ghw=ghw, lab=lab, fl=fl, g1=g1[:, 0], g2=g2[:, 0], idx=idx, mx=mx, h=h, w=w)
+
+    def _yolo_terms(self, L_, m, nc, thr, acc):
+        """acc = (coord, class, obj, noobj) sums plus one level's terms: the positive terms of the GTs that mask m
+        selects, the no-object term of every (cell, prior) whose cell holds no GT and whose best IoU with the GTs is
+        <= thr."""
+        r, pri = L_["r"], L_["pri"]
+        bce = F.binary_cross_entropy_with_logits
+        coord, cls_l, obj_l, noobj = acc
+        gi = torch.nonzero(m).squeeze(1)
+        if gi.numel():
+            rws = r[L_["fl"][gi, 0], L_["fl"][gi, 1], L_["idx"][gi]]                 # [n,row]
+            tyx = L_["gyx"][gi] - torch.floor(L_["gyx"][gi])
+            thw = torch.log(L_["ghw"][gi] / pri[L_["idx"][gi]])
+            coord = coord + bce(rws[:, nc:nc + 2], tyx, reduction="sum") \
+                + 0.5 * ((rws[:, nc + 2:nc + 4] - thw) ** 2).sum()
+            cls_l = cls_l + bce(rws[:, :nc], F.one_hot(L_["lab"][gi], nc).to(self.dtype), reduction="sum")
+            obj_l = obj_l + bce(rws[:, nc + 4], torch.ones_like(rws[:, nc + 4]), reduction="sum")
+        h, w, a = L_["h"], L_["w"], pri.shape[0]
+        with torch.no_grad():
+            occ = torch.zeros((h, w), dtype=torch.bool, device=self.device)
+            occ[L_["fl"][:, 0], L_["fl"][:, 1]] = True
+            cy = (torch.arange(h, device=self.device, dtype=self.dtype) + 0.5).view(h, 1, 1, 1).expand(h, w, a, 1)
+            cx = (torch.arange(w, device=self.device, dtype=self.dtype) + 0.5).view(1, w, 1, 1).expand(h, w, a, 1)
+            ayx = torch.cat([cy, cx], dim=-1)
+            yx_nb = ayx - pri.view(1, 1, a, 2) / 2.0        # really y1x1, re-used as a centre (:249-262)
+            hw_nb = ayx + pri.view(1, 1, a, 2) / 2.0        # really y2x2, re-used as a size
+            b1 = (yx_nb - hw_nb / 2.0)[..., None, :]
+            b2 = (yx_nb + hw_nb / 2.0)[..., None, :]
+            gg1, gg2 = L_["g1"].view(1, 1, 1, -1, 2), L_["g2"].view(1, 1, 1, -1, 2)
+            inter = (torch.minimum(gg2, b2) - torch.maximum(gg1, b1)).prod(-1)
+            iou = (inter / ((b2 - b1).prod(-1) + (gg2 - gg1).prod(-1) - inter)).max(dim=-1).values
+            mask = ((iou <= thr) & (~occ)[..., None]).to(self.dtype)
+        noobj = noobj + (bce(r[..., nc + 4], torch.zeros_like(r[..., nc + 4]), reduction="none") * mask).sum()
+        return coord, cls_l, obj_l, noobj
+
+    def _yolo_scales(self):
+        return (float(self.cfg["coord_scale"]), float(self.cfg["noobj_scale"]), float(self.cfg["obj_scale"]),
+                float(self.cfg["class_scale"]))
+
     def yolo_image_loss(self, row, gt):
         """YOLOv3.py:115-318 for one image, quirks kept (see oracle/loss.py::yolo_image_loss): returns pos_loss + neg_loss."""
         nc = self.row - 5
-        cs, ns = float(self.cfg["coord_scale"]), float(self.cfg["noobj_scale"])
-        os_, ks = float(self.cfg["obj_scale"]), float(self.cfg["class_scale"])
+        cs, ns, os_, ks = self._yolo_scales()
         gt = torch.as_tensor(gt, device=self.device, dtype=self.dtype)
         cnt = int(torch.argmin(gt[:, 0]).item())
         g = gt[:cnt]
@@ -480,57 +542,42 @@ class GraphTrainer:
         for k, (h, w, a) in enumerate(self.net.levels):
             r = row[off:off + h * w * a].view(h, w, a, self.row)
             off += h * w * a
-            with torch.no_grad():
-                pri = torch.tensor(self.cfg["priors"][k], device=self.device, dtype=self.dtype) / pstride[k]
-                gn = g / torch.tensor([norm[k]] * 4 + [1.0], device=self.device, dtype=self.dtype)
-                gyx, ghw, lab = gn[:, :2], gn[:, 2:4], gn[:, 4].long()
-                fl = torch.floor(gyx).long()
-                ayx = (fl.to(self.dtype) + 0.5)[:, None, :]
-                a1, a2 = ayx - pri[None] / 2, ayx + pri[None] / 2
-                g1, g2 = (gyx - ghw / 2.0)[:, None, :], (gyx + ghw / 2.0)[:, None, :]
-                inter = (torch.minimum(g2, a2) - torch.maximum(g1, a1)).prod(-1)        # not clamped (:171-173)
-                iou = inter / (pri.prod(-1)[None] + (g2 - g1).prod(-1) - inter)
-                mx, idx = iou.max(dim=-1)
-            lv.append(dict(r=r, pri=pri, gyx=gyx, ghw=ghw, lab=lab, fl=fl, g1=g1[:, 0], g2=g2[:, 0], idx=idx, mx=mx, h=h, w=w))
+            pri = torch.tensor(self.cfg["priors"][k], device=self.device, dtype=self.dtype) / pstride[k]
+            lv.append(self._yolo_level(r, pri, g, norm[k]))
         m1 = (lv[0]["mx"] > lv[1]["mx"]) & (lv[0]["mx"] > lv[2]["mx"])
         m2 = (lv[1]["mx"] > lv[0]["mx"]) & (lv[1]["mx"] > lv[2]["mx"])
         m3 = ~(m1 | m2)
-        bce = F.binary_cross_entropy_with_logits
-        coord = cls_l = obj_l = noobj = 0.0
+        acc = (0.0, 0.0, 0.0, 0.0)
         for L_, m in zip(lv, (m1, m2, m3)):
-            r, pri = L_["r"], L_["pri"]
-            gi = torch.nonzero(m).squeeze(1)
-            if gi.numel():
-                rws = r[L_["fl"][gi, 0], L_["fl"][gi, 1], L_["idx"][gi]]                 # [n,row]
-                tyx = L_["gyx"][gi] - torch.floor(L_["gyx"][gi])
-                thw = torch.log(L_["ghw"][gi] / pri[L_["idx"][gi]])
-                coord = coord + bce(rws[:, nc:nc + 2], tyx, reduction="sum") \
-                    + 0.5 * ((rws[:, nc + 2:nc + 4] - thw) ** 2).sum()
-                cls_l = cls_l + bce(rws[:, :nc], F.one_hot(L_["lab"][gi], nc).to(self.dtype), reduction="sum")
-                obj_l = obj_l + bce(rws[:, nc + 4], torch.ones_like(rws[:, nc + 4]), reduction="sum")
-            h, w, a = L_["h"], L_["w"], pri.shape[0]
-            with torch.no_grad():
-                occ = torch.zeros((h, w), dtype=torch.bool, device=self.device)
-                occ[L_["fl"][:, 0], L_["fl"][:, 1]] = True
-                cy = (torch.arange(h, device=self.device, dtype=self.dtype) + 0.5).view(h, 1, 1, 1).expand(h, w, a, 1)
-                cx = (torch.arange(w, device=self.device, dtype=self.dtype) + 0.5).view(1, w, 1, 1).expand(h, w, a, 1)
-                ayx = torch.cat([cy, cx], dim=-1)
-                yx_nb = ayx - pri.view(1, 1, a, 2) / 2.0        # really y1x1, re-used as a centre (:249-262)
-                hw_nb = ayx + pri.view(1, 1, a, 2) / 2.0        # really y2x2, re-used as a size
-                b1 = (yx_nb - hw_nb / 2.0)[..., None, :]
-                b2 = (yx_nb + hw_nb / 2.0)[..., None, :]
-                gg1, gg2 = L_["g1"].view(1, 1, 1, -1, 2), L_["g2"].view(1, 1, 1, -1, 2)
-                inter = (torch.minimum(gg2, b2) - torch.maximum(gg1, b1)).prod(-1)
-                iou = (inter / ((b2 - b1).prod(-1) + (gg2 - gg1).prod(-1) - inter)).max(dim=-1).values
-                mask = ((iou <= 0.5) & (~occ)[..., None]).to(self.dtype)
-            noobj = noobj + (bce(r[..., nc + 4], torch.zeros_like(r[..., nc + 4]), reduction="none") * mask).sum()
+            acc = self._yolo_terms(L_, m, nc, 0.5, acc)
+        coord, cls_l, obj_l, noobj = acc
         ng = float(cnt)
         return (cs * coord + ks * cls_l + os_ * obj_l) / ng + ns * noobj / ng
+
+    def yolo2_image_loss(self, row, gt):
+        """YOLOv2.py:105-173 for one image: the YOLOv3 terms on its one level (GT / 32, priors in grid cells, the GT's
+        cell clamped to the grid), the no-object term where the best IoU <= 0.6; cs * coord + ks * class + os * obj +
+        ns * noobj, NOT divided by the GT count -- an image without boxes gets the no-object term of every row."""
+        nc = self.row - 5
+        cs, ns, os_, ks = self._yolo_scales()
+        gt = torch.as_tensor(gt, device=self.device, dtype=self.dtype)
+        cnt = int(torch.argmin(gt[:, 0]).item())
+        if cnt == 0:  # no GT: no positive term, and every row is a no-object row (YOLOv2.py:155-171 over zero GTs)
+            obj = row[:, nc + 4]
+            return ns * F.binary_cross_entropy_with_logits(obj, torch.zeros_like(obj), reduction="sum")
+        g = gt[:cnt]
+        (h, w, a), = self.net.levels
+        pri = torch.tensor(self.cfg["priors"], device=self.device, dtype=self.dtype)
+        L_ = self._yolo_level(row.view(h, w, a, self.row), pri, g, 32.0, clamp=True)
+        every = torch.ones(cnt, dtype=torch.bool, device=self.device)
+        coord, cls_l, obj_l, noobj = self._yolo_terms(L_, every, nc, 0.6, (0.0, 0.0, 0.0, 0.0))
+        return cs * coord + ks * cls_l + os_ * obj_l + ns * noobj
 
     def image_loss(self, row, gt):
         if self.kind == "ssd":
             return self._ssd.image_loss(row, gt)[0]
-        return {"retina": self.retina_image_loss, "fcos": self.fcos_image_loss, "yolo": self.yolo_image_loss}[self.kind](row, gt)
+        return {"retina": self.retina_image_loss, "fcos": self.fcos_image_loss, "yolo": self.yolo_image_loss,
+                "yolo2": self.yolo2_image_loss}[self.kind](row, gt)
 
     def total_loss(self, rows, ground_truth):
         if self._loss_kernels is not None:
@@ -540,7 +587,7 @@ class GraphTrainer:
             data = torch.stack([torch.as_tensor(p, device=self.device, dtype=self.dtype) for p in per]).sum() \
                 / rows.shape[0]
         if self.kind == "yolo":
-            data = 0.5 * data                                   # YOLOv3.py:313
+            data = 0.5 * data                                   # YOLOv3.py:313 (YOLOv2.py:174: no 0.5)
         l2 = sum((p * p).sum() for p in self.params.values()) * 0.5
         return data + self.weight_decay * l2, data
 
