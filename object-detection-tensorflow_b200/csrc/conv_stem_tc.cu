@@ -53,10 +53,15 @@ struct StemK {
   static constexpr int KSTEPS = (KREAL + 15) / 16;
   static constexpr int NBLK = (KSTEPS * 16 + 63) / 64;
   static constexpr int STAGES = NBLK >= 4 ? 3 : ST_MAX_STAGES;  // 64 KiB stages: three fit
+  // CTAs per SM the register budget is built for.  The 3x3 fp32-gather stems take two: with one, the single consumer
+  // warpgroup has one warp per scheduler and its epilogue runs at the latency of each dependent instruction (the layer
+  // took 3x its HBM-write floor); two CTAs (<= 85 registers per thread, 2 x ~93 KiB of shared memory) interleave two
+  // epilogues and four gathers per SM.  The 7x7 variants keep one: their gathers hold the whole window in registers.
+  static constexpr int MIN_CTAS = KS == 3 ? 2 : 1;
 };
 
 template <int COUT, int KS, int STRIDE, bool H4>
-__global__ void __launch_bounds__(ST_THREADS)
+__global__ void __launch_bounds__(ST_THREADS, StemK<KS, H4>::MIN_CTAS)
     conv_stem_tc_kernel(const void* __restrict__ img_any, const __half* __restrict__ wgt,
                         const __grid_constant__ StemGeom g, const __grid_constant__ Epi e) {
   const float* img = reinterpret_cast<const float*>(img_any);
@@ -282,11 +287,13 @@ __global__ void __launch_bounds__(ST_THREADS)
     // Staging row h*16 + i holds tile row 64h + 16w + i.
     uint8_t* warp_stage = smem_raw + (stage_out - raw) + (uint32_t)w * ST_WARP_STAGE;
     for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
-      float acc[2][COUT / 2];
       mbar_wait(full_bar(stage), phase);
-      wg_fence();
+      // the two 64-row halves one after the other: one half's accumulators live at a time (the two-CTA budget of the
+      // 3x3 variants holds COUT/2 of them, not COUT); each half's K steps are the same MMAs in the same order
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
+        float acc[COUT / 2];
+        wg_fence();
 #pragma unroll
         for (int k = 0; k < KSTEPS; ++k) {
           const uint32_t blk = k >> 2, kin = k & 3;
@@ -294,31 +301,30 @@ __global__ void __launch_bounds__(ST_THREADS)
               make_desc_sw128(a_base + (uint32_t)stage * A_BYTES + blk * (128 * 128) + (uint32_t)h * (64 * 128)) +
               (uint64_t)(2 * kin);
           const uint64_t bdesc = make_desc_sw128(b_base + blk * (COUT * 128)) + (uint64_t)(2 * kin);
-          wg_mma_f16<COUT>(acc[h], adesc, bdesc, (uint32_t)(k != 0));
+          wg_mma_f16<COUT>(acc, adesc, bdesc, (uint32_t)(k != 0));
         }
-      }
-      wg_commit();
-      wg_wait<0>();
-      // the stage has been read: hand it back before the epilogue
-      __syncwarp();
-      if (lane == 0) mbar_arrive(empty_bar(stage));
-      if (++stage == ST_STAGES) {
-        stage = 0;
-        phase ^= 1u;
-      }
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
+        wg_commit();
+        wg_wait<0>();
+        if (h == 1) {
+          // the stage has been read: hand it back before the rest of the epilogue
+          __syncwarp();
+          if (lane == 0) mbar_arrive(empty_bar(stage));
+          if (++stage == ST_STAGES) {
+            stage = 0;
+            phase ^= 1u;
+          }
+        }
         uint8_t* r0 = warp_stage + (h * 16 + (lane >> 2)) * ST_PITCH;
 #pragma unroll
         for (int i = 0; i < COUT / 8; ++i) {
           const int c0 = 8 * i + 2 * (lane & 3);
           const float sc0 = s_scale[c0], sc1 = s_scale[c0 + 1], sh0 = s_shift[c0], sh1 = s_shift[c0 + 1];
           *reinterpret_cast<__half2*>(r0 + c0 * 2) =
-              __floats2half2_rn(apply_act(fmaf(acc[h][4 * i], sc0, sh0), e.act),
-                                apply_act(fmaf(acc[h][4 * i + 1], sc1, sh1), e.act));
+              __floats2half2_rn(apply_act(fmaf(acc[4 * i], sc0, sh0), e.act),
+                                apply_act(fmaf(acc[4 * i + 1], sc1, sh1), e.act));
           *reinterpret_cast<__half2*>(r0 + 8 * ST_PITCH + c0 * 2) =
-              __floats2half2_rn(apply_act(fmaf(acc[h][4 * i + 2], sc0, sh0), e.act),
-                                apply_act(fmaf(acc[h][4 * i + 3], sc1, sh1), e.act));
+              __floats2half2_rn(apply_act(fmaf(acc[4 * i + 2], sc0, sh0), e.act),
+                                apply_act(fmaf(acc[4 * i + 3], sc1, sh1), e.act));
         }
       }
       __syncwarp();
