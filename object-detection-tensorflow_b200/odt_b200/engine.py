@@ -30,6 +30,13 @@ def _round_up(x, m):
     return (x + m - 1) // m * m
 
 
+def slice_store_width(cout, tensor_cores):
+    """Channels per output pixel a convolution may store into an extra output (out1 / out2) from its first channel:
+    the tensor-core kernels store whole 32-channel chunks up to Cout_pad (zero past Cout), the CUDA-core kernels
+    exactly Cout.  Net.concat relies on it: a part must not reach the next part's channels."""
+    return _round_up(cout, 32) if tensor_cores else cout
+
+
 def same_pad(size, k, stride, dil=1):
     """TF SAME geometry (SURVEY App. A.1); host twin of odt_same_pad."""
     out = -(-size // stride)
@@ -114,6 +121,15 @@ class ConvOp(Op):
         self.writes = (y,) if y is not None else ()
         self.flops = 0
 
+    def on_tensor_cores(self, net):
+        """odt_conv2d_f16_tc runs this layer (conv_tc and the kernels its planner picks); otherwise the CUDA-core
+        direct convolution or the stem."""
+        return net.precision == "fp16" and net.allow_tc and not self.is_image and self.x.ld % 64 == 0
+
+    def slice_channels(self, net):
+        """Channels of each output pixel this layer may store into an extra output (slice_store_width)."""
+        return slice_store_width(self.y.C, self.on_tensor_cores(net))
+
     def prepare(self, net):
         x, W = self.x, net.weights
         dev = net.device
@@ -123,7 +139,7 @@ class ConvOp(Op):
         self.cout = cout
         f16 = net.precision == "fp16"
         adt = torch.float16 if f16 else torch.float32
-        self.use_tc = f16 and (not self.is_image) and x.ld % 64 == 0 and net.allow_tc
+        self.use_tc = self.on_tensor_cores(net)
         ohwi = np.transpose(kern, (3, 0, 1, 2))  # [Cout,R,S,Cin]
         if self.use_tc:
             cpad = _round_up(cout, 32)
@@ -584,13 +600,14 @@ class Net:
         for op in self.ops:
             if isinstance(op, AffineActOp):
                 q = producer.get(id(op.x))
+                if op.y.base is not None:
+                    self._check_slice_producer(q, op.y)
                 ok = isinstance(q, (ConvOp, UpsampleAddOp, PoolOp)) and q.pre is None
                 if ok and isinstance(q, ConvOp):
                     ok = q.head is None
                 # second pre-activation of the same tensor: tensor-core convs (third epilogue output) and pools
                 second = (not ok and isinstance(q, ConvOp) and q.head is None and q.pre is not None
-                          and q.pre2 is None and not q.is_image and self.precision == "fp16" and self.allow_tc
-                          and q.x.ld % 64 == 0)
+                          and q.pre2 is None and q.on_tensor_cores(self))
                 second = second or (not ok and isinstance(q, PoolOp) and q.pre is not None and q.pre2 is None)
                 if ok or second:
                     if ok:
@@ -606,6 +623,22 @@ class Net:
                 raise ValueError("concat: the producer of %s cannot store its channel slice" % op.x.name)
             kept.append(op)
         self.ops = kept
+
+    def _check_slice_producer(self, q, v):
+        """A concat part `v` is stored by its producer `q` as an extra epilogue output at the concat's pixel stride.
+        Only the convolution kernels take that stride (the pooling and upsampling kernels address their extra output
+        with their own), and a producer that stores whole chunks of channels must not reach the next part's first
+        channels, or past the concat's row for the last part."""
+        if not isinstance(q, ConvOp) or q.head is not None:
+            raise ValueError("concat: the producer of %s cannot store its channel slice (%s)"
+                             % (v.name, type(q).__name__ if q is not None else "no producer"))
+        parts = v.base.parts
+        i = next(j for j, t in enumerate(parts) if t is v)
+        end = parts[i + 1].c0 if i + 1 < len(parts) else v.base.ld
+        stored = q.slice_channels(self)
+        if v.c0 + stored > end:
+            raise ValueError("concat: the producer of %s cannot store its channel slice (%d channels per pixel from "
+                             "channel %d reach past channel %d)" % (v.name, stored, v.c0, end))
 
     # -------------------------------------------------------------- halos ----
     STEM_TC_VARIANTS = {(3, 1, 64), (3, 1, 32), (7, 2, 16)}

@@ -50,6 +50,27 @@ def mask(shape, halo=0, c=None):
     return m
 
 
+def _bits(t):
+    return t.view(torch.int16 if t.dtype == torch.float16 else torch.int32)
+
+
+def assert_slice_writes(now, was, c0, cout, end, what):
+    """The write rules of a channel slice [c0, c0 + cout) of a wider tensor (Net.concat's parts): every element of the
+    slice written; channels [c0 + cout, end) untouched or +0 (the pad lanes of a producer that stores whole chunks);
+    every other channel keeps its initial bits.  Returns how many channels past the slice were written (with +0)."""
+    assert not bool((now[..., c0:c0 + cout] == SENT).any()), "%s: a slice element left unwritten" % what
+    pad = now[..., c0 + cout:end]
+    wrote = _bits(pad) != _bits(was[..., c0 + cout:end])
+    assert bool((~wrote | (_bits(pad) == 0)).all()), "%s: channels [c0 + Cout, %d) hold neither +0 nor the initial " \
+                                                     "contents" % (what, end)
+    assert torch.equal(_bits(now[..., :c0]), _bits(was[..., :c0])), "%s: channels below the slice written" % what
+    assert torch.equal(_bits(now[..., end:]), _bits(was[..., end:])), "%s: channels >= %d written" % (what, end)
+    if wrote.shape[-1] == 0:
+        return 0
+    cols = wrote.reshape(-1, wrote.shape[-1]).any(dim=0).nonzero()
+    return int(cols.max()) + 1 if cols.numel() else 0
+
+
 def interior(t, halo):
     return t[:, halo:t.shape[1] - halo, halo:t.shape[2] - halo] if halo else t
 
@@ -87,7 +108,7 @@ def last_conv_kernel():
 
 
 def model(kind, precision, **over):
-    """One of the five detectors with trained-style BN statistics (helpers.model_cfg), no checkpoint."""
+    """One of the six detectors with trained-style BN statistics (helpers.model_cfg), no checkpoint."""
     from helpers import model_cfg
     import FCOS
     import RetinaNet
@@ -102,4 +123,8 @@ def model(kind, precision, **over):
         return RetinaNet.RetinaNet(model_cfg("retinanet", precision=precision, bn_init="trained", **over), None)
     if kind == "yolov3":
         return YOLOv3.YOLOv3(model_cfg("yolov3", precision=precision, bn_init="trained", **over), None)
+    if kind == "yolov2":  # `over` takes _cfg's A (priors), nc (classes) and size as well
+        import YOLOv2
+        from test_gpu_yolov2 import _cfg
+        return YOLOv2.YOLOv2(_cfg(precision=precision, bn_init="trained", **over), None)
     return FCOS.FCOS(model_cfg("fcos", precision=precision, bn_init="trained", **over), None)

@@ -10,7 +10,7 @@ import pytest
 import torch
 
 import conv_ends_ref as R
-from gpu_harness import SENT, Guarded, interior, last_conv_kernel, mask
+from gpu_harness import SENT, Guarded, assert_slice_writes, interior, last_conv_kernel, mask
 
 pytestmark = pytest.mark.gpu
 
@@ -18,10 +18,11 @@ pytestmark = pytest.mark.gpu
 class ConvResult:
     """One _conv_case launch: the interior outputs [B, OH, OW, Cout] as float32 arrays (got, got1, got2; None where
     the output is absent), the launched kernel's name (kernel) and the worst error over every output as a fraction of
-    its per-element bound (worst, at most 1)."""
+    its per-element bound (worst, at most 1); with slice_at, how many channels past Cout out1 / out2 wrote (spill)."""
 
-    def __init__(self, got, got1, got2, kernel, worst):
+    def __init__(self, got, got1, got2, kernel, worst, spill=0):
         self.got, self.got1, self.got2, self.kernel, self.worst = got, got1, got2, kernel, worst
+        self.spill = spill
 
 
 def _bits(t):
@@ -53,12 +54,14 @@ def _assert_write_rules(g, halo, Cout, cpad, what):
 
 def _conv_case(B, H, W, Cin, Cout, k, stride, dil, mode, act="relu", residual=False, pre=False,
                bn=True, f32_out=False, seed=0, in_halo=0, out_halo=0, pool=0, pre2=False, no_out0=False, aux_halo=0,
-               off=0):
+               off=0, slice_at=None):
     """One convolution through odt_conv2d_f16_tc (mode 'tc') or odt_conv2d_direct ('direct16', 'direct32'), every
     output inside a sentinel-filled guarded buffer, checked against the float64 reference of tests/conv_ends_ref.py
     with the per-element bound of the path that ran (named by the library's launch record) and against the write
     rules of _assert_write_rules.  out1 = relu(v * s2 + h2), out2 = leaky(v * s3 + h3).  off: every output and the residual
-    start `off` elements past a 16-byte boundary.  Returns a ConvResult."""
+    start `off` elements past a 16-byte boundary.  slice_at = (c0, ld): out1 / out2 are channel slices [c0, c0 + Cout)
+    of wider sentinel-filled tensors with pixel stride ld (a Net.concat part), checked by assert_slice_writes with the
+    producer's store width (engine.slice_store_width).  Returns a ConvResult."""
     from odt_b200 import lib as L
     from odt_b200.engine import same_pad
     lib = L.load()
@@ -122,6 +125,12 @@ def _conv_case(B, H, W, Cin, Cout, k, stride, dil, mode, act="relu", residual=Fa
     p.in_halo, p.out0_halo = in_halo, out_halo
     ah = aux_halo
     ashape = (B, OH + 2 * ah, OW + 2 * ah, old)
+    c0, ald = 0, old
+    if slice_at is not None:
+        assert ah == 0
+        c0, ald = slice_at
+        ashape = (B, OH, OW, ald)
+    aoff = c0 * (2 if f16 else 4)           # byte offset of out1 / out2 in their buffers
     extras = []                             # (guarded buffer, scale, shift, activation) of out1 / out2
     for on, a2 in ((pre, "relu"), (pre2, "leaky")):
         if not on:
@@ -132,11 +141,11 @@ def _conv_case(B, H, W, Cin, Cout, k, stride, dil, mode, act="relu", residual=Fa
     if pre:
         g1, s2, h2, a2 = extras[0]
         p.scale2, p.shift2, p.act2 = s2.data_ptr(), h2.data_ptr(), R.ACTS[a2]
-        p.out1, p.out1_img_stride, p.out1_pix_stride, p.out1_halo = g1.ptr(), ashape[1] * ashape[2] * old, old, ah
+        p.out1, p.out1_img_stride, p.out1_pix_stride, p.out1_halo = g1.ptr() + aoff, ashape[1] * ashape[2] * ald, ald, ah
     if pre2:
         g2, s3, h3, a3 = extras[-1]
         p.scale3, p.shift3, p.act3 = s3.data_ptr(), h3.data_ptr(), R.ACTS[a3]
-        p.out2, p.out2_img_stride, p.out2_pix_stride, p.out2_halo = g2.ptr(), ashape[1] * ashape[2] * old, old, ah
+        p.out2, p.out2_img_stride, p.out2_pix_stride, p.out2_halo = g2.ptr() + aoff, ashape[1] * ashape[2] * ald, ald, ah
     st = torch.cuda.current_stream().cuda_stream
 
     def launch():
@@ -167,11 +176,18 @@ def _conv_case(B, H, W, Cin, Cout, k, stride, dil, mode, act="relu", residual=Fa
             worst["out0"] = R.ratio(got0, R.pool2(v), R.pool2(b0))
         else:
             worst["out0"] = R.ratio(got0, v, b0)
-    gots = []
+    gots, spill = [], 0
     for i, (g, s2, h2, a2) in enumerate(extras):
         name = "out%d" % (i + 1 if pre else 2)
-        _assert_write_rules(g, ah, Cout, cpad, name)
-        got = interior(g.t, ah)[..., :Cout]
+        if slice_at is None:
+            _assert_write_rules(g, ah, Cout, cpad, name)
+            got = interior(g.t, ah)[..., :Cout]
+        else:
+            from odt_b200.engine import slice_store_width
+            g.assert_outside_untouched()
+            end = c0 + slice_store_width(Cout, mode == "tc")
+            spill = max(spill, assert_slice_writes(g.t, g.initial(), c0, Cout, end, name))
+            got = g.t[..., c0:c0 + Cout]
         if no_out0:
             t = R.consumer(v, s2, h2, a2)
             worst[name] = R.ratio(got, t, R.bound_through(t, b0, s2, f16))
@@ -187,7 +203,7 @@ def _conv_case(B, H, W, Cin, Cout, k, stride, dil, mode, act="relu", residual=Fa
         assert r <= 1.0, (kernel, n, r, at)
     got1 = gots[0] if pre else None
     got2 = gots[-1] if pre2 else None
-    return ConvResult(got0.float().cpu().numpy(), got1, got2, kernel, top)
+    return ConvResult(got0.float().cpu().numpy(), got1, got2, kernel, top, spill)
 
 
 TC_SHAPES = [

@@ -365,9 +365,11 @@ INSITU = [("ssd300", "fp16", 64, {}), ("ssd512", "fp16", 8, {}),
           ("yolov3", "fp16", 32, {"data_shape": [416, 416, 3], "num_classes": 20}),
           ("fcos", "fp16", 4, {"data_shape": [1024, 1024, 3]}),
           ("fcos", "fp32", 4, {"data_shape": [1024, 1024, 3]}),
-          ("retinanet", "fp32", 2, {"data_shape": [512, 512, 3]})]
+          ("retinanet", "fp32", 2, {"data_shape": [512, 512, 3]}),
+          ("yolov2", "fp16", 64, {}), ("yolov2", "fp16", 8, {"size": 200}), ("yolov2", "fp32", 2, {})]
 INSITU_IDS = ["ssd300-fp16-B64", "ssd512-fp16-B8", "retinanet800-fp16-B16", "retinanet800-basic-fp16-B16",
-              "yolov3-416-fp16-B32", "fcos1024-fp16-B4", "fcos1024-fp32-B4", "retinanet512-fp32-B2"]
+              "yolov3-416-fp16-B32", "fcos1024-fp16-B4", "fcos1024-fp32-B4", "retinanet512-fp32-B2",
+              "yolov2-480-fp16-B64", "yolov2-200-fp16-B8", "yolov2-480-fp32-B2"]
 
 
 @pytest.mark.gpu
@@ -375,20 +377,34 @@ INSITU_IDS = ["ssd300-fp16-B64", "ssd512-fp16-B8", "retinanet800-fp16-B16", "ret
 def test_body_convs_in_situ(built, kind, precision, B, over):
     """Every body convolution of the network at its full per-GPU geometry, on its real buffers after one eager
     forward: launched kernel (the library's record of the op's own launch, against the host planners), out0 (pooled
-    or not), residual, out1 / out2 against the bound, and zero halo rings and pad lanes."""
+    or not), residual, out1 / out2 against the bound (a concat part's out1 read through its slice view), and zero
+    halo rings and pad lanes.  A concat tensor is NaN-filled before the forward: its parts' slices must tile it."""
     from odt_b200 import engine as E
     m = _model(kind, precision, **over)
     net = m.engine(B, graph=False)
     img = torch.from_numpy(np.random.default_rng(1).integers(0, 256, (B, net.in_h, net.in_w, 3)).astype(np.float32))
     net.image_buf.copy_(img)
+    concats = [t for t in net.acts if t.parts]
+    for y in concats:
+        y.buf[..., :y.C] = float("nan")
     net.forward(with_tail=False)
     torch.cuda.synchronize()
-    # every activation owns its buffer: re-launching one op cannot change another op's input
+    for y in concats:
+        assert [(v.c0, v.c0 + v.C) for v in y.parts] == list(zip([0] + [v.c0 + v.C for v in y.parts[:-1]],
+                                                                 [v.c0 + v.C for v in y.parts]))
+        assert y.parts[-1].c0 + y.parts[-1].C == y.C
+        for v in y.parts:
+            assert v.buf.data_ptr() == y.buf.data_ptr() + v.c0 * y.buf.element_size() and v.buf.stride() == y.buf.stride()
+        assert not bool(torch.isnan(y.buf).any()), "%s: a channel no slice covers" % y.name
+        if y.ld > y.C:
+            assert not bool(y.buf[..., y.C:].ne(0).any()), "%s: pad lanes written" % y.name
+    # every activation owns its buffer (a concat's slices are views of it): re-launching one op cannot change another
+    # op's input
     acts = {}
     for op in net.ops:
         extra = tuple(pr[2] for pr in (getattr(op, "pre", None), getattr(op, "pre2", None)) if pr is not None)
         for t in tuple(op.reads) + tuple(op.writes) + extra:
-            if t is not None and t.buf is not None:
+            if t is not None and t.buf is not None and t.base is None:
                 acts[id(t)] = t
     spans = sorted((t.buf.data_ptr(), t.buf.data_ptr() + t.buf.numel() * t.buf.element_size(), t.name)
                    for t in acts.values())

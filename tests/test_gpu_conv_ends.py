@@ -18,6 +18,7 @@ import pytest
 import torch
 
 import conv_ends_ref as R
+import prior_count_ref as PR
 from gpu_harness import Guarded, kernels_launched
 from gpu_harness import interior as _interior
 from gpu_harness import mask as _mask
@@ -542,10 +543,18 @@ INSITU = [("ssd300", "fp16", 64, {}), ("ssd512", "fp16", 8, {}),
           ("yolov3", "fp16", 32, {"data_shape": [416, 416, 3], "num_classes": 80}),
           ("fcos", "fp16", 4, {"data_shape": [1024, 1024, 3]}),
           ("fcos", "fp32", 4, {"data_shape": [1024, 1024, 3]}),
-          ("retinanet", "fp32", 2, {"data_shape": [512, 512, 3]})]
+          ("retinanet", "fp32", 2, {"data_shape": [512, 512, 3]}),
+          ("yolov2", "fp16", 64, {}), ("yolov2", "fp16", 8, {"size": 200}),
+          # the widest head the code accepts (9 priors x 133 = 1197 channels) and the narrowest (6)
+          ("yolov2", "fp16", 8, {"A": 9, "nc": 128}), ("yolov2", "fp16", 8, {"A": 1, "nc": 1}),
+          ("yolov3", "fp16", 8, {"data_shape": [416, 416, 3], "num_classes": 128, "num_priors": 9,
+                                 "priors": PR.priors_for(9)}),
+          ("yolov3", "fp16", 8, {"data_shape": [416, 416, 3], "num_classes": 1, "num_priors": 1,
+                                 "priors": PR.priors_for(1)})]
 INSITU_IDS = ["ssd300-fp16-B64", "ssd512-fp16-B8", "retinanet800-fp16-B16", "retinanet800-basic-fp16-B16",
               "yolov3-416-nc20-fp16-B32", "yolov3-416-nc80-fp16-B32", "fcos1024-fp16-B4", "fcos1024-fp32-B4",
-              "retinanet512-fp32-B2"]
+              "retinanet512-fp32-B2", "yolov2-480-fp16-B64", "yolov2-200-fp16-B8", "yolov2-480-A9-nc128-fp16-B8",
+              "yolov2-480-A1-nc1-fp16-B8", "yolov3-416-A9-nc128-fp16-B8", "yolov3-416-A1-nc1-fp16-B8"]
 
 
 @pytest.mark.gpu

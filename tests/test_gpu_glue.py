@@ -717,10 +717,12 @@ def _insitu_concat(net, op):
 
 INSITU = [("ssd300", "fp16", 64, {}), ("retinanet", "fp16", 16, {"data_shape": [800, 800, 3]}),
           ("yolov3", "fp16", 32, {"data_shape": [416, 416, 3]}), ("fcos", "fp16", 4, {"data_shape": [1024, 1024, 3]}),
-          ("fcos", "fp32", 4, {"data_shape": [1024, 1024, 3]}), ("ssd512", "fp16", 1, {})]
+          ("fcos", "fp32", 4, {"data_shape": [1024, 1024, 3]}), ("ssd512", "fp16", 1, {}),
+          ("yolov2", "fp16", 64, {}), ("yolov2", "fp16", 8, {"size": 200}), ("yolov2", "fp32", 2, {})]
 
 
-@pytest.mark.parametrize("kind,precision,B,over", INSITU, ids=["%s-%s-B%d" % (k, p, b) for k, p, b, _ in INSITU])
+@pytest.mark.parametrize("kind,precision,B,over", INSITU, ids=["%s-%s-B%d%s" % (k, p, b, "-%d" % o["size"] if "size" in o
+                                                                            else "") for k, p, b, o in INSITU])
 def test_glue_ops_in_situ(built, kind, precision, B, over):
     """Every glue op of the network at its full per-GPU geometry, checked on its actual input and output buffers
     after one eager forward (every activation owns its buffer, so all of them are live): the planner's own launch
