@@ -985,8 +985,11 @@ __global__ void __launch_bounds__(kLossThreads)
     const float inv = s_inv[c.lvl];
     unsigned cmask[W];
     const FcosCell t = fcos_cell(c, cnt, s_gt, cmask);
-    float gbox = 0.f;  // lanes 0..3: the gradient of distance column nfg + 1 + lane
-    if (t.loc) {
+    // lanes 0..3: the gradient of distance column nfg + 1 + lane.  The IoU term is -log(IoU + 1e-12) * loc on every
+    // location (FCOS.py:319-320): outside every GT it is 0 * the same product, +0 for a finite product and NaN where
+    // an exp() overflowed, as in the reference graph.
+    float gbox;
+    {
       const float pl = expf(r[nfg + 1]), pr = expf(r[nfg + 2]), pt = expf(r[nfg + 3]), pb = expf(r[nfg + 4]);
       const float iw = __fadd_rn(fminf(t.dl, pl), fminf(t.dr, pr)), ih = __fadd_rn(fminf(t.dt, pt), fminf(t.db, pb));
       const float inter = __fmul_rn(iw, ih);
@@ -1001,7 +1004,8 @@ __global__ void __launch_bounds__(kLossThreads)
       const float psum = lane < 2 ? __fadd_rn(pt, pb) : __fadd_rn(pl, pr);      // d (pl+pr)(pt+pb) / d p_k
       const float dinter = pk < dk ? other : 0.f;
       const float diou = __fdiv_rn(dinter - iou * (psum - dinter), u);
-      gbox = dl_diou * diou * pk * inv;
+      const float g = dl_diou * diou * pk * inv;
+      gbox = t.loc ? g : __fadd_rn(__fmul_rn(g, 0.f), 0.f);
     }
     for (int k0 = 0; k0 < row; k0 += 32) {
       const int k = k0 + lane;

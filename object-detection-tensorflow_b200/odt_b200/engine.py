@@ -1043,12 +1043,14 @@ class Tail:
         #mined negatives) per image."""
         return self._loss_call(net, kind, ground_truth, return_info, False, kw)
 
-    def loss_grad(self, net, kind, ground_truth, return_info=False, **kw):
+    def loss_grad(self, net, kind, ground_truth, return_info=False, grad_out=None, **kw):
         """odt_<kind>_loss_grad on the rows this tail reads (arguments as `loss`): (loss float32 [B], gradient
-        d loss[b] / d rows[b] float32 [B,N,row]), and for 'ssd' with return_info=True the info as a third item."""
-        return self._loss_call(net, kind, ground_truth, return_info, True, kw)
+        d loss[b] / d rows[b] float32 [B,N,row]), and for 'ssd' with return_info=True the info as a third item.
+        grad_out: the float32 device buffer shaped as the rows to write the gradient into (default: a fresh
+        uninitialised one), e.g. one pre-filled with a sentinel to show the kernel writes every element."""
+        return self._loss_call(net, kind, ground_truth, return_info, True, kw, grad_out)
 
-    def _loss_call(self, net, kind, ground_truth, return_info, with_grad, kw):
+    def _loss_call(self, net, kind, ground_truth, return_info, with_grad, kw, grad_out=None):
         if kind not in self.LOSS_SCALARS:
             raise ValueError(kind)
         if return_info and kind != "ssd":
@@ -1061,7 +1063,12 @@ class Tail:
         scratch = torch.zeros((nbytes + 7) // 8, dtype=torch.int64, device=net.device)
         out = torch.zeros(B, dtype=torch.float32, device=net.device)
         info = torch.zeros((B, 3), dtype=torch.int32, device=net.device) if return_info else None
-        grad = torch.empty_like(self.head_buf) if with_grad else None
+        grad = None
+        if with_grad:
+            grad = torch.empty_like(self.head_buf) if grad_out is None else grad_out
+            if (grad.shape != self.head_buf.shape or grad.dtype != torch.float32 or grad.device != self.head_buf.device
+                    or not grad.is_contiguous()):
+                raise ValueError("grad_out: a contiguous float32 buffer shaped as the rows, on their device")
         args = [float(kw.get(k, d)) for k, d in self.LOSS_SCALARS[kind]] + [scratch.data_ptr(), out.data_ptr()]
         if kind == "ssd":
             args.append(None if info is None else info.data_ptr())
@@ -1231,9 +1238,9 @@ class RowsHarness:
         """Training-loss forward kernels on the same rows (Tail.loss)."""
         return self.tail.loss(self, kind, ground_truth, return_info, **kw)
 
-    def loss_grad(self, kind, ground_truth, return_info=False, **kw):
+    def loss_grad(self, kind, ground_truth, return_info=False, grad_out=None, **kw):
         """Training-loss gradient kernels on the same rows (Tail.loss_grad): (loss [B], gradient [B,N,row])."""
-        return self.tail.loss_grad(self, kind, ground_truth, return_info, **kw)
+        return self.tail.loss_grad(self, kind, ground_truth, return_info, grad_out, **kw)
 
 
 # ------------------------------------------------------------------ weights --

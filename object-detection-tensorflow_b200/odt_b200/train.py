@@ -244,6 +244,12 @@ def _act(x, act):
     return x
 
 
+def tf_minimum(x, y):
+    """min(x, y) with TF's Minimum gradient: a tie sends the whole gradient to x (torch.minimum splits it 0.5 / 0.5).
+    FCOS.py:315-316 writes tf.minimum(GT distance, predicted distance), so at a tie the prediction gets none."""
+    return torch.where(x <= y, x, y)
+
+
 class GraphTrainer:
     """Training state + step of SSD300 / SSD512 / RetinaNet / YOLOv3 / YOLOv2 / FCOS (reference: SSD300.py:129-155,
     RetinaNet.py:193-222, YOLOv3.py:115-318, YOLOv2.py:103-181, FCOS.py:153-195).  Same interface as SSDTrainer."""
@@ -464,7 +470,7 @@ class GraphTrainer:
                     hgt[..., c] = heat[..., cid == c].max(dim=-1).values
             p = torch.exp(reg)
             pl, pr, pt, pb = p[..., 0], p[..., 1], p[..., 2], p[..., 3]
-            inter = (torch.minimum(dl, pl) + torch.minimum(dr, pr)) * (torch.minimum(dt, pt) + torch.minimum(db, pb))
+            inter = (tf_minimum(dl, pl) + tf_minimum(dr, pr)) * (tf_minimum(dt, pt) + tf_minimum(db, pb))
             union = (dl + dr) * (dt + db) + (pl + pr) * (pt + pb) - inter
             iou_loss = (-torch.log(inter / (union + 1e-12) + 1e-12) * loc).sum()
             center = F.binary_cross_entropy_with_logits(ctr, cgt, reduction="sum")

@@ -31,12 +31,7 @@ def _kw(kind, cfg):
 
 def reference(kind, levels, cfg, size, nc, row, gt):
     """(loss, gradient, dtype) of the restatement: float64 where its decisions are float32's (see above)."""
-    with np.errstate(all="ignore"):
-        l32, g32 = LR.grad(LR.restatement(kind, levels, cfg, size, nc, dtype=torch.float32), row, gt)
-        l64, g64 = LR.grad(LR.restatement(kind, levels, cfg, size, nc), row, gt)
-    if abs(l64 - l32) <= 1e-6 * max(abs(l32), 1.0):
-        return l64, g64, "float64"
-    return l32, g32, "float32"
+    return LR.reference(kind, levels, cfg, size, nc, row, gt)[:3]
 
 
 def check(kind, levels, size, cfg, rows, gt, nc=20, images=None):
