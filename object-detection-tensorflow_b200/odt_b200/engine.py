@@ -882,6 +882,9 @@ class Net:
         self.head_buf1 = torch.zeros_like(self.head_buf)
         t1 = copy.copy(self.tail)
         t1.prepare(self, head_buf=self.head_buf1)
+        # slot 1 decodes and selects with slot 0's parameter block as it stands, not as the config built it: a score
+        # threshold set on `tail.p` after the build (bench.py's dense-threshold RetinaNet) holds for every batch
+        C.memmove(C.byref(t1.p), C.byref(self.tail.p), C.sizeof(t1.p))
         self.tails = [self.tail, t1]
         delta = self.head_buf1.data_ptr() - self.head_buf.data_ptr()
         for op in self.ops:
