@@ -195,6 +195,20 @@ int odt_upsample_bilinear_add(const void* top, const void* a, void* out, int dty
 int odt_upsample_nearest_concat(const void* a, const void* b, void* out, int dtype, int B, int H,
                                 int W, int Ca, int lda, int BH, int BW, int Cb, int ldb, int ldo,
                                 void* stream);
+/* PFPNet-R's pyramid glue (ref PFPNetR.py:321-362,413-421); NHWC, fp32 math, one rounding per TF op.
+ * out[b,2i+py,2j+px,c] = act(in[b,i,j,(2py+px)*C+c] (+ res[b,2i+py,2j+px,c])): the four phases of a 4x4/2 SAME
+ * conv2d_transpose, computed as one 3x3 stride-1 convolution of 4*C phase-major outputs, placed on the 2x grid.
+ * res may be NULL; act is ODT_ACT_*. */
+int odt_pixel_shuffle2x(const void* in, void* out, const void* res, int dtype, int B, int h, int w, int C,
+                        int in_ld, int out_ld, int res_ld, int act, void* stream);
+/* tf.image.resize_bilinear(align_corners=True) of [B,H,W,C] to [B,OH,OW,C]: scale (in-1)/(out-1) in float32 (0 when
+ * out == 1).  out2 (may be NULL): the same values again at channel stride out2_ld (a concat slice). */
+int odt_resize_bilinear_ac(const void* in, void* out, void* out2, int dtype, int B, int H, int W, int C, int in_ld,
+                           int OH, int OW, int out_ld, int out2_ld, void* stream);
+/* 2x2/2 SAME average pool to [B,ceil(H/2),ceil(W/2),C]: the window's cells inside the image, summed in row-major
+ * order, divided by their count (TF's SAME average, not /4). */
+int odt_avgpool2x2_same(const void* in, void* out, int dtype, int B, int H, int W, int C, int in_ld, int out_ld,
+                        void* stream);
 /* GroupNorm(groups) statistics: stats[b][g] = (mean, rstd), eps inside; stats holds B*groups*2 floats.
  * One CTA per (group, image), two passes (mean, then the sum of squared deviations) in a fixed order: the result
  * does not depend on B or on scheduling.  ref: FCOS.py:438-446 */
@@ -222,6 +236,9 @@ int odt_groupnorm_act(const void* in, void* out, void* workspace, int dtype, int
 #define ODT_DECODE_SSD 0    /* SSD300/SSD512/RetinaNet: softmax+argmax+bg filter */
 #define ODT_DECODE_YOLO3 1  /* sigmoid cls * sigmoid obj, additive exp           */
 #define ODT_DECODE_FCOS 2   /* sigmoid cls * sigmoid ctr, exp(l,r,t,b)           */
+#define ODT_DECODE_TWO_STEP 3 /* PFPNet-R: ARM -> ODM two-step softmax decode, rows of
+                               num_fg + 11 floats [odm logits(21), odm t(4), arm logits(2),
+                               arm t(4)]; num_fg must be 20 (ref PFPNetR.py:187-228)  */
 
 typedef struct {
   int H, W, A;  /* feature grid and priors per cell                            */
@@ -239,7 +256,8 @@ typedef struct {
   int num_levels;
   int N;          /* candidates (rows) per image                               */
   int num_fg;     /* classes thresholded (SSD/RetinaNet: 20 of 21; YOLOv3 /
-                     FCOS: 1..128); a candidate row is num_fg + 5 floats       */
+                     FCOS: 1..128); a candidate row is num_fg + 5 floats,
+                     num_fg + 11 for ODT_DECODE_TWO_STEP                       */
   int nms_classes;/* classes the NMS loop visits, 0..num_fg (FCOS: num_fg - 1,
                      ref FCOS.py:252)                                          */
   float score_thr, iou_thr;
@@ -249,10 +267,11 @@ typedef struct {
 } odt_tail_params;
 
 /* fused: score activation + anchor/prior generation + threshold + candidate
- * compaction.  head: fp32 [B,N,num_fg+5] rows (layout per kind, see DESIGN.md).
+ * compaction.  head: fp32 [B,N,row] rows, row = num_fg+5 (num_fg+11 for ODT_DECODE_TWO_STEP; layout per kind,
+ * see DESIGN.md).
  * cand_keys: u64 [B,num_fg,cap]; cand_count: i32 [B,num_fg] (zeroed here).
  * ref: SSD300.py:157-172,323-343; RetinaNet.py:224-239,328-355;
- *      YOLOv3.py:320-351,419-433; FCOS.py:130-150,197-248 */
+ *      YOLOv3.py:320-351,419-433; FCOS.py:130-150,197-248; PFPNetR.py:187-209,447-467 */
 int odt_decode_candidates(const float* head, const odt_tail_params* p, int B,
                           unsigned long long* cand_keys, int* cand_count, void* stream);
 /* per-(image,class) exact TF NonMaxSuppressionV3 + class-major compaction.
@@ -352,6 +371,17 @@ int odt_yolo_loss_grad(const float* head, const odt_tail_params* p, int B, const
 int odt_yolo2_loss_grad(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
                         float coord_scale, float noobj_scale, float obj_scale, float class_scale,
                         void* scratch, float* loss_out, float* grad_out, void* stream);
+/* PFPNet-R's two-step loss (ref PFPNetR.py:469-610) on ODT_DECODE_TWO_STEP rows, 20 classes, G <= 128: per image,
+ * each GT's arg-max anchor plus IoU > 0.5 positives, < 0.4 negatives; ARM cross-entropy (positives to 0, the
+ * min(#neg, 3 #pos) negatives mined by NMS at IoU 0.7 to 1) and smooth-L1 to the anchor targets; ODM cross-entropy
+ * (positives to their class, mined negatives with raw ARM logit 1 < 0.99 to 20) and smooth-L1 to the targets of the
+ * decoded ARM box.  Every mean over zero elements is 0.  loss_out: f32 [B] (image losses); scratch: an 8-byte
+ * aligned buffer of odt_pfpnet_loss_scratch_bytes.  _grad also writes d loss[b] / d rows[b], every element. */
+long long odt_pfpnet_loss_scratch_bytes(const odt_tail_params* p, int B);
+int odt_pfpnet_loss_fwd(const float* head, const odt_tail_params* p, int B, const float* gt, int G, void* scratch,
+                        float* loss_out, void* stream);
+int odt_pfpnet_loss_grad(const float* head, const odt_tail_params* p, int B, const float* gt, int G, void* scratch,
+                         float* loss_out, float* grad_out, void* stream);
 
 /* ------------------------------------------------ training augmentation --- */
 /* image_augmentor's pixel work (utils/image_augmentor.py:7-264, as odt_b200/tfrecord.py's augment_pixels restates

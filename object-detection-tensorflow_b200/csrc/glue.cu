@@ -1030,3 +1030,145 @@ extern "C" int odt_groupnorm_act(const void* in, void* out, void* workspace, int
   if (rc == ODT_ERR_UNSUPPORTED) set_error("odt_groupnorm_act: shape outside the two-launch path (use stats + apply)");
   return rc;
 }
+
+// ---- PFPNet-R pyramid glue (ref PFPNetR.py:321-362,413-421) -----------------
+// One thread per output element: the channel counts are 85 (an odd width, no vector access) or 256, and the three
+// kernels move a few MB per image next to the convolutions around them.
+namespace odt {
+
+// The four output phases of a 4x4 / stride-2 SAME conv2d_transpose, computed by one stride-1 3x3 convolution with
+// 4 * C output channels (phase p = 2 * py + px major, channel minor), placed on the 2x grid:
+// out[b, 2i+py, 2j+px, c] = act(in[b, i, j, p*C + c] (+ res[b, 2i+py, 2j+px, c])).
+template <typename T>
+__global__ void pixel_shuffle2x_kernel(const T* __restrict__ in, T* __restrict__ out, const T* __restrict__ res,
+                                       int B, int h, int w, int C, int in_ld, int out_ld, int res_ld, int act) {
+  pdl_launch_dependents();
+  const int OH = 2 * h, OW = 2 * w;
+  const long long total = (long long)B * OH * OW * C;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C);
+    const long long pix = i / C;
+    const int ox = (int)(pix % OW);
+    const long long t = pix / OW;
+    const int oy = (int)(t % OH);
+    const int b = (int)(t / OH);
+    const int ph = 2 * (oy & 1) + (ox & 1);
+    float v = Elem<T>::ld(in + (((long long)b * h + (oy >> 1)) * w + (ox >> 1)) * in_ld + ph * C + c);
+    if (res) v = __fadd_rn(v, Elem<T>::ld(res + pix * res_ld + c));
+    Elem<T>::st(out + pix * out_ld + c, apply_act(v, act));
+  }
+}
+
+// tf.image.resize_bilinear(align_corners=True), TF 1.13: src = dst * scale, scale = (in - 1) / (out - 1) in float32
+// (0 when out == 1: the only sample is 0 either way), lower = floor, upper = min(ceil, in - 1), lerp = src - lower;
+// top = tl + (tr - tl) * lx, bottom = bl + (br - bl) * lx, out = top + (bottom - top) * ly, each step rounded.
+// out2: an optional second copy (a concat slice) at its own channel stride.
+template <typename T>
+__global__ void resize_bilinear_ac_kernel(const T* __restrict__ in, T* __restrict__ out, T* __restrict__ out2,
+                                          int B, int H, int W, int C, int in_ld, int OH, int OW, int out_ld,
+                                          int out2_ld, float hs, float ws) {
+  pdl_launch_dependents();
+  const long long total = (long long)B * OH * OW * C;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C);
+    const long long pix = i / C;
+    const int ox = (int)(pix % OW);
+    const long long t = pix / OW;
+    const int oy = (int)(t % OH);
+    const int b = (int)(t / OH);
+    const float sy = __fmul_rn((float)oy, hs), sx = __fmul_rn((float)ox, ws);
+    const float fy = floorf(sy), fx = floorf(sx);
+    const int y0 = (int)fy, x0 = (int)fx;
+    const int y1 = min((int)ceilf(sy), H - 1), x1 = min((int)ceilf(sx), W - 1);
+    const float ly = __fsub_rn(sy, fy), lx = __fsub_rn(sx, fx);
+    const T* base = in + (long long)b * H * W * in_ld + c;
+    const float tl = Elem<T>::ld(base + ((long long)y0 * W + x0) * in_ld);
+    const float tr = Elem<T>::ld(base + ((long long)y0 * W + x1) * in_ld);
+    const float bl = Elem<T>::ld(base + ((long long)y1 * W + x0) * in_ld);
+    const float br = Elem<T>::ld(base + ((long long)y1 * W + x1) * in_ld);
+    const float top = __fadd_rn(tl, __fmul_rn(__fsub_rn(tr, tl), lx));
+    const float bot = __fadd_rn(bl, __fmul_rn(__fsub_rn(br, bl), lx));
+    const float v = __fadd_rn(top, __fmul_rn(__fsub_rn(bot, top), ly));
+    Elem<T>::st(out + pix * out_ld + c, v);
+    if (out2) Elem<T>::st(out2 + pix * out2_ld + c, v);
+  }
+}
+
+// tf.layers.average_pooling2d(2, 2, 'same'): out = ceil(in / 2), padding only after (odd sizes), and the sum of the
+// window cells inside the image -- added in row-major order -- divided by their number, not by 4.
+template <typename T>
+__global__ void avgpool2x2_same_kernel(const T* __restrict__ in, T* __restrict__ out, int B, int H, int W, int C,
+                                       int in_ld, int out_ld) {
+  pdl_launch_dependents();
+  const int OH = (H + 1) / 2, OW = (W + 1) / 2;
+  const long long total = (long long)B * OH * OW * C;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C);
+    const long long pix = i / C;
+    const int ox = (int)(pix % OW);
+    const long long t = pix / OW;
+    const int oy = (int)(t % OH);
+    const int b = (int)(t / OH);
+    const T* base = in + (long long)b * H * W * in_ld + c;
+    float s = 0.f;
+    int n = 0;
+    for (int dy = 0; dy < 2; ++dy) {
+      const int y = 2 * oy + dy;
+      if (y >= H) break;
+      for (int dx = 0; dx < 2; ++dx) {
+        const int x = 2 * ox + dx;
+        if (x >= W) break;
+        s = __fadd_rn(s, Elem<T>::ld(base + ((long long)y * W + x) * in_ld));
+        ++n;
+      }
+    }
+    Elem<T>::st(out + pix * out_ld + c, __fdiv_rn(s, (float)n));
+  }
+}
+
+}  // namespace odt
+
+extern "C" int odt_pixel_shuffle2x(const void* in, void* out, const void* res, int dtype, int B, int h, int w, int C,
+                                   int in_ld, int out_ld, int res_ld, int act, void* stream) {
+  ODT_CHECK_ARG(in && out && B > 0 && h > 0 && w > 0 && C > 0 && in_ld >= 4 * C && out_ld >= C &&
+                    (!res || res_ld >= C) && act >= ODT_ACT_NONE && act <= ODT_ACT_LEAKY,
+                "args");
+  cudaStream_t st = (cudaStream_t)stream;
+  DISPATCH_DTYPE(dtype, {
+    pixel_shuffle2x_kernel<T><<<grid_for((long long)B * 4 * h * w * C, 256), 256, 0, st>>>(
+        (const T*)in, (T*)out, (const T*)res, B, h, w, C, in_ld, out_ld, res_ld, act);
+  })
+  ODT_LAUNCH_OK();
+  return ODT_OK;
+}
+
+extern "C" int odt_resize_bilinear_ac(const void* in, void* out, void* out2, int dtype, int B, int H, int W, int C,
+                                      int in_ld, int OH, int OW, int out_ld, int out2_ld, void* stream) {
+  ODT_CHECK_ARG(in && out && B > 0 && H > 0 && W > 0 && C > 0 && OH > 0 && OW > 0 && in_ld >= C && out_ld >= C &&
+                    (!out2 || out2_ld >= C),
+                "args");
+  cudaStream_t st = (cudaStream_t)stream;
+  const float hs = OH > 1 ? (float)(H - 1) / (float)(OH - 1) : 0.f;
+  const float ws = OW > 1 ? (float)(W - 1) / (float)(OW - 1) : 0.f;
+  DISPATCH_DTYPE(dtype, {
+    resize_bilinear_ac_kernel<T><<<grid_for((long long)B * OH * OW * C, 256), 256, 0, st>>>(
+        (const T*)in, (T*)out, (T*)out2, B, H, W, C, in_ld, OH, OW, out_ld, out2_ld, hs, ws);
+  })
+  ODT_LAUNCH_OK();
+  return ODT_OK;
+}
+
+extern "C" int odt_avgpool2x2_same(const void* in, void* out, int dtype, int B, int H, int W, int C, int in_ld,
+                                   int out_ld, void* stream) {
+  ODT_CHECK_ARG(in && out && B > 0 && H > 0 && W > 0 && C > 0 && in_ld >= C && out_ld >= C, "args");
+  cudaStream_t st = (cudaStream_t)stream;
+  DISPATCH_DTYPE(dtype, {
+    avgpool2x2_same_kernel<T><<<grid_for((long long)B * ((H + 1) / 2) * ((W + 1) / 2) * C, 256), 256, 0, st>>>(
+        (const T*)in, (T*)out, B, H, W, C, in_ld, out_ld);
+  })
+  ODT_LAUNCH_OK();
+  return ODT_OK;
+}

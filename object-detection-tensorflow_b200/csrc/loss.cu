@@ -1414,3 +1414,288 @@ extern "C" int odt_yolo2_loss_grad(const float* head, const odt_tail_params* p, 
   return yolo_forward_grad<Yolo2Loss>(head, p, B, gt, G, coord_scale, noobj_scale, obj_scale, class_scale, scratch,
                                       loss_out, grad_out, (cudaStream_t)stream);
 }
+
+// ============================ PFPNet-R loss =================================
+// Restates _compute_one_image_loss of PFPNetR.py:469-610 (never copied) on the two-step rows
+// [ODM logits(21), ODM t(4), ARM logits(2), ARM t(4)]:
+//   * matching: each GT's arg-max anchor (loss_best_anchor_kernel, first maximum, duplicates kept); among the other
+//     anchors best IoU > 0.5 is a positive of its arg-max GT, < 0.4 a negative (RetinaNet's band);
+//   * ARM: positives cross-entropy to label 0 and smooth-L1 against the anchor targets; hard negatives: exact greedy
+//     NMS over the negative anchor boxes scored by their ARM cross-entropy to label 1, min(#neg, 3 #pos) of them at
+//     IoU 0.7 (the SSD mining), their mean;
+//   * ODM: the mined negatives whose RAW ARM logit of class 1 is < 0.99 (:584), cross-entropy to label 20; positives
+//     cross-entropy to their GT class and smooth-L1 against targets built from the decoded ARM box (:598-605), so
+//     the ODM box term also depends on the ARM deltas, and its gradient reaches them.
+//   * every mean over zero elements is 0: tf.losses' Reduction.MEAN divides with div_no_nan (_safe_mean, TF 1.13)
+//     [TF-sem], and the kernel applies the same rule where the reference's tf.reduce_mean would give NaN (no mined
+//     negative, no positive): an image without boxes has loss 0 and gradient 0.
+// One CTA per image; sums in a fixed order (per-thread anchor order, then block_sum), so the loss is run-to-run
+// deterministic.  The gradient kernel writes d(image loss)/d(row) for every column of every row.
+namespace odt {
+
+constexpr int kPfpOdmT = 21, kPfpArmC = 25, kPfpArmT = 27;
+
+__device__ __forceinline__ float xent2(float a0, float a1, int label) {
+  const float m = fmaxf(a0, a1);
+  const float s = __fadd_rn(expf(__fsub_rn(a0, m)), expf(__fsub_rn(a1, m)));
+  return __fsub_rn(logf(s), __fsub_rn(label ? a1 : a0, m));
+}
+
+template <bool kGrad>
+__global__ void __launch_bounds__(kLossThreads)
+    pfpnet_loss_kernel(const float* __restrict__ head, const __grid_constant__ TailP tp, const float* __restrict__ gt,
+                       int G, const int* __restrict__ best, unsigned long long* __restrict__ neg_keys,
+                       int* __restrict__ assign_all, float* __restrict__ loss_out, float* __restrict__ grad) {
+  pdl_launch_dependents();
+  const odt_tail_params& p = tp.p;
+  constexpr int row = kind_row_floats(ODT_DECODE_TWO_STEP, 20);
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int N = p.N;
+  const float* hb = head + (long long)b * N * row;
+  const float* gb = gt + (long long)b * G * 5;
+  unsigned long long* keys = neg_keys + (long long)b * N;
+  int* assign = assign_all + (long long)b * N;
+  __shared__ int s_best[kMaxGT];
+  __shared__ int s_npos, s_nneg, s_nsel, s_nodm;
+  __shared__ unsigned long long s_wkey[kLossThreads / 32];
+  __shared__ int s_wpos[kLossThreads / 32];
+  __shared__ float s_sum[6][kLossThreads];
+  const int cnt = block_gt_count(gb, G);
+  for (int g = tid; g < cnt; g += blockDim.x) s_best[g] = best[b * G + g];
+  if (tid == 0) {
+    s_npos = 0;
+    s_nneg = 0;
+  }
+  __syncthreads();
+  // (1) assignment of every anchor; negatives become (ARM cross-entropy, row) mining keys
+  for (int n = tid; n < N; n += blockDim.x) {
+    bool is_best = false;
+    for (int g = 0; g < cnt; ++g) is_best |= s_best[g] == n;
+    int as = kAsBest;
+    if (!is_best) {
+      const Anchor a = anchor_ssd(p, locate(p, n));
+      float bv = -INFINITY;  // reduce_max over no GT: every anchor is a negative
+      int bg = 0;
+      for (int g = 0; g < cnt; ++g) {
+        const GtBox gx = gt_box(gb, g);
+        const float v = iou_match(a, gx.y1, gx.x1, gx.y2, gx.x2, gx.area);
+        if (v > bv) {
+          bv = v;
+          bg = g;
+        }
+      }
+      if (bv > 0.5f) {
+        as = bg;
+        atomicAdd(&s_npos, 1);
+      } else if (bv < 0.4f) {
+        as = kAsNegative;
+        const float* r = hb + (long long)n * row;
+        const float ce = xent2(r[kPfpArmC], r[kPfpArmC + 1], 1);
+        keys[atomicAdd(&s_nneg, 1)] = ((unsigned long long)__float_as_uint(ce) << 32) | (0xFFFFFFFFu - (unsigned)n);
+      } else {
+        as = kAsIgnored;
+      }
+    }
+    assign[n] = as;
+  }
+  __syncthreads();
+  // (2) hard-negative mining, as ssd_loss_mine_kernel: greedy NMS by repeated arg-max of the keys
+  const int P = cnt + s_npos, nneg = s_nneg;
+  const int chosen = nneg > 3 * P ? 3 * P : nneg;
+  int nsel = 0, nodm = 0;  // thread 0's count of mined rows that pass the ODM test
+  while (nsel < chosen) {
+    unsigned long long bk = 0ull;
+    int bp = 0x7fffffff;
+    for (int i = tid; i < nneg; i += blockDim.x) {
+      const unsigned long long k = keys[i];
+      if (k > bk) {
+        bk = k;
+        bp = i;
+      }
+    }
+    {
+      const unsigned hi = (unsigned)(bk >> 32), lo = (unsigned)bk;
+      const unsigned whi = __reduce_max_sync(0xffffffffu, hi);
+      const unsigned wlo = __reduce_max_sync(0xffffffffu, hi == whi ? lo : 0u);
+      const int wpos = __reduce_min_sync(0xffffffffu, (hi == whi && lo == wlo) ? bp : 0x7fffffff);
+      if (lane == 0) {
+        s_wkey[warp] = ((unsigned long long)whi << 32) | wlo;
+        s_wpos[warp] = wpos;
+      }
+    }
+    __syncthreads();
+    unsigned long long hk = 0ull;
+    int hp = -1;
+#pragma unroll
+    for (int w = 0; w < kLossThreads / 32; ++w) {
+      if (s_wkey[w] > hk) {
+        hk = s_wkey[w];
+        hp = s_wpos[w];
+      }
+    }
+    if (hk == 0ull) break;
+    const int hn = (int)(0xFFFFFFFFu - (unsigned)(hk & 0xFFFFFFFFull));
+    const float4 cur = neg_anchor_box(p, hn);
+    ++nsel;
+    if (tid == 0) {
+      assign[hn] = kAsMined;
+      nodm += hb[(long long)hn * row + kPfpArmC + 1] < 0.99f;  // the raw logit, as the reference (:584)
+    }
+    for (int j = tid; j < nneg; j += blockDim.x) {
+      const unsigned long long kj = keys[j];
+      if (kj == 0ull) continue;
+      if (j == hp) {
+        keys[j] = 0ull;
+        continue;
+      }
+      const int n = (int)(0xFFFFFFFFu - (unsigned)(kj & 0xFFFFFFFFull));
+      if (iou_tf(neg_anchor_box(p, n), cur) > 0.7f) keys[j] = 0ull;
+    }
+    __syncthreads();
+  }
+  if (tid == 0) {
+    s_nsel = nsel;
+    s_nodm = nodm;
+  }
+  __syncthreads();
+  const int S = s_nsel, M = s_nodm;
+  const float invP = P ? __fdiv_rn(1.f, (float)P) : 0.f;
+  const float invS = S ? __fdiv_rn(1.f, (float)S) : 0.f;
+  const float invM = M ? __fdiv_rn(1.f, (float)M) : 0.f;
+  // (3) the terms: v = (ARM pos CE, ARM coord, ODM pos CE, ODM coord, ARM mined CE, ODM mined CE), and the gradient
+  float v[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  for (int n = tid; n < N; n += blockDim.x) {
+    const int as = assign[n];
+    const float* r = hb + (long long)n * row;
+    float gr[row];
+#pragma unroll
+    for (int k = 0; k < row; ++k) gr[k] = 0.f;
+    const bool pos = as >= 0 || as == kAsBest;
+    if (pos) {
+      const Anchor a = anchor_ssd(p, locate(p, n));
+      for (int e = 0; e < (as == kAsBest ? cnt : 1); ++e) {  // a best anchor: once per GT it is the best of
+        const int g = as == kAsBest ? e : as;
+        if (as == kAsBest && s_best[g] != n) continue;
+        const float gy = gb[g * 5], gx = gb[g * 5 + 1], gh = gb[g * 5 + 2], gw = gb[g * 5 + 3];
+        const int label = (int)gb[g * 5 + 4];
+        v[0] += xent2(r[kPfpArmC], r[kPfpArmC + 1], 0);
+        v[1] += coord_loss(r + (kPfpArmT - kPfpOdmT), a, gy, gx, gh, gw);
+        v[2] += xent21(r, label);
+        // the ARM box (:598-599), then the ODM targets relative to it (:602-603)
+        const float ay = __fadd_rn(__fmul_rn(r[kPfpArmT], a.h), a.cy);
+        const float ax = __fadd_rn(__fmul_rn(r[kPfpArmT + 1], a.w), a.cx);
+        const float ah = __fmul_rn(expf(r[kPfpArmT + 2]), a.h);
+        const float aw = __fmul_rn(expf(r[kPfpArmT + 3]), a.w);
+        const float oy = __fdiv_rn(__fsub_rn(gy, ay), ah), ox = __fdiv_rn(__fsub_rn(gx, ax), aw);
+        const float oh = logf(__fdiv_rn(gh, ah)), ow = logf(__fdiv_rn(gw, aw));
+        const float e0 = __fsub_rn(r[kPfpOdmT], oy), e1 = __fsub_rn(r[kPfpOdmT + 1], ox);
+        const float e2 = __fsub_rn(r[kPfpOdmT + 2], oh), e3 = __fsub_rn(r[kPfpOdmT + 3], ow);
+        v[3] += __fadd_rn(__fadd_rn(smooth_l1(e0), smooth_l1(e1)), __fadd_rn(smooth_l1(e2), smooth_l1(e3)));
+        if constexpr (kGrad) {
+          const float m = fmaxf(r[kPfpArmC], r[kPfpArmC + 1]);
+          const float x0 = expf(r[kPfpArmC] - m), x1 = expf(r[kPfpArmC + 1] - m), inv = 1.f / (x0 + x1);
+          gr[kPfpArmC] += (x0 * inv - 1.f) * invP;
+          gr[kPfpArmC + 1] += x1 * inv * invP;
+          float prob[21];
+          softmax21(r, prob);
+#pragma unroll
+          for (int k = 0; k < 21; ++k) gr[k] += (prob[k] - (k == label ? 1.f : 0.f)) * invP;
+          const float ty = (gy - a.cy) / a.h, tx = (gx - a.cx) / a.w;
+          const float th = logf(gh / a.h), tw = logf(gw / a.w);
+          gr[kPfpArmT] += smooth_l1_grad(r[kPfpArmT] - ty) * invP;
+          gr[kPfpArmT + 1] += smooth_l1_grad(r[kPfpArmT + 1] - tx) * invP;
+          gr[kPfpArmT + 2] += smooth_l1_grad(r[kPfpArmT + 2] - th) * invP;
+          gr[kPfpArmT + 3] += smooth_l1_grad(r[kPfpArmT + 3] - tw) * invP;
+          const float d0 = smooth_l1_grad(e0), d1 = smooth_l1_grad(e1);
+          const float d2 = smooth_l1_grad(e2), d3 = smooth_l1_grad(e3);
+          gr[kPfpOdmT] += d0 * invP;
+          gr[kPfpOdmT + 1] += d1 * invP;
+          gr[kPfpOdmT + 2] += d2 * invP;
+          gr[kPfpOdmT + 3] += d3 * invP;
+          // through the ODM targets: d oy / d t_y = -a.h / ah, d oy / d t_h = -oy, d oh / d t_h = -1
+          gr[kPfpArmT] += d0 * (a.h / ah) * invP;
+          gr[kPfpArmT + 1] += d1 * (a.w / aw) * invP;
+          gr[kPfpArmT + 2] += (d0 * oy + d2) * invP;
+          gr[kPfpArmT + 3] += (d1 * ox + d3) * invP;
+        }
+      }
+    } else if (as == kAsMined) {
+      v[4] += xent2(r[kPfpArmC], r[kPfpArmC + 1], 1);
+      const bool odm = r[kPfpArmC + 1] < 0.99f;
+      if (odm) v[5] += xent21(r, 20);
+      if constexpr (kGrad) {
+        const float m = fmaxf(r[kPfpArmC], r[kPfpArmC + 1]);
+        const float x0 = expf(r[kPfpArmC] - m), x1 = expf(r[kPfpArmC + 1] - m), inv = 1.f / (x0 + x1);
+        gr[kPfpArmC] = x0 * inv * invS;
+        gr[kPfpArmC + 1] = (x1 * inv - 1.f) * invS;
+        if (odm) {
+          float prob[21];
+          softmax21(r, prob);
+#pragma unroll
+          for (int k = 0; k < 21; ++k) gr[k] = (prob[k] - (k == 20 ? 1.f : 0.f)) * invM;
+        }
+      }
+    }
+    if constexpr (kGrad) {
+      float* go = grad + ((long long)b * N + n) * row;
+#pragma unroll
+      for (int k = 0; k < row; ++k) go[k] = gr[k];
+    }
+  }
+  block_sum<6, kLossThreads>(s_sum, v);
+  if (tid == 0) {
+    const float arm = __fadd_rn(__fadd_rn(__fmul_rn(s_sum[4][0], invS), __fmul_rn(s_sum[0][0], invP)),
+                                __fmul_rn(s_sum[1][0], invP));
+    const float odm = __fadd_rn(__fadd_rn(__fmul_rn(s_sum[5][0], invM), __fmul_rn(s_sum[2][0], invP)),
+                                __fmul_rn(s_sum[3][0], invP));
+    loss_out[b] = __fadd_rn(arm, odm);
+  }
+}
+
+}  // namespace odt
+
+// scratch: mining keys u64 [B, N], assignment i32 [B, N], per-GT best anchors i32 [B, 128]
+extern "C" long long odt_pfpnet_loss_scratch_bytes(const odt_tail_params* p, int B) {
+  if (!p || B <= 0 || p->N <= 0) return -1;
+  return (long long)B * p->N * 8 + (long long)B * p->N * 4 + (long long)B * kMaxGT * 4;
+}
+
+static int pfpnet_loss(const float* head, const odt_tail_params* p, int B, const float* gt, int G, void* scratch,
+                       float* loss_out, float* grad_out, bool with_grad, cudaStream_t st) {
+  ODT_CHECK_ARG(head && p && gt && scratch && loss_out, "null pointer");
+  ODT_CHECK_ARG(!with_grad || grad_out, "null pointer (gradient)");
+  ODT_CHECK_ARG(p->kind == ODT_DECODE_TWO_STEP && p->num_fg == 20, "two-step head with 20 classes expected");
+  ODT_CHECK_ARG(p->num_levels >= 1 && p->num_levels <= ODT_MAX_LEVELS, "two-step head with 20 classes expected");
+  long long rows = 0;
+  for (int i = 0; i < p->num_levels; ++i) {
+    const odt_level& L = p->level[i];
+    ODT_CHECK_ARG(L.A >= 1 && L.A <= ODT_MAX_PRIORS && L.H > 0 && L.W > 0 && L.offset == rows, "level geometry");
+    rows += (long long)L.H * L.W * L.A;
+  }
+  ODT_CHECK_ARG(rows == p->N, "level geometry");
+  ODT_CHECK_ARG(B > 0 && G > 0 && G <= kMaxGT, "B/G (G <= 128)");
+  ODT_CHECK_ARG(((uintptr_t)scratch & 7) == 0, "scratch must be 8-byte aligned");
+  unsigned long long* keys = reinterpret_cast<unsigned long long*>(scratch);
+  int* assign = reinterpret_cast<int*>(keys + (long long)B * p->N);
+  int* best = assign + (long long)B * p->N;
+  TailP tp;
+  tp.p = *p;
+  loss_best_anchor_kernel<<<dim3(G, B), kLossThreads, 0, st>>>(tp, gt, G, best);
+  ODT_LAUNCH_OK();
+  if (with_grad)
+    pfpnet_loss_kernel<true><<<B, kLossThreads, 0, st>>>(head, tp, gt, G, best, keys, assign, loss_out, grad_out);
+  else
+    pfpnet_loss_kernel<false><<<B, kLossThreads, 0, st>>>(head, tp, gt, G, best, keys, assign, loss_out, nullptr);
+  ODT_LAUNCH_OK();
+  return ODT_OK;
+}
+
+extern "C" int odt_pfpnet_loss_fwd(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
+                                   void* scratch, float* loss_out, void* stream) {
+  return pfpnet_loss(head, p, B, gt, G, scratch, loss_out, nullptr, false, (cudaStream_t)stream);
+}
+
+extern "C" int odt_pfpnet_loss_grad(const float* head, const odt_tail_params* p, int B, const float* gt, int G,
+                                    void* scratch, float* loss_out, float* grad_out, void* stream) {
+  return pfpnet_loss(head, p, B, gt, G, scratch, loss_out, grad_out, true, (cudaStream_t)stream);
+}

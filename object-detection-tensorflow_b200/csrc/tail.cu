@@ -45,12 +45,13 @@ __global__ void __launch_bounds__(WARPS * 32, OCC)
     decode_candidates_kernel(const float* __restrict__ head, const __grid_constant__ TailP tp,
                              long long total_rows, unsigned long long* __restrict__ cand_keys,
                              int* __restrict__ cand_count) {
-  static_assert(NFG == 0 ? KIND != ODT_DECODE_SSD : NFG == 20, "instantiations: NFG = 20, or 0 for YOLOv3 / FCOS");
+  static_assert(NFG == 0 ? (KIND != ODT_DECODE_SSD && KIND != ODT_DECODE_TWO_STEP) : NFG == 20,
+                "instantiations: NFG = 20, or 0 for YOLOv3 / FCOS");
   constexpr int W = NFG ? (NFG + 31) / 32 : kMaskWords;  // pass-mask words per row
   pdl_launch_dependents();
   const odt_tail_params& p = tp.p;
   const int nfg = NFG ? NFG : p.num_fg;
-  const int row = row_floats(nfg);
+  const int row = kind_row_floats(KIND, nfg);
   const int group_floats = 32 * row;
   const uint32_t group_bytes = (uint32_t)group_floats * 4u;
   extern __shared__ __align__(128) unsigned char dsm_raw[];
@@ -118,7 +119,7 @@ __global__ void __launch_bounds__(WARPS * 32, OCC)
 #pragma unroll
     for (int w = 0; w < W; ++w) pass[w] = 0u;
     float k0 = 0.f, k1 = 0.f;  // SSD: (max logit, 1/sum); YOLO / FCOS: (sigmoid(obj | ctr), unused)
-    if (KIND == ODT_DECODE_SSD) {
+    if (KIND == ODT_DECODE_SSD || KIND == ODT_DECODE_TWO_STEP) {
       // softmax over 21 logits, TF form exp(x-max) * (1/sum); rows whose arg-max (first maximum) is the
       // background (last index) are dropped: background wins only if strictly greater than every foreground
       // probability.  ref SSD300.py:159-164
@@ -144,6 +145,13 @@ __global__ void __launch_bounds__(WARPS * 32, OCC)
         bits |= (pi >= p.score_thr) ? (1u << i) : 0u;
       }
       if (!active || __fmul_rn(e[20], inv) > best_fg) bits = 0u;
+      if (KIND == ODT_DECODE_TWO_STEP) {
+        // ARM's softmax background (second) probability must stay below 0.99: ref PFPNetR.py:188-192
+        const float a0 = r[25], a1 = r[26];
+        const float am = fmaxf(a0, a1);
+        const float x0 = exp_score(__fsub_rn(a0, am)), x1 = exp_score(__fsub_rn(a1, am));
+        if (!(__fmul_rn(x1, __frcp_rn(__fadd_rn(x0, x1))) < 0.99f)) bits = 0u;
+      }
       pass[0] = bits;
       k0 = m;
       k1 = inv;
@@ -165,7 +173,7 @@ __global__ void __launch_bounds__(WARPS * 32, OCC)
       }
     }
     auto score = [&](int c) -> float {
-      if (KIND == ODT_DECODE_SSD) return __fmul_rn(exp_score(__fsub_rn(r[c], k0)), k1);
+      if (KIND == ODT_DECODE_SSD || KIND == ODT_DECODE_TWO_STEP) return __fmul_rn(exp_score(__fsub_rn(r[c], k0)), k1);
       return __fmul_rn(sigmoid_score(r[c]), k0);
     };
 #pragma unroll
@@ -377,7 +385,7 @@ __global__ void __launch_bounds__(kNmsThreads)
     cnt = p.cap;
   }
   unsigned long long* gkeys = cand_keys + ((long long)b * p.num_fg + c) * p.cap;
-  const int row = row_floats(p.num_fg);
+  const int row = kind_row_floats(p.kind, p.num_fg);
   const float* hb = head + (long long)b * p.N * row;
   const int cnt_all = cnt;
   int nsel = 0;
@@ -619,10 +627,11 @@ using namespace odt;
 
 static int check_tail(const odt_tail_params* p) {
   ODT_CHECK_ARG(p != nullptr, "params null");
-  ODT_CHECK_ARG(p->kind >= 0 && p->kind <= 2, "kind");
+  ODT_CHECK_ARG(p->kind >= 0 && p->kind <= ODT_DECODE_TWO_STEP, "kind");
   ODT_CHECK_ARG(p->num_levels >= 1 && p->num_levels <= ODT_MAX_LEVELS, "num_levels");
   // the softmax family (SSD / RetinaNet) decodes 21 logits; YOLOv3 / FCOS rows carry 1..kMaxFg class scores
-  if (p->kind == ODT_DECODE_SSD) ODT_CHECK_ARG(p->num_fg == 20, "num_fg must be 20 for the softmax family");
+  if (p->kind == ODT_DECODE_SSD || p->kind == ODT_DECODE_TWO_STEP)
+    ODT_CHECK_ARG(p->num_fg == 20, "num_fg must be 20 for the softmax family");
   else ODT_CHECK_ARG(p->num_fg >= 1 && p->num_fg <= kMaxFg, "num_fg must be 1..128");
   // 0 NMS classes: FCOS with one class visits range(num_classes - 1) = no class (ref FCOS.py:252)
   ODT_CHECK_ARG(p->nms_classes >= 0 && p->nms_classes <= p->num_fg, "nms_classes");
@@ -683,7 +692,7 @@ extern "C" int odt_decode_candidates(const float* head, const odt_tail_params* p
       attr_done = true;                                                                                          \
     }                                                                                                            \
     decode_candidates_kernel<KIND_, WARPS_, OCC_, ST_, NFG_>                                                     \
-        <<<blocks, (WARPS_) * 32, decode_smem_bytes(WARPS_, ST_, row_floats(p->num_fg)), st>>>(                  \
+        <<<blocks, (WARPS_) * 32, decode_smem_bytes(WARPS_, ST_, kind_row_floats(p->kind, p->num_fg)), st>>>(     \
             head, tp, rows, cand_keys, cand_count);                                                              \
   } while (0)
 #define ODT_DECODE_LAUNCH20(KIND_) \
@@ -692,6 +701,9 @@ extern "C" int odt_decode_candidates(const float* head, const odt_tail_params* p
   ODT_DECODE_LAUNCH(KIND_, kDecodeWarpsWide, 1, 2, 0, decode_smem_bytes(kDecodeWarpsWide, 2, row_floats(kMaxFg)))
   if (p->kind == ODT_DECODE_SSD) {
     ODT_DECODE_LAUNCH20(ODT_DECODE_SSD);
+  } else if (p->kind == ODT_DECODE_TWO_STEP) {
+    ODT_DECODE_LAUNCH(ODT_DECODE_TWO_STEP, kDecodeWarps, 3, 2, 20,
+                      decode_smem_bytes(kDecodeWarps, 2, kind_row_floats(ODT_DECODE_TWO_STEP, 20)));
   } else if (p->kind == ODT_DECODE_YOLO3) {
     if (wide) ODT_DECODE_LAUNCH_WIDE(ODT_DECODE_YOLO3); else ODT_DECODE_LAUNCH20(ODT_DECODE_YOLO3);
   } else {

@@ -10,6 +10,13 @@ namespace odt {
 // stride and column offset of the tail and the loss kernels goes through this function.
 __host__ __device__ __forceinline__ constexpr int row_floats(int num_fg) { return num_fg + 5; }
 
+// Floats per candidate row of a tail of decode kind `kind`: PFPNet-R's two-step rows carry both stages,
+// [ODM logits (num_fg + 1), ODM ty tx th tw, ARM logits (2), ARM ty tx th tw] = num_fg + 11; every other kind
+// row_floats(num_fg).
+__host__ __device__ __forceinline__ constexpr int kind_row_floats(int kind, int num_fg) {
+  return kind == ODT_DECODE_TWO_STEP ? num_fg + 11 : row_floats(num_fg);
+}
+
 // Largest num_fg of the sigmoid families (YOLOv3 / FCOS): the decode kernel stages 32 rows of row_floats(128) = 133
 // floats (17 KB) per warp and stage, and keeps one pass mask of kMaxFg / 32 = 4 words per row in registers.
 constexpr int kMaxFg = 128;
@@ -89,7 +96,7 @@ __device__ __forceinline__ Anchor anchor_ssd(const odt_tail_params& p, const Cel
   return a;
 }
 
-// Box (y1,x1,y2,x2) of candidate row `row` (row_floats(p.num_fg) floats) at cell c.
+// Box (y1,x1,y2,x2) of candidate row `row` (kind_row_floats(p.kind, p.num_fg) floats) at cell c.
 __device__ __forceinline__ float4 decode_box(const odt_tail_params& p, const Cell& c,
                                              const float* __restrict__ row) {
   const odt_level& L = p.level[c.lvl];
@@ -105,6 +112,23 @@ __device__ __forceinline__ float4 decode_box(const odt_tail_params& p, const Cel
     float dh = __fmul_rn(ah, expf(th));
     float dw = __fmul_rn(aw, expf(tw));
     float h2 = __fmul_rn(dh, 0.5f), w2 = __fmul_rn(dw, 0.5f);
+    o.x = __fsub_rn(dy, h2);
+    o.y = __fsub_rn(dx, w2);
+    o.z = __fadd_rn(dy, h2);
+    o.w = __fadd_rn(dx, w2);
+  } else if (p.kind == ODT_DECODE_TWO_STEP) {
+    // ref PFPNetR.py:447-467 (anchors), :202-209 (two steps): the ARM deltas refine the anchor, the ODM deltas that
+    // refined box.  r[0]: ODM background logit, r[1..4]: ODM t, r[5..6]: ARM logits, r[7..10]: ARM t
+    const Anchor an = anchor_ssd(p, c);
+    const float ay = __fadd_rn(__fmul_rn(r[7], an.h), an.cy);
+    const float ax = __fadd_rn(__fmul_rn(r[8], an.w), an.cx);
+    const float ah = __fmul_rn(expf(r[9]), an.h);
+    const float aw = __fmul_rn(expf(r[10]), an.w);
+    const float dy = __fadd_rn(__fmul_rn(r[1], ah), ay);
+    const float dx = __fadd_rn(__fmul_rn(r[2], aw), ax);
+    const float dh = __fmul_rn(expf(r[3]), ah);
+    const float dw = __fmul_rn(expf(r[4]), aw);
+    const float h2 = __fmul_rn(dh, 0.5f), w2 = __fmul_rn(dw, 0.5f);
     o.x = __fsub_rn(dy, h2);
     o.y = __fsub_rn(dx, w2);
     o.z = __fadd_rn(dy, h2);

@@ -5,6 +5,7 @@ asserts and method names as the reference model scripts, so its test*.py
 drivers run unchanged (SURVEY.md section 8b):
     SSD300.py:11-50,473-504   SSD512.py   RetinaNet.py:11-79,505-539
     YOLOv3.py:11-60,444-483   YOLOv2.py:11-54,305-343   FCOS.py:11-49,401-436
+    PFPNetR.py:11-53,615-661
 Inference (`test_one_image`) runs entirely on the hand-written GPU kernels; there is no CPU
 fallback.  `train_one_epoch` runs the training step of odt_b200/train.py (PyTorch autograd over the
 engine's layer list + the reference's losses + Momentum: the first stage of SURVEY 8f row 2; RetinaNet's
@@ -705,3 +706,25 @@ class FCOS(_Detector):
     def _build(self, batch, precision, allow_tc=True):
         return nets.build_fcos(batch, self.config, precision, self.device, allow_tc,
                                share_heads=self.config.get("share_heads", True))
+
+
+class PFPNetR(_Detector):
+    """PFPNet-R (ref PFPNetR.py): VGG-16 to conv4_3, a parallel pyramid of bilinear resizes, transposed convolutions
+    and average pools, ARM / TCB / ODM heads and the two-step decode."""
+    name = "PFPNetR"
+    # matching in the 0.5 / 0.4 band, ARM cross-entropy with NMS hard-negative mining, ODM negatives on the raw ARM
+    # logit, smooth-L1 against the anchor (ARM) and the decoded ARM box (ODM): ref PFPNetR.py:469-610
+    loss_kind = "pfpnet"
+
+    def __init__(self, config, data_provider):
+        nets.check_pfpnet_config(config)
+        self._common_init(config, data_provider)
+        self.input_size = config["input_size"]
+        self.num_classes = config["num_classes"] + 1
+        s = self.input_size
+        self.data_shape = [s, s, 3] if config["data_format"] == "channels_last" else [3, s, s]
+        self.anchor_ratios = list(nets.PFPNET_RATIOS)
+        self.num_anchors = len(self.anchor_ratios)
+
+    def _build(self, batch, precision, allow_tc=True):
+        return nets.build_pfpnet(batch, self.config, precision, self.device, allow_tc)

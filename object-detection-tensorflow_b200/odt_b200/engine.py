@@ -83,6 +83,11 @@ class Act:
         self.halo = 0       # 1: stored as [B, H+2, W+2, ld] with a zero border (halo-flat 3x3 convs)
         self.base, self.c0 = None, 0  # a channel slice [c0, c0 + C) of the tensor `base` (Net.concat)
         self.parts = ()               # Net.concat: the slices that make up this tensor
+        self.chan_map = None          # Net.padded_concat: stored channel of every real channel (None: the identity)
+
+    @property
+    def real_channels(self):
+        return self.C if self.chan_map is None else len(self.chan_map)
 
     @property
     def img_stride(self):
@@ -130,10 +135,27 @@ class ConvOp(Op):
         """Channels of each output pixel this layer may store into an extra output (slice_store_width)."""
         return slice_store_width(self.y.C, self.on_tensor_cores(net))
 
+    def host_weights(self, net):
+        """HWIO kernel and bias of the convolution the kernels run.  The filter rows of an input stored with gaps
+        between its parts (Net.padded_concat) are scattered to the stored channels, zero at the gaps."""
+        kern = np.asarray(net.weights[self.kernel], dtype=np.float32)
+        bias = (np.asarray(net.weights[self.bias], dtype=np.float32) if self.bias
+                else np.zeros(kern.shape[3], np.float32))
+        x = self.x
+        if x is not None and x.chan_map is not None:
+            full = np.zeros(kern.shape[:2] + (x.C, kern.shape[3]), np.float32)
+            full[:, :, x.chan_map, :] = kern
+            kern = full
+        return kern, bias
+
+    def host_bn(self, net):
+        """(scale, shift) of the folded inference BN, per output channel of the convolution the kernels run."""
+        return net.bn_fold(self.bn)
+
     def prepare(self, net):
-        x, W = self.x, net.weights
+        x = self.x
         dev = net.device
-        kern = np.asarray(W[self.kernel], dtype=np.float32)  # HWIO
+        kern, bias = self.host_weights(net)  # HWIO
         R, S, cin, cout = kern.shape
         assert cin == (3 if self.is_image else x.C), (self.kernel, cin, x.C)
         self.cout = cout
@@ -150,9 +172,8 @@ class ConvOp(Op):
             wp = np.ascontiguousarray(ohwi)
             self.w_ld, self.cout_pad = cin, cout
         self.wdev = torch.from_numpy(wp).to(dev).to(adt).contiguous()
-        bias = np.asarray(W[self.bias], dtype=np.float32) if self.bias else np.zeros(cout, np.float32)
         if self.bn:
-            sc, sh = net.bn_fold(self.bn)
+            sc, sh = self.host_bn(net)
             shift = sh + bias * sc
             scale = sc
         else:
@@ -320,7 +341,7 @@ class PoolOp(Op):
 class L2NormOp(Op):
     def __init__(self, x, y, var):
         self.x, self.y, self.var = x, y, var
-        self.reads, self.writes = (x,), (y,)
+        self.reads, self.writes = (x,) + x.parts, (y,)
 
     def prepare(self, net):
         self.gamma = float(np.asarray(net.weights[self.var], dtype=np.float32).reshape(-1)[0])
@@ -434,6 +455,84 @@ class NearestConcatOp(Op):
                 "nearest_concat")
 
 
+# a tap of TF's 4x4 / stride-2 SAME conv2d_transpose (pad_before = 1) seen from output phase p along one axis, as a
+# 3x3 stencil row r on the low-resolution input (input index i + r - 1): output 2i + p takes input i + d through
+# kernel tap k = p + 1 - 2d.  None: that stencil row has no tap in this phase
+_DECONV_TAP = ((3, 1, None), (None, 2, 0))
+
+
+class PhaseConvOp(ConvOp):
+    """The 4x4 / stride-2 SAME conv2d_transpose (+ bias + BN) as one 3x3 stride-1 convolution with 4 * cout outputs:
+    output channel p * cout + c is phase p = 2 * py + px of channel c (PixelShuffleOp places it).  Each phase uses 2x2
+    of the 16 taps; the other stencil taps are zero."""
+
+    def __init__(self, x, y, kernel, bias, bn):
+        super().__init__(x, y, 3, 1, 1, kernel, bias, bn, None, None, None, False)
+
+    def host_weights(self, net):
+        k4 = np.asarray(net.weights[self.kernel], dtype=np.float32)  # [4, 4, cout, cin]
+        cout, cin = k4.shape[2], k4.shape[3]
+        kern = np.zeros((3, 3, cin, 4 * cout), np.float32)
+        for py in range(2):
+            for px in range(2):
+                p = 2 * py + px
+                for r in range(3):
+                    for s in range(3):
+                        ky, kx = _DECONV_TAP[py][r], _DECONV_TAP[px][s]
+                        if ky is not None and kx is not None:
+                            kern[r, s, :, p * cout:(p + 1) * cout] = k4[ky, kx].T
+        bias = np.tile(np.asarray(net.weights[self.bias], dtype=np.float32), 4)
+        return kern, bias
+
+    def host_bn(self, net):
+        sc, sh = net.bn_fold(self.bn)
+        return np.tile(sc, 4), np.tile(sh, 4)
+
+
+class PixelShuffleOp(Op):
+    """Phases [B, h, w, 4C] of PhaseConvOp -> act(out [B, 2h, 2w, C] (+ residual))."""
+
+    def __init__(self, x, y, residual, act):
+        self.x, self.y, self.residual, self.act = x, y, residual, act
+        self.reads = (x,) if residual is None else (x, residual)
+        self.writes = (y,)
+
+    def launch(self, net, stream):
+        x, y, r = self.x, self.y, self.residual
+        assert x.halo == 0 and y.halo == 0 and (r is None or r.halo == 0)
+        L.check(net.lib.odt_pixel_shuffle2x(x.ptr(), y.ptr(), r.ptr() if r is not None else None, net.dt, x.B, x.H,
+                                            x.W, y.C, x.ld, y.ld, r.ld if r is not None else 0, ACT[self.act],
+                                            stream), "pixel_shuffle2x")
+
+
+class ResizeOp(Op):
+    """Align-corners bilinear resize; `out2`: a concat slice that takes a second copy (Net.padded_concat)."""
+
+    def __init__(self, x, y):
+        self.x, self.y, self.out2 = x, y, None
+        self.reads, self.writes = (x,), (y,)
+
+    def launch(self, net, stream):
+        x, y, o2 = self.x, self.y, self.out2
+        assert x.halo == 0 and y.halo == 0
+        L.check(net.lib.odt_resize_bilinear_ac(x.ptr(), y.ptr() if y.needed else None,
+                                               o2.ptr() if o2 is not None else None, net.dt, x.B, x.H, x.W, x.C,
+                                               x.ld, y.H, y.W, y.ld, o2.ld if o2 is not None else 0, stream),
+                "resize_bilinear_ac")
+
+
+class AvgPoolOp(Op):
+    def __init__(self, x, y):
+        self.x, self.y = x, y
+        self.reads, self.writes = (x,), (y,)
+
+    def launch(self, net, stream):
+        x, y = self.x, self.y
+        assert x.halo == 0 and y.halo == 0
+        L.check(net.lib.odt_avgpool2x2_same(x.ptr(), y.ptr(), net.dt, x.B, x.H, x.W, x.C, x.ld, y.ld, stream),
+                "avgpool2x2_same")
+
+
 class Net:
     """A built network: buffers + op list + the decode/NMS tail."""
 
@@ -498,7 +597,7 @@ class Net:
              bn=False, act=None, residual=None, head=None, bias_init="zeros"):
         """tf.layers.conv2d (+ BN + activation + residual).  x=None means the image."""
         is_image = x is None
-        cin = 3 if is_image else x.C
+        cin = 3 if is_image else x.real_channels
         if kernel_var is None:
             vs = self.namer.named(name) if name else self.namer.unique("conv2d")
             kernel_var, bias_var = vs + "/kernel", vs + "/bias"
@@ -546,9 +645,11 @@ class Net:
         self.ops.append(PoolOp(x, y, k, stride))
         return y
 
-    def l2norm(self, x, var):
-        self.var(var, (1,), "l2norm")
+    def l2norm(self, x, var, init=20.0):
+        """x * rsqrt(sum_c x^2) * factor, with the scalar variable `var` initialised to `init`."""
+        self.var(var, (1,), "l2norm" if init == 20.0 else "l2norm_%g" % init)
         y = self.new_act(var + "/out", x.H, x.W, x.C)
+        y.chan_map = x.chan_map  # zero gap channels stay zero
         self.ops.append(L2NormOp(x, y, var))
         return y
 
@@ -577,6 +678,66 @@ class Net:
             views.append(v)
             c0 += t.C
         y.parts = tuple(views)
+        return y
+
+    def padded_concat(self, parts):
+        """tf.concat(parts, axis=channels) of parts whose widths are not multiples of 32 (PFPNet-R's 85-channel parts,
+        PFPNetR.py:364-395), with no copy: each part is stored at a 32-aligned channel offset of one buffer, the channels
+        between a part's end and the next offset stay zero, so a tensor-core producer's whole-chunk store stays inside
+        its slice.  `chan_map` of the result lists the stored channel of every real channel, and its consumers scatter
+        their filter rows to those channels (ConvOp.host_weights).  A part comes from a convolution (an extra
+        epilogue output, as in `concat`) or from `resize_ac` (its second output)."""
+        offs, c0 = [], 0
+        for t in parts:
+            assert (t.B, t.H, t.W) == (parts[0].B, parts[0].H, parts[0].W), (t.name, parts[0].name)
+            offs.append(c0)
+            c0 += _round_up(t.C, 32)
+        y = self.new_act(parts[0].name + "/concat", parts[0].H, parts[0].W, c0)
+        y.chan_map = np.concatenate([np.arange(o, o + t.C) for o, t in zip(offs, parts)])
+        views = []
+        for t, o in zip(parts, offs):
+            v = Act(t.name + "/slice", t.B, t.H, t.W, t.C, y.ld, t.dtype)
+            v.base, v.c0 = y, o
+            self.acts.append(v)
+            rs = next((op for op in self.ops if isinstance(op, ResizeOp) and op.y is t), None)
+            if rs is not None:
+                assert rs.out2 is None, t.name
+                rs.out2, rs.writes = v, (t, v)
+            else:
+                self.ops.append(AffineActOp(t, v, None, None))
+            views.append(v)
+        y.parts = tuple(views)
+        return y
+
+    def deconv(self, x, cout, residual=None, act=None):
+        """tf.layers.conv2d_transpose(cout, 4, 2, 'same') -> BN (PFPNetR.py:696-709), then `+ residual` and `act`:
+        one 3x3 stride-1 convolution of 4 * cout phase-major outputs on the low-resolution grid (PhaseConvOp) and their
+        placement on the 2x grid (PixelShuffleOp)."""
+        vs = self.namer.unique("conv2d_transpose")
+        kernel_var, bias_var = vs + "/kernel", vs + "/bias"
+        self.var(kernel_var, (4, 4, cout, x.real_channels), "he")
+        self.var(bias_var, (cout,), "zeros")
+        bn_scope = self.bn_vars(cout)
+        ph = self.new_act(kernel_var + "/phases", x.H, x.W, 4 * cout)
+        op = PhaseConvOp(x, ph, kernel_var, bias_var, bn_scope)
+        op.out_hw = (x.H, x.W)
+        self.ops.append(op)
+        y = self.new_act(kernel_var + "/out", 2 * x.H, 2 * x.W, cout)
+        if residual is not None:
+            assert (residual.H, residual.W, residual.C) == (y.H, y.W, y.C), (residual.name, y.name)
+        self.ops.append(PixelShuffleOp(ph, y, residual, act))
+        return y
+
+    def resize_ac(self, x, OH, OW):
+        """tf.image.resize_bilinear(x, [OH, OW], align_corners=True) (PFPNetR.py:324-326)."""
+        y = self.new_act(x.name + "/resize%dx%d" % (OH, OW), OH, OW, x.C)
+        self.ops.append(ResizeOp(x, y))
+        return y
+
+    def avgpool(self, x):
+        """tf.layers.average_pooling2d(x, 2, 2, 'same') (PFPNetR.py:721-728)."""
+        y = self.new_act(x.name + "/avgpool", (x.H + 1) // 2, (x.W + 1) // 2, x.C)
+        self.ops.append(AvgPoolOp(x, y))
         return y
 
     def add_level(self, H, W, A):
@@ -966,8 +1127,9 @@ class Tail:
     def __init__(self, kind, num_fg, nms_classes, score_thr, iou_thr, max_boxes, level_fn, cap=None):
         self.kind, self.num_fg, self.nms_classes = kind, num_fg, nms_classes
         # floats per candidate row, the one place the host decides it (DESIGN.md section 2): num_fg class scores + 5
-        # (SSD / RetinaNet: 20 + background + 4 box; YOLOv3: 4 box + objectness; FCOS: centre-ness + 4 distances)
-        self.row = num_fg + 5
+        # (SSD / RetinaNet: 20 + background + 4 box; YOLOv3: 4 box + objectness; FCOS: centre-ness + 4 distances);
+        # PFPNet-R's two-step rows + 11 (ODM background + 4 box, ARM 2 logits + 4 box)
+        self.row = num_fg + 11 if kind == L.DECODE_TWO_STEP else num_fg + 5
         self.score_thr, self.iou_thr, self.max_boxes = score_thr, iou_thr, max_boxes
         self.level_fn, self.cap = level_fn, cap
         self.pool_cap = 8 << 20  # box-pool entries (16 B each) for lists beyond the shared-memory window
@@ -1037,10 +1199,12 @@ class Tail:
     # training-loss kind -> the family's scalars of odt_<kind>_loss_fwd, in argument order, with their defaults
     LOSS_SCALARS = {"retina": (("alpha", 0.25), ("gamma", 2.0)), "ssd": (), "fcos": (),
                     "yolo": (("coord_scale", 1.0), ("noobj_scale", 1.0), ("obj_scale", 5.0), ("class_scale", 1.0)),
-                    "yolo2": (("coord_scale", 1.0), ("noobj_scale", 1.0), ("obj_scale", 5.0), ("class_scale", 1.0))}
+                    "yolo2": (("coord_scale", 1.0), ("noobj_scale", 1.0), ("obj_scale", 5.0), ("class_scale", 1.0)),
+                    "pfpnet": ()}
 
     def loss(self, net, kind, ground_truth, return_info=False, **kw):
-        """Training-loss forward kernels on the rows this tail reads: kind in 'retina' | 'ssd' | 'fcos' | 'yolo' | 'yolo2',
+        """Training-loss forward kernels on the rows this tail reads: kind in 'retina' | 'ssd' | 'fcos' | 'yolo' | 'yolo2' |
+        'pfpnet',
         the family's scalars (LOSS_SCALARS) as keywords.  ground_truth [B,G,5] (y,x,h,w,id) padded with -1.
         Returns float32 [B]; for 'ssd' with return_info=True also int32 [B,3] = (#positives, #negatives,
         #mined negatives) per image."""
@@ -1283,8 +1447,8 @@ def init_weights(variables, seed=1, bn_mode="tf_init", stem_scale=1.0 / 64.0):
             out[name] = np.zeros(shape, np.float32)
         elif kind == "pi":
             out[name] = np.full(shape, -math.log((1 - 0.01) / 0.01), np.float32)
-        elif kind == "l2norm":
-            out[name] = np.full(shape, 20.0, np.float32)
+        elif kind.startswith("l2norm"):  # "l2norm": 20 (SSD); "l2norm_<v>": v
+            out[name] = np.full(shape, 20.0 if kind == "l2norm" else float(kind[7:]), np.float32)
         elif kind in ("bn_gamma", "gn_gamma"):
             out[name] = (rng.uniform(0.8, 1.2, shape).astype(np.float32) if trained
                          else np.ones(shape, np.float32))

@@ -11,7 +11,7 @@ LIB_PATH = os.path.join(_HERE, "libodt_b200.so")
 
 ODT_F16, ODT_F32 = 0, 1
 ACT_NONE, ACT_RELU, ACT_LEAKY = 0, 1, 2
-DECODE_SSD, DECODE_YOLO3, DECODE_FCOS = 0, 1, 2
+DECODE_SSD, DECODE_YOLO3, DECODE_FCOS, DECODE_TWO_STEP = 0, 1, 2, 3
 MAX_LEVELS, MAX_PRIORS = 8, 9
 ERR_OVERFLOW = -4
 ERR_UNSUPPORTED = -3
@@ -97,6 +97,9 @@ SYMBOLS = {
     "odt_affine_act": (_I, [_P, _P, _I, _L, _I, _I, _P, _P, _I, _P]),
     "odt_upsample_bilinear_add": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _I, _P, _P]),
     "odt_upsample_nearest_concat": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "odt_pixel_shuffle2x": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "odt_resize_bilinear_ac": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "odt_avgpool2x2_same": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
     "odt_groupnorm_stats": (_I, [_P, _P, _I, _I, _L, _I, _I, _I, _F, _P]),
     "odt_groupnorm_apply": (_I, [_P, _P, _P, _I, _I, _L, _I, _I, _I, _P, _P, _I, _P]),
     "odt_groupnorm_act_workspace_bytes": (_L, [_I, _I, _L, _I, _I]),
@@ -119,6 +122,9 @@ SYMBOLS = {
     "odt_yolo2_loss_scratch_bytes": (_L, [C.POINTER(TailParams), _I]),
     "odt_yolo2_loss_fwd": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _F, _F, _F, _F, _P, _P, _P]),
     "odt_yolo2_loss_grad": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _F, _F, _F, _F, _P, _P, _P, _P]),
+    "odt_pfpnet_loss_scratch_bytes": (_L, [C.POINTER(TailParams), _I]),
+    "odt_pfpnet_loss_fwd": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _P, _P, _P]),
+    "odt_pfpnet_loss_grad": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _P, _P, _P, _P]),
     "odt_augment_scratch_bytes": (_L, [C.POINTER(AugmentParams), _I]),
     "odt_augment_batch": (_I, [_P, C.POINTER(AugmentParams), _I, _P, _P, _P, _P]),
     "odt_pool_classify": (_I, [_P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P]),

@@ -1,4 +1,4 @@
-"""Layer graphs of SSD300 / SSD512 / RetinaNet / YOLOv3 / YOLOv2 / FCOS expressed on the
+"""Layer graphs of SSD300 / SSD512 / RetinaNet / YOLOv3 / YOLOv2 / FCOS / PFPNet-R expressed on the
 H100 engine (engine.Net).  Each builder mirrors the reference's layer creation
 order so variables get the same TF1 names as in the reference checkpoints
 (SURVEY.md App. D); citations give the reference lines each block stands for.
@@ -468,4 +468,122 @@ def fcos_tail(cfg):
         lv.out_mul = strides[i]
 
     return Tail(L.DECODE_FCOS, nc, nc - 1, cfg["nms_score_threshold"], cfg["nms_iou_threshold"],
+                cfg["nms_max_boxes"], level_fn)
+
+
+# -------------------------------------------------------------- PFPNet-R ----
+def check_pfpnet_config(cfg):
+    """PFPNet-R's input size (a positive multiple of 64, PFPNetR.py:15: the pyramid halves the stride-8 grid three
+    times) and class count (20: the 21-logit softmax rows of the SSD family, see check_num_classes)."""
+    size = cfg["input_size"]
+    if isinstance(size, bool) or not isinstance(size, (int, np.integer)) or size <= 0 or size % 64:
+        raise ValueError("input_size = %r: PFPNet-R takes a positive multiple of 64" % (size,))
+    check_num_classes(cfg)
+
+
+PFPNET_STRIDES = (8, 16, 32, 64)  # PFPNetR.py:397-400
+PFPNET_RATIOS = (0.5, 1.0, 2.0)   # PFPNetR.py:30
+
+
+def build_pfpnet(batch, cfg, precision="fp16", device="cuda", allow_tc=True):
+    """ref PFPNetR.py:74-108,230-431.  Every `_conv_layer` / `_dconv_layer` is conv (+ bias) -> BN (-> ReLU); the
+    four 767-channel pyramid concats are stored 800 wide with their 85-channel parts at 32-aligned offsets
+    (Net.padded_concat).  Candidate rows: [ODM logits(21), ODM t(4), ARM logits(2), ARM t(4)] per anchor."""
+    check_pfpnet_config(cfg)
+    size = cfg["input_size"]
+    nc = cfg["num_classes"] + 1
+    A = len(PFPNET_RATIOS)
+    net = Net(batch, size, size, precision, device, allow_tc)
+    f = 512 // 6
+
+    def cl(x, cout, k, act=None):  # _conv_layer (:680-694)
+        return net.conv(x, cout, k, 1, bn=True, act=act)
+
+    with net.scope("feature_extractor"):
+        x = None
+        for item in _VGG[:13]:  # conv1_1 .. conv4_3 with the pools between (:231-315)
+            if item == "pool":
+                x = net.maxpool(x, 2, 2)
+                continue
+            _, kn, bnm, cout = item
+            x = net.conv(x, cout, 3, kernel_var="feature_extractor/" + kn, bias_var="feature_extractor/" + bnm,
+                         act="relu")
+        fh1 = x
+        fh2 = net.resize_ac(fh1, fh1.H // 2, fh1.W // 2)  # :319-326
+        fh3 = net.resize_ac(fh1, fh1.H // 4, fh1.W // 4)
+        fh4 = net.resize_ac(fh1, fh1.H // 8, fh1.W // 8)
+        fl1, fl2, fl3, fl4 = (cl(t, f, 1, "relu") for t in (fh1, fh2, fh3, fh4))  # :332-335
+
+        def up(low, lateral):  # _dconv_layer + lateral, then a 1x1 _conv_layer with ReLU (:336-347)
+            return cl(net.deconv(low, f, residual=lateral), f, 1, "relu")
+
+        fl2_1 = up(fl2, fl1)
+        fl3_2 = up(fl3, fl2)
+        fl3_1 = up(fl3_2, fl1)
+        fl4_3 = up(fl4, fl3)
+        fl4_2 = up(fl4_3, fl2)
+        fl4_1 = up(fl4_2, fl1)
+        fl1_2 = cl(net.avgpool(fl1), f, 1)  # avg-pool, then a 1x1 _conv_layer without activation (:349-362)
+        fl1_3 = cl(net.avgpool(fl1_2), f, 1)
+        fl1_4 = cl(net.avgpool(fl1_3), f, 1)
+        fl2_3 = cl(net.avgpool(fl2), f, 1)
+        fl2_4 = cl(net.avgpool(fl2_3), f, 1)
+        fl3_4 = cl(net.avgpool(fl3), f, 1)
+        feat1 = net.padded_concat([fh1, fl2_1, fl3_1, fl4_1])  # :364-395
+        feat2 = net.padded_concat([fl1_2, fh2, fl3_2, fl4_2])
+        feat3 = net.padded_concat([fl1_3, fl2_3, fh3, fl4_3])
+        feat4 = net.padded_concat([fl1_4, fl2_4, fl3_4, fh4])
+        feat1 = net.l2norm(feat1, "feature_extractor/feat1_l2_norm", 10.0)  # :77-93
+        feat2 = net.l2norm(feat2, "feature_extractor/feat2_l2_norm", 8.0)
+    feats = (feat1, feat2, feat3, feat4)
+    offs = [net.add_level(t.H, t.W, A) for t in feats]
+
+    def tower(x):  # four 3x3 / 256 _conv_layers with ReLU (:403-408, :423-428)
+        for _ in range(4):
+            x = cl(x, 256, 3, "relu")
+        return x
+
+    # head scatter: channel a * K + k of a K-wide prediction is column col + k of anchor a's row
+    row = nc + 10
+    with net.scope("ARM"):  # :94-98, :403-411
+        for i, t in enumerate(feats):
+            with net.scope("arm%d" % (i + 1)):
+                y = tower(t)
+                net.conv(y, 4 * A, 3, 1, bn=True, head=(offs[i], nc + 6, 4, row, A))
+                net.conv(y, 2 * A, 3, 1, bn=True, head=(offs[i], nc + 4, 2, row, A))
+    tcbs = [None] * 4
+    with net.scope("TCB"):  # :99-103, :413-421
+        for i in (3, 2, 1, 0):
+            with net.scope("tcb%d" % (i + 1)):
+                y = cl(feats[i], 256, 3, "relu")
+                if i == 3:
+                    tcbs[i] = cl(y, 256, 3, "relu")  # relu(conv2): the top level has no higher feature
+                else:
+                    c2 = cl(y, 256, 3)
+                    tcbs[i] = net.deconv(tcbs[i + 1], 256, residual=c2, act="relu")  # relu(conv2 + BN(dconv))
+    with net.scope("ODM"):  # :104-108, :423-431
+        for i, t in enumerate(tcbs):
+            with net.scope("odm%d" % (i + 1)):
+                y = tower(t)
+                net.conv(y, 4 * A, 3, 1, bn=True, head=(offs[i], nc, 4, row, A))
+                net.conv(y, nc * A, 3, 1, bn=True, head=(offs[i], 0, nc, row, A))
+    return net, pfpnet_tail(cfg)
+
+
+def pfpnet_tail(cfg):
+    """two-step decode / NMS tail of PFPNet-R (ref PFPNetR.py:187-228,447-467): anchors of size 4 * stride at ratios
+    0.5 / 1 / 2 centred at (i + 0.5) * stride; a row survives when ARM's background probability is below 0.99 and
+    ODM's arg-max is a foreground class; ODM's deltas refine the ARM-refined anchor."""
+    nc = cfg["num_classes"] + 1
+
+    def level_fn(i, h, w, lv):
+        stride = PFPNET_STRIDES[i]
+        lv.cmul_y = lv.cmul_x = float(stride)
+        lv.cdiv_y = lv.cdiv_x = 1.0
+        lv.out_mul = 1.0
+        size = 4 * stride
+        for a, r in enumerate(PFPNET_RATIOS):
+            lv.prior_h[a], lv.prior_w[a] = float(F32(size * (r ** 0.5))), float(F32(size / (r ** 0.5)))
+
+    return Tail(L.DECODE_TWO_STEP, nc - 1, nc - 1, cfg["nms_score_threshold"], cfg["nms_iou_threshold"],
                 cfg["nms_max_boxes"], level_fn)

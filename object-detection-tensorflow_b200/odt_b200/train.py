@@ -258,7 +258,7 @@ class GraphTrainer:
         from . import engine as E
         self.model, self.cfg, self.E = model, model.config, E
         self.kind = {"SSD300": "ssd", "SSD512": "ssd", "RetinaNet": "retina", "YOLOv3": "yolo", "YOLOv2": "yolo2",
-                     "FCOS": "fcos"}[model.name]
+                     "FCOS": "fcos", "PFPNetR": "pfpnet"}[model.name]
         if getattr(model, "is_pretraining", False):
             self.kind = "classify"                # RetinaNet's ImageNet-pretraining mode
         self.weight_decay = float(model.weight_decay)
@@ -281,7 +281,7 @@ class GraphTrainer:
         # CUDA, fp32 rows: the data term is the family's loss-gradient kernel (csrc/loss.cu) behind one autograd
         # Function; the CPU (and float64) keep the restatement below, which the kernels are tested against
         self._loss_kernels = None
-        if self.kind in ("ssd", "retina", "yolo", "yolo2", "fcos") and self.device.type == "cuda" and dtype == torch.float32:
+        if self.kind in ("ssd", "retina", "yolo", "yolo2", "fcos", "pfpnet") and self.device.type == "cuda" and dtype == torch.float32:
             self._loss_kernels = LossKernels(self)
         if self.kind == "ssd":
             self._ssd = SSDTrainer.__new__(SSDTrainer)   # borrows the SSD loss / anchors
@@ -324,7 +324,11 @@ class GraphTrainer:
         rows = torch.zeros((B, N * (self.row or 0)), device=self.device, dtype=self.dtype)
         val = {}
         for op in self.net.ops:
-            if isinstance(op, E.ConvOp):
+            if isinstance(op, E.PhaseConvOp):          # tf.layers.conv2d_transpose(4, 2, 'same') + BN
+                k = P[op.kernel].permute(3, 2, 0, 1)   # [4, 4, out, in] -> [in, out, 4, 4]
+                y = F.conv_transpose2d(val[id(op.x)], k, P[op.bias], stride=2, padding=1)
+                val[id(op.y)] = self._bn(y, op.bn, training, stats)
+            elif isinstance(op, E.ConvOp):
                 if op.is_image:
                     x = x0
                 elif op.x.parts:                    # engine.Net.concat: the slices in channel order
@@ -357,7 +361,7 @@ class GraphTrainer:
                 y = F.group_norm(x, op.groups, P[op.gn + "/gamma"], P[op.gn + "/beta"], eps=E.GN_EPS)
                 val[id(op.y)] = _act(y, op.act)
             elif isinstance(op, E.L2NormOp):
-                x = val[id(op.x)]
+                x = torch.cat([val[id(v)] for v in op.x.parts], dim=1) if op.x.parts else val[id(op.x)]
                 x = x * torch.rsqrt(torch.clamp((x * x).sum(dim=1, keepdim=True), min=1e-12))
                 val[id(op.y)] = x * P[op.var].view(1, 1, 1, 1)
             elif isinstance(op, E.UpsampleAddOp):
@@ -366,6 +370,18 @@ class GraphTrainer:
             elif isinstance(op, E.NearestConcatOp):
                 a, b = val[id(op.a)], val[id(op.b)]
                 val[id(op.y)] = torch.cat([a, _resize_nearest_legacy(b, a.shape[2], a.shape[3])], dim=1)
+            elif isinstance(op, E.PixelShuffleOp):     # the transposed convolution (+ lateral) (+ ReLU)
+                y = val[id(op.x)]
+                if op.residual is not None:
+                    y = y + val[id(op.residual)]
+                val[id(op.y)] = _act(y, op.act)
+            elif isinstance(op, E.ResizeOp):           # resize_bilinear(align_corners=True): (in-1)/(out-1) scale
+                y = F.interpolate(val[id(op.x)], size=(op.y.H, op.y.W), mode="bilinear", align_corners=True)
+                val[id(op.y)] = y
+                if op.out2 is not None:
+                    val[id(op.out2)] = y
+            elif isinstance(op, E.AvgPoolOp):          # 2x2/2 SAME: partial windows divided by their cells inside
+                val[id(op.y)] = F.avg_pool2d(val[id(op.x)], 2, 2, ceil_mode=True, count_include_pad=False)
             else:
                 raise TypeError(type(op))
         return val, rows
@@ -579,11 +595,89 @@ class GraphTrainer:
         coord, cls_l, obj_l, noobj = self._yolo_terms(L_, every, nc, 0.6, (0.0, 0.0, 0.0, 0.0))
         return cs * coord + ks * cls_l + os_ * obj_l + ns * noobj
 
+    def _pfpnet_anchors(self):
+        """_get_abbox of PFPNetR.py:447-467 over the engine's levels: (y1x1, y2x2, yx, hw), each [N, 2]."""
+        if self._anchor_cache is None:
+            from . import nets as NN
+            y1x1, y2x2 = [], []
+            for (h, w, _), s in zip(self.net.levels, NN.PFPNET_STRIDES):
+                pri = torch.tensor([[4 * s * (r ** 0.5), 4 * s / (r ** 0.5)] for r in NN.PFPNET_RATIOS],
+                                   dtype=torch.float32).view(1, 1, -1, 2)
+                cy = (torch.arange(h, dtype=torch.float32) + 0.5) * float(s)
+                cx = (torch.arange(w, dtype=torch.float32) + 0.5) * float(s)
+                yx = torch.stack(torch.meshgrid(cy, cx, indexing="ij"), dim=-1).view(h, w, 1, 2)
+                y1x1.append((yx - pri / 2.0).reshape(-1, 2))
+                y2x2.append((yx + pri / 2.0).reshape(-1, 2))
+            a1 = torch.cat(y1x1).to(self.device, self.dtype)
+            a2 = torch.cat(y2x2).to(self.device, self.dtype)
+            self._anchor_cache = (a1, a2, a1 / 2.0 + a2 / 2.0, a2 - a1)
+        return self._anchor_cache
+
+    def pfpnet_image_loss(self, row, gt):
+        """PFPNetR.py:469-610 for one image: row [N, 31] = [ODM logits(21), ODM t(4), ARM logits(2), ARM t(4)].  Per-GT
+        arg-max anchors + IoU > 0.5 positive, < 0.4 negative; ARM: positives' cross-entropy to 0 and smooth-L1 to the
+        anchor targets, hard negatives by NMS (IoU 0.7, min(#neg, 3 #pos)) scored by their cross-entropy to 1; ODM: the
+        mined negatives whose raw ARM logit 1 is < 0.99, cross-entropy to 20; positives' cross-entropy to their class
+        and smooth-L1 to targets from the decoded ARM box, differentiated through it.  A mean over no element is 0
+        (csrc/loss.cu, DESIGN.md section 7)."""
+        from torchvision.ops import nms
+        a1, a2, ayx, ahw = self._pfpnet_anchors()
+        gt = torch.as_tensor(gt, device=self.device, dtype=self.dtype)
+        cnt = int(torch.argmin(gt[:, 0]).item())
+        g = gt[:cnt]
+        gyx, ghw, label = g[:, 0:2], g[:, 2:4], g[:, 4].long()
+        g1, g2 = gyx - ghw / 2.0, gyx + ghw / 2.0
+        oc, ot, ac, at = row[:, :21], row[:, 21:25], row[:, 25:27], row[:, 27:31]
+        N = row.shape[0]
+        dev = self.device
+        with torch.no_grad():
+            inter = torch.clamp(torch.minimum(a2[None], g2[:, None]) - torch.maximum(a1[None], g1[:, None]), min=0).prod(-1)
+            iou = inter / (ahw.prod(-1)[None] + ghw.prod(-1)[:, None] - inter)
+            best = torch.argmax(iou, dim=1) if cnt else torch.zeros(0, dtype=torch.long, device=dev)
+            other = torch.ones(N, dtype=torch.bool, device=dev)
+            other[best] = False
+            o_idx = torch.nonzero(other).squeeze(1)
+            if cnt:
+                o_best, rg = iou[:, o_idx].max(dim=0)
+            else:                                  # reduce_max over no GT: every anchor is a negative
+                o_best = torch.full((o_idx.numel(),), -float("inf"), device=dev, dtype=self.dtype)
+                rg = torch.zeros(o_idx.numel(), dtype=torch.long, device=dev)
+            pos, neg = o_best > 0.5, o_best < 0.4
+            pos_idx = torch.cat([best, o_idx[pos]])
+            pos_g = torch.cat([torch.arange(cnt, device=dev), rg[pos]])
+            neg_idx = o_idx[neg]
+
+        def mean0(x):
+            return x.sum() / x.numel() if x.numel() else x.sum()
+
+        P, nneg = int(pos_idx.numel()), int(neg_idx.numel())
+        chosen = 3 * P if nneg > 3 * P else nneg
+        neg_arm = F.cross_entropy(ac[neg_idx], torch.ones(nneg, dtype=torch.long, device=dev), reduction="none")
+        with torch.no_grad():
+            nbox = torch.cat([ayx[neg_idx] - ahw[neg_idx] / 2.0, ayx[neg_idx] + ahw[neg_idx] / 2.0], dim=1)
+            sel = nms(nbox.float(), neg_arm.detach().float(), 0.7)[:chosen]
+            mined = neg_idx[sel]
+            mined_odm = mined[ac[mined, 1] < 0.99]
+        sl1 = SSDTrainer._smooth_l1
+        arm = mean0(neg_arm[sel]) + mean0(F.cross_entropy(ac[pos_idx], torch.zeros(P, dtype=torch.long, device=dev),
+                                                          reduction="none"))
+        pa, pyx, phw = ahw[pos_idx], ayx[pos_idx], at[pos_idx]
+        tyx, thw = (gyx[pos_g] - pyx) / pa, torch.log(ghw[pos_g] / pa)
+        arm = arm + mean0(sl1(phw[:, :2] - tyx).sum(-1) + sl1(phw[:, 2:] - thw).sum(-1))
+        arm_yx = phw[:, :2] * pa + pyx
+        arm_hw = torch.exp(phw[:, 2:]) * pa
+        oyx, ohw = (gyx[pos_g] - arm_yx) / arm_hw, torch.log(ghw[pos_g] / arm_hw)
+        odm = mean0(F.cross_entropy(oc[mined_odm], torch.full((mined_odm.numel(),), 20, dtype=torch.long, device=dev),
+                                    reduction="none"))
+        odm = odm + mean0(F.cross_entropy(oc[pos_idx], label[pos_g], reduction="none"))
+        odm = odm + mean0(sl1(ot[pos_idx, :2] - oyx).sum(-1) + sl1(ot[pos_idx, 2:] - ohw).sum(-1))
+        return arm + odm
+
     def image_loss(self, row, gt):
         if self.kind == "ssd":
             return self._ssd.image_loss(row, gt)[0]
         return {"retina": self.retina_image_loss, "fcos": self.fcos_image_loss, "yolo": self.yolo_image_loss,
-                "yolo2": self.yolo2_image_loss}[self.kind](row, gt)
+                "yolo2": self.yolo2_image_loss, "pfpnet": self.pfpnet_image_loss}[self.kind](row, gt)
 
     def total_loss(self, rows, ground_truth):
         if self._loss_kernels is not None:
