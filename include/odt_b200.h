@@ -209,6 +209,11 @@ int odt_resize_bilinear_ac(const void* in, void* out, void* out2, int dtype, int
  * order, divided by their count (TF's SAME average, not /4). */
 int odt_avgpool2x2_same(const void* in, void* out, int dtype, int B, int H, int W, int C, int in_ld, int out_ld,
                         void* stream);
+/* CenterNet's DLA joins (ref CenterNet.py:93-110,390-401); NHWC, fp32 math, one rounding per TF op.
+ * pooled = 0: out = a + b, all [B,H,W,C].  pooled = 1: out [B,ceil(H/2),ceil(W/2),C] = 2x2/2 SAME max pool of a + 2x2/2
+ * SAME average pool of b (the window's cells inside the image, summed in row-major order, divided by their count). */
+int odt_dla_join(const void* a, const void* b, void* out, int dtype, int B, int H, int W, int C, int a_ld, int b_ld,
+                 int out_ld, int pooled, void* stream);
 /* GroupNorm(groups) statistics: stats[b][g] = (mean, rstd), eps inside; stats holds B*groups*2 floats.
  * One CTA per (group, image), two passes (mean, then the sum of squared deviations) in a fixed order: the result
  * does not depend on B or on scheduling.  ref: FCOS.py:438-446 */
@@ -239,6 +244,8 @@ int odt_groupnorm_act(const void* in, void* out, void* workspace, int dtype, int
 #define ODT_DECODE_TWO_STEP 3 /* PFPNet-R: ARM -> ODM two-step softmax decode, rows of
                                num_fg + 11 floats [odm logits(21), odm t(4), arm logits(2),
                                arm t(4)]; num_fg must be 20 (ref PFPNetR.py:187-228)  */
+#define ODT_DECODE_PEAK 4   /* CenterNet: one stride-4 level, rows of num_fg + 4 floats [keypoint logits
+                               (num_fg), dy dx, h w]; decoded by odt_peak_topk, not odt_decode_candidates */
 
 typedef struct {
   int H, W, A;  /* feature grid and priors per cell                            */
@@ -382,6 +389,28 @@ int odt_pfpnet_loss_fwd(const float* head, const odt_tail_params* p, int B, cons
                         float* loss_out, void* stream);
 int odt_pfpnet_loss_grad(const float* head, const odt_tail_params* p, int B, const float* gt, int G, void* scratch,
                          float* loss_out, float* grad_out, void* stream);
+/* CenterNet's detection tail (ref CenterNet.py:159-185) on ODT_DECODE_PEAK rows [B, H*W, num_fg + 4] (p: one level
+ * H x W, A = 1, N = H*W, num_fg 1..128, max_boxes = K 1..1024, score_thr).  Per image: s = the largest class sigmoid
+ * (the float32 value nearest the exact sigmoid; first maximum for the class), a cell's score is s where s equals its
+ * 3x3 SAME max pool and 0 elsewhere, kept when > score_thr; the top min(n, K) by descending score, lower cell index
+ * first on ties; box ((i, j) + (dy, dx) -/+ (h, w) / 2) * 4.  rec [B, rec_ld >= 6K + 2]: K rows (score, y1, x1, y2, x2,
+ * class), zero past the count, then (count, 0) -- the packed record of odt_nms_per_class.  det_anchor (may be NULL):
+ * i32 [B, K] cell index of every row.  scratch: 8-byte aligned, odt_peak_topk_scratch_bytes.  Two launches, exact
+ * and deterministic. */
+long long odt_peak_topk_scratch_bytes(const odt_tail_params* p, int B);
+int odt_peak_topk(const float* head, const odt_tail_params* p, int B, void* scratch, float* rec, int rec_ld,
+                  int* det_anchor, void* stream);
+/* CenterNet's loss (ref CenterNet.py:187-270) on ODT_DECODE_PEAK rows, G <= 128, in float64: per image, GT / 4, centre
+ * cells floored (and clamped into the grid); one sigma, the least CornerNet radius over every GT; per class the maximum
+ * of exp(-d^2 / 2 sigma^2) around its GTs' unfloored centres; positive focal -(1-p)^2 log p at the centre cells,
+ * negative -(1-r)^4 p^2 log(1-p) elsewhere, both summed / G; + 0.1 * mean |size| + mean |offset| L1 over G x 2 at the
+ * centre cells.  An image without boxes has loss 0 and gradient 0.  loss_out: f32 [B]; _grad also writes
+ * d loss[b] / d rows[b], every element (sign(0) = 0; GTs sharing a cell add up in GT order). */
+long long odt_centernet_loss_scratch_bytes(const odt_tail_params* p, int B);
+int odt_centernet_loss_fwd(const float* head, const odt_tail_params* p, int B, const float* gt, int G, void* scratch,
+                           float* loss_out, void* stream);
+int odt_centernet_loss_grad(const float* head, const odt_tail_params* p, int B, const float* gt, int G, void* scratch,
+                            float* loss_out, float* grad_out, void* stream);
 
 /* ------------------------------------------------ training augmentation --- */
 /* image_augmentor's pixel work (utils/image_augmentor.py:7-264, as odt_b200/tfrecord.py's augment_pixels restates

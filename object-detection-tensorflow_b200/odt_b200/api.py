@@ -5,7 +5,7 @@ asserts and method names as the reference model scripts, so its test*.py
 drivers run unchanged (SURVEY.md section 8b):
     SSD300.py:11-50,473-504   SSD512.py   RetinaNet.py:11-79,505-539
     YOLOv3.py:11-60,444-483   YOLOv2.py:11-54,305-343   FCOS.py:11-49,401-436
-    PFPNetR.py:11-53,615-661
+    PFPNetR.py:11-53,615-661  CenterNet.py:11-48,272-324
 Inference (`test_one_image`) runs entirely on the hand-written GPU kernels; there is no CPU
 fallback.  `train_one_epoch` runs the training step of odt_b200/train.py (PyTorch autograd over the
 engine's layer list + the reference's losses + Momentum: the first stage of SURVEY 8f row 2; RetinaNet's
@@ -63,6 +63,12 @@ class _Detector:
     seed = 1
 
     def _common_init(self, config, data_provider):
+        self._base_init(config, data_provider)
+        self.nms_score_threshold = config["nms_score_threshold"]
+        self.nms_max_boxes = config["nms_max_boxes"]
+        self.nms_iou_threshold = config["nms_iou_threshold"]
+
+    def _base_init(self, config, data_provider):
         assert config["mode"] in ["train", "test"]
         assert config["data_format"] in ["channels_first", "channels_last"]
         self.config = config
@@ -72,9 +78,6 @@ class _Detector:
         self.weight_decay = config["weight_decay"]
         self.prob = 1.0 - config["keep_prob"]
         self.batch_size = config["batch_size"] if config["mode"] == "train" else 1
-        self.nms_score_threshold = config["nms_score_threshold"]
-        self.nms_max_boxes = config["nms_max_boxes"]
-        self.nms_iou_threshold = config["nms_iou_threshold"]
         if self.mode == "train":
             self.num_train = data_provider["num_train"]
             self.num_val = data_provider["num_val"]
@@ -728,3 +731,27 @@ class PFPNetR(_Detector):
 
     def _build(self, batch, precision, allow_tc=True):
         return nets.build_pfpnet(batch, self.config, precision, self.device, allow_tc)
+
+
+class CenterNet(_Detector):
+    """CenterNet (ref CenterNet.py): a DLA backbone with pooled stage joins, three transposed-convolution upsampling
+    paths summed at stride 4, keypoint / offset / size heads, a peak + top-k tail; trained with Adam."""
+    name = "CenterNet"
+    backbone_scope = "backone"  # sic (CenterNet.py:73,279)
+    # Gaussian-heatmap focal loss with one sigma per image, L1 offset and size at the centre cells:
+    # ref CenterNet.py:187-270
+    loss_kind = "centernet"
+
+    def __init__(self, config, data_provider):
+        nets.check_centernet_config(config)
+        self._base_init(config, data_provider)  # the config has no nms_* keys
+        self.input_size = config["input_size"]
+        s = self.input_size
+        self.data_shape = [s, s, 3] if config["data_format"] == "channels_last" else [3, s, s]
+        self.num_classes = config["num_classes"]
+        if self.mode == "test":
+            self.score_threshold = config["score_threshold"]
+            self.top_k_results_output = config["top_k_results_output"]
+
+    def _build(self, batch, precision, allow_tc=True):
+        return nets.build_centernet(batch, self.config, precision, self.device, allow_tc)

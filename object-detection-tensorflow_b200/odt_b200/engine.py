@@ -142,6 +142,9 @@ class ConvOp(Op):
         bias = (np.asarray(net.weights[self.bias], dtype=np.float32) if self.bias
                 else np.zeros(kern.shape[3], np.float32))
         x = self.x
+        if self.is_image and net.in_scale is not None:
+            # a per-channel input scale folds exactly into the input-channel rows: SAME padding pads with zeros
+            kern = (kern * np.asarray(net.in_scale, np.float32).reshape(1, 1, 3, 1)).astype(np.float32)
         if x is not None and x.chan_map is not None:
             full = np.zeros(kern.shape[:2] + (x.C, kern.shape[3]), np.float32)
             full[:, :, x.chan_map, :] = kern
@@ -466,8 +469,8 @@ class PhaseConvOp(ConvOp):
     output channel p * cout + c is phase p = 2 * py + px of channel c (PixelShuffleOp places it).  Each phase uses 2x2
     of the 16 taps; the other stencil taps are zero."""
 
-    def __init__(self, x, y, kernel, bias, bn):
-        super().__init__(x, y, 3, 1, 1, kernel, bias, bn, None, None, None, False)
+    def __init__(self, x, y, kernel, bias, bn, act=None):
+        super().__init__(x, y, 3, 1, 1, kernel, bias, bn, act, None, None, False)
 
     def host_weights(self, net):
         k4 = np.asarray(net.weights[self.kernel], dtype=np.float32)  # [4, 4, cout, cin]
@@ -533,6 +536,20 @@ class AvgPoolOp(Op):
                 "avgpool2x2_same")
 
 
+class DlaJoinOp(Op):
+    """CenterNet's DLA joins: a + b, or (pooled) 2x2 SAME max pool of a + 2x2 SAME average pool of b."""
+
+    def __init__(self, a, b, y, pooled):
+        self.a, self.b, self.y, self.pooled = a, b, y, pooled
+        self.reads, self.writes = (a, b), (y,)
+
+    def launch(self, net, stream):
+        a, b, y = self.a, self.b, self.y
+        assert a.halo == 0 and b.halo == 0 and y.halo == 0
+        L.check(net.lib.odt_dla_join(a.ptr(), b.ptr(), y.ptr(), net.dt, a.B, a.H, a.W, a.C, a.ld, b.ld, y.ld,
+                                     int(self.pooled), stream), "dla_join")
+
+
 class Net:
     """A built network: buffers + op list + the decode/NMS tail."""
 
@@ -552,6 +569,7 @@ class Net:
         self.levels = []    # (H, W, A) per head level, in candidate order
         self.tail = None
         self.mean3 = (C.c_float * 3)(123.68, 116.779, 103.979)  # ref SSD300.py:55
+        self.in_scale = None  # per-channel multiplier of the mean-subtracted image, folded into the stem's kernel
         # ODT_HALO=0 keeps every tensor dense: the end-to-end reference the halo layouts are tested against
         self.use_halo = os.environ.get("ODT_HALO", "1") != "0"
         self.weights = None
@@ -594,8 +612,9 @@ class Net:
         return _S()
 
     def conv(self, x, cout, k, stride=1, dil=1, name=None, kernel_var=None, bias_var=None,
-             bn=False, act=None, residual=None, head=None, bias_init="zeros"):
-        """tf.layers.conv2d (+ BN + activation + residual).  x=None means the image."""
+             bn=False, act=None, residual=None, head=None, bias_init="zeros", bn_scope=None):
+        """tf.layers.conv2d (+ BN + activation + residual).  x=None means the image.  bn_scope: the BN variables'
+        scope when they were named ahead of this call (TF order differs from op order)."""
         is_image = x is None
         cin = 3 if is_image else x.real_channels
         if kernel_var is None:
@@ -604,7 +623,8 @@ class Net:
         self.var(kernel_var, (k, k, cin, cout), "he")
         if bias_var:
             self.var(bias_var, (cout,), bias_init)
-        bn_scope = self.bn_vars(cout) if bn else None
+        if bn and bn_scope is None:
+            bn_scope = self.bn_vars(cout)
         H, W = (self.in_h, self.in_w) if is_image else (x.H, x.W)
         OH, _, _ = same_pad(H, k, stride, dil)
         OW, _, _ = same_pad(W, k, stride, dil)
@@ -713,19 +733,37 @@ class Net:
         """tf.layers.conv2d_transpose(cout, 4, 2, 'same') -> BN (PFPNetR.py:696-709), then `+ residual` and `act`:
         one 3x3 stride-1 convolution of 4 * cout phase-major outputs on the low-resolution grid (PhaseConvOp) and their
         placement on the 2x grid (PixelShuffleOp)."""
+        return self.shuffle(self.deconv_phases(x, cout), residual, act)
+
+    def deconv_phases(self, x, cout, act=None):
+        """tf.layers.conv2d_transpose(cout, 4, 2, 'same') -> BN (-> act) as the four phases on the low-resolution grid,
+        `act` in the phase convolution's epilogue (CenterNet.py:349-361: the ReLU comes before its sums); `shuffle`
+        places them."""
         vs = self.namer.unique("conv2d_transpose")
         kernel_var, bias_var = vs + "/kernel", vs + "/bias"
         self.var(kernel_var, (4, 4, cout, x.real_channels), "he")
         self.var(bias_var, (cout,), "zeros")
         bn_scope = self.bn_vars(cout)
         ph = self.new_act(kernel_var + "/phases", x.H, x.W, 4 * cout)
-        op = PhaseConvOp(x, ph, kernel_var, bias_var, bn_scope)
+        op = PhaseConvOp(x, ph, kernel_var, bias_var, bn_scope, act)
         op.out_hw = (x.H, x.W)
         self.ops.append(op)
-        y = self.new_act(kernel_var + "/out", 2 * x.H, 2 * x.W, cout)
+        return ph
+
+    def shuffle(self, ph, residual=None, act=None):
+        """act(the phases of `deconv_phases` on the 2x grid (+ residual))."""
+        y = self.new_act(ph.name + "/out%d" % len(self.ops), 2 * ph.H, 2 * ph.W, ph.C // 4)
         if residual is not None:
             assert (residual.H, residual.W, residual.C) == (y.H, y.W, y.C), (residual.name, y.name)
         self.ops.append(PixelShuffleOp(ph, y, residual, act))
+        return y
+
+    def dla_join(self, a, b, pooled):
+        """a + b, or (pooled) max_pool(a, 2, 2, SAME) + average_pool(b, 2, 2, SAME) (CenterNet.py:93-110)."""
+        assert (a.H, a.W, a.C) == (b.H, b.W, b.C), (a.name, b.name)
+        H, W = ((a.H + 1) // 2, (a.W + 1) // 2) if pooled else (a.H, a.W)
+        y = self.new_act(a.name + ("/join_pooled" if pooled else "/join"), H, W, a.C)
+        self.ops.append(DlaJoinOp(a, b, y, pooled))
         return y
 
     def resize_ac(self, x, OH, OW):
@@ -1129,7 +1167,8 @@ class Tail:
         # floats per candidate row, the one place the host decides it (DESIGN.md section 2): num_fg class scores + 5
         # (SSD / RetinaNet: 20 + background + 4 box; YOLOv3: 4 box + objectness; FCOS: centre-ness + 4 distances);
         # PFPNet-R's two-step rows + 11 (ODM background + 4 box, ARM 2 logits + 4 box)
-        self.row = num_fg + 11 if kind == L.DECODE_TWO_STEP else num_fg + 5
+        # CenterNet's peak rows + 4 (dy, dx, h, w after the keypoint logits)
+        self.row = num_fg + 11 if kind == L.DECODE_TWO_STEP else num_fg + 4 if kind == L.DECODE_PEAK else num_fg + 5
         self.score_thr, self.iou_thr, self.max_boxes = score_thr, iou_thr, max_boxes
         self.level_fn, self.cap = level_fn, cap
         self.pool_cap = 8 << 20  # box-pool entries (16 B each) for lists beyond the shared-memory window
@@ -1200,7 +1239,7 @@ class Tail:
     LOSS_SCALARS = {"retina": (("alpha", 0.25), ("gamma", 2.0)), "ssd": (), "fcos": (),
                     "yolo": (("coord_scale", 1.0), ("noobj_scale", 1.0), ("obj_scale", 5.0), ("class_scale", 1.0)),
                     "yolo2": (("coord_scale", 1.0), ("noobj_scale", 1.0), ("obj_scale", 5.0), ("class_scale", 1.0)),
-                    "pfpnet": ()}
+                    "pfpnet": (), "centernet": ()}
 
     def loss(self, net, kind, ground_truth, return_info=False, **kw):
         """Training-loss forward kernels on the rows this tail reads: kind in 'retina' | 'ssd' | 'fcos' | 'yolo' | 'yolo2' |
@@ -1258,6 +1297,41 @@ class Tail:
         """ONE D2H read of the packed records -> per-image [scores f32[K], bbox f32[K,4] (y1,x1,y2,x2),
         class_id i32[K]] (ref SSD300.py:190)."""
         return unpack_records(self.rec.cpu().numpy(), self.p.cap)
+
+
+class PeakTail(Tail):
+    """CenterNet's tail (CenterNet.py:159-185) on rows [B, H*W, num_fg + 4] of one stride-4 level: the peaks of the
+    per-cell best class sigmoid above `score_thr`, the top `max_boxes` of them, boxes around their integer cells --
+    odt_peak_topk, two launches, into the packed record every tail writes (D = max_boxes rows)."""
+
+    def __init__(self, num_fg, score_thr, max_boxes):
+        super().__init__(L.DECODE_PEAK, num_fg, 1, score_thr, 0.0, max_boxes, lambda i, h, w, lv: None)
+
+    def prepare(self, net, head_buf=None):
+        dev = net.device
+        B = net.batch
+        self.head_buf = net.head_buf if head_buf is None else head_buf
+        self.p = p = self.params(net.levels)
+        self.D = D = self.max_boxes
+        self.rec = torch.zeros((B, D * 6 + 2), dtype=torch.float32, device=dev)
+        self.dets = self.rec[:, :D * 6].view(B, D, 6)
+        self.det_anchor = torch.zeros((B, D), dtype=torch.int32, device=dev)
+        nbytes = net.lib.odt_peak_topk_scratch_bytes(C.byref(p), B)
+        if nbytes < 0:
+            raise L.OdtError("odt_peak_topk_scratch_bytes: %s" % net.lib.odt_last_error().decode())
+        self.scratch = torch.zeros((nbytes + 7) // 8, dtype=torch.int64, device=dev)
+
+    @property
+    def det_count(self):
+        return self.rec[:, self.D * 6].to(torch.int32)
+
+    def launch(self, net, stream):
+        L.check(net.lib.odt_peak_topk(self.head_buf.data_ptr(), C.byref(self.p), net.batch, self.scratch.data_ptr(),
+                                      self.rec.data_ptr(), self.rec.shape[1], self.det_anchor.data_ptr(), stream),
+                "peak_topk")
+
+    def num_launches(self):
+        return 2  # per-cell score + peak / top-k selection
 
 
 MAX_LOSS_GT = 128  # GT rows per image the loss kernels hold (kMaxGT in csrc/loss.cu)

@@ -11,7 +11,7 @@ LIB_PATH = os.path.join(_HERE, "libodt_b200.so")
 
 ODT_F16, ODT_F32 = 0, 1
 ACT_NONE, ACT_RELU, ACT_LEAKY = 0, 1, 2
-DECODE_SSD, DECODE_YOLO3, DECODE_FCOS, DECODE_TWO_STEP = 0, 1, 2, 3
+DECODE_SSD, DECODE_YOLO3, DECODE_FCOS, DECODE_TWO_STEP, DECODE_PEAK = 0, 1, 2, 3, 4
 MAX_LEVELS, MAX_PRIORS = 8, 9
 ERR_OVERFLOW = -4
 ERR_UNSUPPORTED = -3
@@ -100,6 +100,7 @@ SYMBOLS = {
     "odt_pixel_shuffle2x": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     "odt_resize_bilinear_ac": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     "odt_avgpool2x2_same": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "odt_dla_join": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     "odt_groupnorm_stats": (_I, [_P, _P, _I, _I, _L, _I, _I, _I, _F, _P]),
     "odt_groupnorm_apply": (_I, [_P, _P, _P, _I, _I, _L, _I, _I, _I, _P, _P, _I, _P]),
     "odt_groupnorm_act_workspace_bytes": (_L, [_I, _I, _L, _I, _I]),
@@ -125,6 +126,11 @@ SYMBOLS = {
     "odt_pfpnet_loss_scratch_bytes": (_L, [C.POINTER(TailParams), _I]),
     "odt_pfpnet_loss_fwd": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _P, _P, _P]),
     "odt_pfpnet_loss_grad": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _P, _P, _P, _P]),
+    "odt_peak_topk_scratch_bytes": (_L, [C.POINTER(TailParams), _I]),
+    "odt_peak_topk": (_I, [_P, C.POINTER(TailParams), _I, _P, _P, _I, _P, _P]),
+    "odt_centernet_loss_scratch_bytes": (_L, [C.POINTER(TailParams), _I]),
+    "odt_centernet_loss_fwd": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _P, _P, _P]),
+    "odt_centernet_loss_grad": (_I, [_P, C.POINTER(TailParams), _I, _P, _I, _P, _P, _P, _P]),
     "odt_augment_scratch_bytes": (_L, [C.POINTER(AugmentParams), _I]),
     "odt_augment_batch": (_I, [_P, C.POINTER(AugmentParams), _I, _P, _P, _P, _P]),
     "odt_pool_classify": (_I, [_P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P]),

@@ -1,4 +1,4 @@
-"""Layer graphs of SSD300 / SSD512 / RetinaNet / YOLOv3 / YOLOv2 / FCOS / PFPNet-R expressed on the
+"""Layer graphs of SSD300 / SSD512 / RetinaNet / YOLOv3 / YOLOv2 / FCOS / PFPNet-R / CenterNet expressed on the
 H100 engine (engine.Net).  Each builder mirrors the reference's layer creation
 order so variables get the same TF1 names as in the reference checkpoints
 (SURVEY.md App. D); citations give the reference lines each block stands for.
@@ -7,7 +7,7 @@ order so variables get the same TF1 names as in the reference checkpoints
 import numpy as np
 
 from . import lib as L
-from .engine import ClassifyTail, Net, Tail
+from .engine import ClassifyTail, Net, PeakTail, Tail
 
 F32 = np.float32
 
@@ -587,3 +587,114 @@ def pfpnet_tail(cfg):
 
     return Tail(L.DECODE_TWO_STEP, nc - 1, nc - 1, cfg["nms_score_threshold"], cfg["nms_iou_threshold"],
                 cfg["nms_max_boxes"], level_fn)
+
+
+# ------------------------------------------------------------- CenterNet ----
+CENTERNET_MEAN = (0.485, 0.456, 0.406)  # CenterNet.py:53-54, on images / 255
+CENTERNET_STD = (0.229, 0.224, 0.225)
+CENTERNET_STRIDE = 4                    # CenterNet.py:129
+MAX_TOP_K = 1024                        # the peak tail selects in one 1024-thread CTA per image
+
+
+def _positive_int(v):
+    return not isinstance(v, bool) and isinstance(v, (int, np.integer)) and v > 0
+
+
+def check_centernet_config(cfg):
+    """CenterNet's input size (a positive multiple of 32: four 2x2 SAME pools after the stride-2 stem, and the
+    upsampling sums of CenterNet.py:112-129 need equal sizes), class count (1..128, as YOLOv3 and FCOS) and
+    top_k_results_output (1..1024)."""
+    size = cfg["input_size"]
+    if not _positive_int(size) or size % 32:
+        raise ValueError("input_size = %r: CenterNet takes a positive multiple of 32" % (size,))
+    nc = cfg["num_classes"]
+    if not _positive_int(nc) or nc > MAX_SIGMOID_CLASSES:
+        raise ValueError("num_classes = %r: CenterNet supports 1 to %d classes" % (nc, MAX_SIGMOID_CLASSES))
+    k = cfg.get("top_k_results_output", 100)
+    if not _positive_int(k) or k > MAX_TOP_K:
+        raise ValueError("top_k_results_output = %r: CenterNet keeps 1 to %d detections" % (k, MAX_TOP_K))
+
+
+def build_centernet(batch, cfg, precision="fp16", device="cuda", allow_tc=True):
+    """ref CenterNet.py:50-135.  Every layer is conv (+ bias) -> BN (-> ReLU).  The input normalisation
+    (x / 255 - mean) / std is the stem's mean subtraction of 255 * mean and a per-channel scale folded into its kernel.
+    Sums run as convolution or pixel-shuffle residuals where one side is produced there, otherwise as DLA joins.
+    Candidate rows: [keypoint logits(C), dy, dx, h, w] per cell of the stride-4 grid."""
+    check_centernet_config(cfg)
+    size, nc = cfg["input_size"], cfg["num_classes"]
+    net = Net(batch, size, size, precision, device, allow_tc)
+    for i in range(3):
+        net.mean3[i] = 255.0 * CENTERNET_MEAN[i]
+    net.in_scale = [1.0 / (255.0 * s) for s in CENTERNET_STD]
+
+    def cba(x, cout, k, stride=1, act="relu", residual=None):  # _conv_bn_activation (:334-347)
+        return net.conv(x, cout, k, stride, bn=True, act=act, residual=residual)
+
+    def basic_block(x, f):
+        """conv-BN-ReLU twice + shortcut (:378-389).  tf.cond builds both branches, so the 1x1 shortcut's variables
+        exist even where the identity is taken; only the taken branch runs."""
+        y = cba(x, f, 3)
+        vs2 = net.namer.unique("conv2d")
+        net.var(vs2 + "/kernel", (3, 3, f, f), "he")
+        net.var(vs2 + "/bias", (f,), "zeros")
+        bn2 = net.bn_vars(f)
+        vs3 = net.namer.unique("conv2d")
+        net.var(vs3 + "/kernel", (1, 1, x.C, f), "he")
+        net.var(vs3 + "/bias", (f,), "zeros")
+        bn3 = net.bn_vars(f)
+        sc = x
+        if x.C != f:
+            sc = net.conv(x, f, 1, kernel_var=vs3 + "/kernel", bias_var=vs3 + "/bias", bn=True, bn_scope=bn3,
+                          act="relu")
+        return net.conv(y, f, 3, kernel_var=vs2 + "/kernel", bias_var=vs2 + "/bias", bn=True, bn_scope=bn2,
+                        act="relu", residual=sc)
+
+    def dla(x, f, levels, residual=None):
+        """_dla_generator (:390-401): conv3x3-BN-ReLU(block1 + block2) (+ residual: the caller's sum)."""
+        if levels == 1:
+            b1 = basic_block(x, f)
+            s = net.dla_join(b1, basic_block(b1, f), pooled=False)
+        else:
+            b1 = dla(x, f, levels - 1)
+            s = dla(b1, f, levels - 1, residual=b1)
+        return cba(s, f, 3, residual=residual)
+
+    def stage(x, f, levels):  # max_pool(dla(x)) + avg_pool(conv1x1(x)) (:95-111)
+        d = dla(x, f, levels)
+        return net.dla_join(d, cba(x, f, 1), pooled=True)
+
+    with net.scope("backone"):
+        x = cba(None, 16, 7)
+        x = cba(x, 16, 3)
+        x = cba(x, 32, 3, 2)
+        s3 = net.maxpool(dla(x, 64, 1), 2, 2)
+        s4 = stage(s3, 128, 2)
+        s5 = stage(s4, 256, 2)
+        s6 = stage(s5, 512, 1)
+    with net.scope("upsampling"):  # :112-129
+        p6_5 = net.deconv_phases(cba(s6, 256, 1), 256, "relu")
+        u6_5 = net.shuffle(p6_5)
+        p6_4 = net.deconv_phases(u6_5, 256, "relu")
+        u6_4 = net.shuffle(p6_4)
+        u6_3 = net.shuffle(net.deconv_phases(u6_4, 256, "relu"))
+        p5_4 = net.deconv_phases(cba(cba(s5, 256, 1, residual=u6_5), 256, 3), 256, "relu")  # conv(s5) + u6_5
+        u5_4 = net.shuffle(p5_4)
+        u5_3 = net.shuffle(net.deconv_phases(u5_4, 256, "relu"), residual=u6_3)
+        sum4 = net.shuffle(p5_4, residual=cba(s4, 256, 1, residual=u6_4))       # u5_4 + (conv(s4) + u6_4)
+        p4_3 = net.deconv_phases(cba(sum4, 256, 3), 256, "relu")
+        feats = cba(cba(net.shuffle(p4_3, residual=u5_3), 256, 3), 256, 1)    # u4_3 + (u5_3 + u6_3)
+    H = size // CENTERNET_STRIDE
+    assert (feats.H, feats.W) == (H, H)
+    net.add_level(H, H, 1)
+    row = nc + 4
+    with net.scope("center_detector"):  # :131-135: conv + bias -> BN, no activation
+        net.conv(feats, nc, 3, bn=True, head=(0, 0, nc, row, 1))
+        net.conv(feats, 2, 3, bn=True, head=(0, nc, 2, row, 1))
+        net.conv(feats, 2, 3, bn=True, head=(0, nc + 2, 2, row, 1))
+    return net, centernet_tail(cfg)
+
+
+def centernet_tail(cfg):
+    """Peak + top-k tail (CenterNet.py:159-185)."""
+    return PeakTail(cfg["num_classes"], float(cfg.get("score_threshold", 0.1)), int(cfg.get("top_k_results_output",
+                                                                                             100)))

@@ -26,6 +26,7 @@ from . import nets
 
 BN_EPS = 1e-3
 BN_MOMENTUM = 0.99
+ADAM_BETA1, ADAM_BETA2, ADAM_EPS = 0.9, 0.999, 1e-8  # tf.train.AdamOptimizer defaults
 
 
 def _same_pad(size, k, stride, dil=1):
@@ -258,7 +259,7 @@ class GraphTrainer:
         from . import engine as E
         self.model, self.cfg, self.E = model, model.config, E
         self.kind = {"SSD300": "ssd", "SSD512": "ssd", "RetinaNet": "retina", "YOLOv3": "yolo", "YOLOv2": "yolo2",
-                     "FCOS": "fcos", "PFPNetR": "pfpnet"}[model.name]
+                     "FCOS": "fcos", "PFPNetR": "pfpnet", "CenterNet": "centernet"}[model.name]
         if getattr(model, "is_pretraining", False):
             self.kind = "classify"                # RetinaNet's ImageNet-pretraining mode
         self.weight_decay = float(model.weight_decay)
@@ -278,10 +279,18 @@ class GraphTrainer:
                 self.slots[name] = torch.zeros_like(t)
         self.global_step = int(getattr(model, "global_step", 0))
         self._anchor_cache = None
+        # CenterNet trains with tf.train.AdamOptimizer (CenterNet.py:154): its slots `<var>/Adam` (m) and `<var>/Adam_1`
+        # (v) and the non-slot accumulators beta1_power / beta2_power, which start at beta1 / beta2
+        self.adam = self.kind == "centernet"
+        if self.adam:
+            self.slots = {k + "/Adam": torch.zeros_like(v) for k, v in self.params.items()}
+            self.slots.update({k + "/Adam_1": torch.zeros_like(v) for k, v in self.params.items()})
+            self.beta1_power, self.beta2_power = ADAM_BETA1, ADAM_BETA2
         # CUDA, fp32 rows: the data term is the family's loss-gradient kernel (csrc/loss.cu) behind one autograd
         # Function; the CPU (and float64) keep the restatement below, which the kernels are tested against
         self._loss_kernels = None
-        if self.kind in ("ssd", "retina", "yolo", "yolo2", "fcos", "pfpnet") and self.device.type == "cuda" and dtype == torch.float32:
+        if self.kind in ("ssd", "retina", "yolo", "yolo2", "fcos", "pfpnet", "centernet") and self.device.type == "cuda" \
+                and dtype == torch.float32:
             self._loss_kernels = LossKernels(self)
         if self.kind == "ssd":
             self._ssd = SSDTrainer.__new__(SSDTrainer)   # borrows the SSD loss / anchors
@@ -317,8 +326,14 @@ class GraphTrainer:
         E, P = self.E, self.params
         stats = [] if stats is None else stats
         x0 = torch.as_tensor(images, device=self.device, dtype=self.dtype)
-        mean = torch.tensor([123.68, 116.779, 103.979], device=self.device, dtype=self.dtype)
-        x0 = (x0 - mean).permute(0, 3, 1, 2)
+        if self.kind == "centernet":               # (x / 255 - mean) / std, CenterNet.py:53-67
+            from . import nets as NN
+            mean = torch.tensor(NN.CENTERNET_MEAN, device=self.device, dtype=self.dtype)
+            std = torch.tensor(NN.CENTERNET_STD, device=self.device, dtype=self.dtype)
+            x0 = ((x0 / 255.0 - mean) / std).permute(0, 3, 1, 2)
+        else:
+            mean = torch.tensor([123.68, 116.779, 103.979], device=self.device, dtype=self.dtype)
+            x0 = (x0 - mean).permute(0, 3, 1, 2)
         B = x0.shape[0]
         N = sum(h * w * a for h, w, a in self.net.levels)
         rows = torch.zeros((B, N * (self.row or 0)), device=self.device, dtype=self.dtype)
@@ -327,7 +342,7 @@ class GraphTrainer:
             if isinstance(op, E.PhaseConvOp):          # tf.layers.conv2d_transpose(4, 2, 'same') + BN
                 k = P[op.kernel].permute(3, 2, 0, 1)   # [4, 4, out, in] -> [in, out, 4, 4]
                 y = F.conv_transpose2d(val[id(op.x)], k, P[op.bias], stride=2, padding=1)
-                val[id(op.y)] = self._bn(y, op.bn, training, stats)
+                val[id(op.y)] = _act(self._bn(y, op.bn, training, stats), op.act)
             elif isinstance(op, E.ConvOp):
                 if op.is_image:
                     x = x0
@@ -382,6 +397,12 @@ class GraphTrainer:
                     val[id(op.out2)] = y
             elif isinstance(op, E.AvgPoolOp):          # 2x2/2 SAME: partial windows divided by their cells inside
                 val[id(op.y)] = F.avg_pool2d(val[id(op.x)], 2, 2, ceil_mode=True, count_include_pad=False)
+            elif isinstance(op, E.DlaJoinOp):          # a + b, or max_pool(a) + avg_pool(b), 2x2/2 SAME
+                a, b = val[id(op.a)], val[id(op.b)]
+                if op.pooled:
+                    a = max_pool_same(a, 2, 2)
+                    b = F.avg_pool2d(b, 2, 2, ceil_mode=True, count_include_pad=False)
+                val[id(op.y)] = a + b
             else:
                 raise TypeError(type(op))
         return val, rows
@@ -673,11 +694,47 @@ class GraphTrainer:
         odm = odm + mean0(sl1(ot[pos_idx, :2] - oyx).sum(-1) + sl1(ot[pos_idx, 2:] - ohw).sum(-1))
         return arm + odm
 
+    def centernet_image_loss(self, row, gt):
+        """CenterNet.py:187-270 for one image: row [H*W, C + 4] = [keypoint logits, dy, dx, h, w].  GT / 4, centres
+        floored to their cells (clamped into the grid); one sigma, the least CornerNet radius over every GT; the per-class
+        maximum of exp(-d^2 / 2 sigma^2) around the unfloored centres; focal terms summed / G; L1 means over G x 2 of the
+        offsets and sizes at the centre cells; kp + 0.1 size + offset.  No GT: 0 (the reference's 0 / 0 is NaN)."""
+        (h, w, _), = self.net.levels
+        nc = self.row - 4
+        gt = torch.as_tensor(gt, device=self.device, dtype=self.dtype)
+        cnt = int(torch.argmin(gt[:, 0]).item())
+        if cnt == 0:
+            return row.sum() * 0.0
+        g = gt[:cnt] / torch.tensor([4.0, 4.0, 4.0, 4.0, 1.0], device=self.device, dtype=self.dtype)
+        with torch.no_grad():
+            gy, gx, gh, gw, cid = g[:, 0], g[:, 1], g[:, 2], g[:, 3], g[:, 4].long()
+            cell = (torch.floor(gy).long().clamp(0, h - 1) * w + torch.floor(gx).long().clamp(0, w - 1))
+            sigma = torch.stack(centernet_radii(gh, gw)).min()
+            yy = torch.arange(h, device=self.device, dtype=self.dtype).view(1, h, 1)
+            xx = torch.arange(w, device=self.device, dtype=self.dtype).view(1, 1, w)
+            heat = torch.exp(-((gy.view(-1, 1, 1) - yy) ** 2 + (gx.view(-1, 1, 1) - xx) ** 2)
+                             / (2.0 * sigma * sigma)).view(cnt, h * w)
+            red = torch.zeros((h * w, nc), device=self.device, dtype=self.dtype)
+            pos = torch.zeros((h * w, nc), device=self.device, dtype=self.dtype)
+            for c in torch.unique(cid).tolist():
+                if 0 <= c < nc:
+                    red[:, c] = heat[cid == c].max(dim=0).values
+                    pos[cell[cid == c], c] = 1.0
+            toff = torch.stack([gy - torch.floor(gy), gx - torch.floor(gx)], dim=1)
+            tsize = torch.stack([gh, gw], dim=1)
+        k = row[:, :nc]
+        ls, p = F.logsigmoid(k), torch.sigmoid(k)
+        kp = (-(1.0 - p) ** 2 * ls * pos).sum() / cnt \
+            + (-(1.0 - red) ** 4 * p ** 2 * (-k + ls) * (1.0 - pos)).sum() / cnt
+        at = row[cell]
+        return kp + 0.1 * (tsize - at[:, nc + 2:nc + 4]).abs().mean() + (toff - at[:, nc:nc + 2]).abs().mean()
+
     def image_loss(self, row, gt):
         if self.kind == "ssd":
             return self._ssd.image_loss(row, gt)[0]
         return {"retina": self.retina_image_loss, "fcos": self.fcos_image_loss, "yolo": self.yolo_image_loss,
-                "yolo2": self.yolo2_image_loss, "pfpnet": self.pfpnet_image_loss}[self.kind](row, gt)
+                "yolo2": self.yolo2_image_loss, "pfpnet": self.pfpnet_image_loss,
+                "centernet": self.centernet_image_loss}[self.kind](row, gt)
 
     def total_loss(self, rows, ground_truth):
         if self._loss_kernels is not None:
@@ -715,8 +772,10 @@ class GraphTrainer:
         names = list(self.params)
         grads = torch.autograd.grad(loss, [self.params[k] for k in names], allow_unused=True)
         with torch.no_grad():
+            if self.adam:
+                self._adam(names, grads, lr)
             for name, gr in zip(names, grads):
-                if gr is None:
+                if gr is None or self.adam:
                     continue
                 acc = self.slots[name]
                 acc.mul_(0.9).add_(gr)
@@ -729,7 +788,32 @@ class GraphTrainer:
             return float(loss.detach()), accuracy
         return float(loss.detach())
 
+    def _adam(self, names, grads, lr):
+        """tf.train.AdamOptimizer(lr).minimize: lr_t = lr * sqrt(1 - beta2_power) / (1 - beta1_power); m = b1 m + (1 - b1) g;
+        v = b2 v + (1 - b2) g^2; var -= lr_t m / (sqrt(v) + eps); then beta1_power *= b1, beta2_power *= b2."""
+        lr_t = float(lr) * (1.0 - self.beta2_power) ** 0.5 / (1.0 - self.beta1_power)
+        for name, gr in zip(names, grads):
+            if gr is None:
+                continue
+            m, v = self.slots[name + "/Adam"], self.slots[name + "/Adam_1"]
+            m.mul_(ADAM_BETA1).add_(gr, alpha=1.0 - ADAM_BETA1)
+            v.mul_(ADAM_BETA2).addcmul_(gr, gr, value=1.0 - ADAM_BETA2)
+            self.params[name].sub_(lr_t * m / (v.sqrt() + ADAM_EPS))
+        self.beta1_power *= ADAM_BETA1
+        self.beta2_power *= ADAM_BETA2
+
     export = SSDTrainer.export
+
+
+def centernet_radii(h, w, min_overlap=0.7):
+    """CornerNet's three radii as CenterNet.py:254-270 writes them: (b + sqrt(b^2 - 4ac)) / 2 for each quadratic."""
+    b1, c1 = h + w, w * h * (1.0 - min_overlap) / (1.0 + min_overlap)
+    r1 = (b1 + torch.sqrt(b1 ** 2 - 4.0 * c1)) / 2.0
+    b2, c2 = 2.0 * (h + w), (1.0 - min_overlap) * w * h
+    r2 = (b2 + torch.sqrt(b2 ** 2 - 16.0 * c2)) / 2.0
+    a3, b3, c3 = 4.0 * min_overlap, -2.0 * min_overlap * (h + w), (min_overlap - 1.0) * w * h
+    r3 = (b3 + torch.sqrt(b3 ** 2 - 4.0 * a3 * c3)) / 2.0
+    return r1, r2, r3
 
 
 class _RowsLoss(torch.autograd.Function):
